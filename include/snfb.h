@@ -1,5 +1,5 @@
 /*
- * snfb.h — C ABI of libsnfb200.so: the B200-native lead -> cluster -> consensus hot path
+ * snfb.h — C ABI of libsnfb200.so: the H100-native lead -> cluster -> consensus hot path
  * of Sniffles2, callable through ctypes from the Python host (sniffles_b200/binding.py).
  *
  * Every entry point replaces a Python call site of the reference (paths relative to

@@ -11,7 +11,7 @@ blk = synth.config_block(cfgi, scale)
 ctx = binding.Context(0); ctx.set_config(abi.Config.from_sniffles(sconfig.default_config())); ctx.load(blk)
 for _ in range(3): res = ctx.run(want_leads=False)
 print({n: round(ms, 3) for n, ms, _ in ctx.timings()})
-nw = 148 * 7 * 4
+nw = 132 * 7 * 4          # k_align grid (NUM_SMS * 7) x ALIGN_WARPS
 out = np.zeros(nw * 8, "<u8")
 rc = binding.lib().snfb_debug_dump(ctx._h, out.ctypes.data, len(out)); print("rc", rc)
 d = out.reshape(nw, 8)

@@ -134,7 +134,7 @@ _OPTIONS = [
     (("--combine-support-threshold",), dict(type=int, default=3)),
     (("--combine-consensus",), dict(action="store_true", default=False)),
     (("--dev-combine-medians",), dict(action="store_true", default=False)),
-    (("--gpus",), dict(type=int, default=1)),          # new: number of B200s to shard contigs over
+    (("--gpus",), dict(type=int, default=1)),          # new: number of GPUs to shard contigs over
 ]
 
 

@@ -140,7 +140,7 @@ static void mark(snfb_ctx* ctx, const char* name, uint64_t bytes = 0) {
     ctx->ev_name[ctx->n_ev] = name; ctx->ev_bytes[ctx->n_ev] = bytes; ++ctx->n_ev;
 }
 #define LAUNCHED(ctx, k) ((ctx)->launches += (k))
-static int grid_for(unsigned long long n, int threads) { unsigned long long g = (n + threads - 1) / threads; if (g < 1) g = 1; if (g > 148ull * 32) g = 148ull * 32; return (int)g; }
+static int grid_for(unsigned long long n, int threads) { unsigned long long g = (n + threads - 1) / threads; if (g < 1) g = 1; if (g > (uint64_t)NUM_SMS * 32) g = (uint64_t)NUM_SMS * 32; return (int)g; }
 static int bits_for(uint32_t n) { int b = 0; while ((1ull << b) < n) ++b; return b; }
 
 __global__ void k_gather_leads(const snfb_lead* __restrict__ leads, const uint32_t* __restrict__ sval, snfb_lead* __restrict__ out, const unsigned long long* n_ptr, unsigned long long cap) {
@@ -226,7 +226,7 @@ template <int NL> static void launch_inflate_nl(snfb_ctx* ctx, const ingest::Bgz
     if (!attr) { cudaFuncSetAttribute(ingest::k_inflate<NL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
     const unsigned per_block = ingest::INF_WARPS * (32 / NL);
     const unsigned resident = (unsigned)std::max<size_t>(1, std::min<size_t>(8, (220 * 1024) / (smem + 1024)));
-    const unsigned grid = std::min<unsigned>((nb + per_block - 1) / per_block, 148u * resident);
+    const unsigned grid = std::min<unsigned>((nb + per_block - 1) / per_block, (unsigned)NUM_SMS * resident);
     ingest::k_inflate<NL><<<grid, ingest::INF_WARPS * 32, smem, ctx->st>>>(ctx->b_comp.as<uint8_t>(), d_blk, nb, ctx->b_raw.as<uint8_t>(), d_ctr);
 }
 static void launch_inflate(snfb_ctx* ctx, const ingest::BgzfBlock* d_blk, unsigned nb, ingest::IngestCounters* d_ctr) {
@@ -583,7 +583,7 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
     const uint32_t evt = evt_need(ctx);
     uint64_t n_rec = 0, n_groups = 0, n_var16 = 0, n_seq16 = 0;
     if (n_raw) {
-        const unsigned warp_grid = (unsigned)std::min<uint64_t>((n_raw + 7) / 8, 148ull * 16);
+        const unsigned warp_grid = (unsigned)std::min<uint64_t>((n_raw + 7) / 8, (uint64_t)NUM_SMS * 16);
         ingest::k_walk<<<(unsigned)((ns + 127) / 128), 128, 0, st>>>(raw, raw_len, d_span, (unsigned)ns, 1, span_cnt, span_base, recs, n_raw, d_ctr);
         mark(ctx, "parse_records", 0);
         ingest::k_parse<<<(unsigned)((n_raw + 127) / 128), 128, 0, st>>>(raw, recs, (unsigned)n_raw, ctx->b_task.as<snfb_task>(), d_ctr);
@@ -604,7 +604,7 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
     mark(ctx, "pack_records", sizeof(snfb_rec) * n_rec + 2 * n_words + 16 * n_var16 + 16 * n_seq16);
     CUDA_TRY(cudaMemsetAsync(ctx->b_cigar.as<uint16_t>() + 8 * n_groups, 0, 2 * 24, st));
     if (n_raw) {
-        const unsigned warp_grid = (unsigned)std::min<uint64_t>((n_raw + 7) / 8, 148ull * 16);
+        const unsigned warp_grid = (unsigned)std::min<uint64_t>((n_raw + 7) / 8, (uint64_t)NUM_SMS * 16);
         ingest::k_pack<<<warp_grid, 256, 0, st>>>(raw, recs, (unsigned)n_raw, evt, keep, idx, grp_off, groups, var_off, seq_off, ctx->b_rec.as<snfb_rec>(), ctx->b_cigar.as<uint16_t>(), ctx->b_var.as<uint8_t>(), ctx->b_seq.as<uint8_t>()); LAUNCHED(ctx, 1);
     }
     mark(ctx, nullptr);
@@ -672,7 +672,7 @@ static void carve_c(snfb_ctx* ctx, Carver& c) {
     cc.alt_off = c.take<uint32_t>(k.cand + 1); cc.scr_off = c.take<uint32_t>(k.cand + 1); cc.work_big = c.take<uint32_t>(k.cand + 1); cc.work_small = c.take<uint32_t>(k.cand + 1); cc.work_ctr = c.take<uint32_t>(64);
     cc.items_big = c.take<consensus::C::Item>(k.item + 1); cc.items_small = c.take<consensus::C::Item>(k.item + 1); cc.tiles = c.take<uint2>(k.tile + 1);
     cc.alt = c.take<uint8_t>(k.alt + 64); cc.scr = c.take<uint8_t>(k.scr16 * 16 + 64);
-    cc.dbg = getenv("SNFB_DEBUG") ? c.take<unsigned long long>(148 * 9 * consensus::ALIGN_WARPS * 8 + 8) : nullptr;
+    cc.dbg = getenv("SNFB_DEBUG") ? c.take<unsigned long long>(NUM_SMS * 9 * consensus::ALIGN_WARPS * 8 + 8) : nullptr;
     ctx->seq_req = c.take<consensus::SeqReq>(k.req + 1); ctx->seq_arena = c.take<uint8_t>(k.req16 * 16 + 64);
 }
 static int ensure_arenas(snfb_ctx* ctx) {
@@ -730,7 +730,7 @@ static int enqueue_stage_a(snfb_ctx* ctx) {
     if (evt_need(ctx) < ctx->evt_min) {
         // the block's E bits were set for longer events than this configuration looks at: lower the threshold in place
         if (ctx->on_device) return fail(ctx, "the device-resident CIGAR16 arena was packed with a larger event length than the configuration needs: repack with snfb_pack_cigar16(evt_min)");
-        extract::k_reflag<<<148 * 8, 256, 0, st>>>(const_cast<uint16_t*>(ctx->d_cigar), ctx->n_cigar, evt_need(ctx)); LAUNCHED(ctx, 1);
+        extract::k_reflag<<<NUM_SMS * 8, 256, 0, st>>>(const_cast<uint16_t*>(ctx->d_cigar), ctx->n_cigar, evt_need(ctx)); LAUNCHED(ctx, 1);
         ctx->evt_min = evt_need(ctx);
     }
     mark(ctx, "k_rec_index");
@@ -747,10 +747,10 @@ static int enqueue_stage_a(snfb_ctx* ctx) {
         extract::k_cdesc<<<(unsigned)((nrec + 255) / 256), 256, 0, st>>>(S); LAUNCHED(ctx, 2);
         // algorithmic bytes of the streaming kernel: chunk descriptors + CIGAR16 words + its per-chunk sums (bench.py adds the last two from the counters)
         mark(ctx, "k_scan", 2 * ctx->n_cigar);
-        extract::k_chunk_sum<<<148 * 8, 256, 0, st>>>(S);
+        extract::k_chunk_sum<<<NUM_SMS * 8, 256, 0, st>>>(S);
         mark(ctx, "k_scan_rare");
         extract::k_rec_base<<<(unsigned)((nrec + 255) / 256), 256, 0, st>>>(S);
-        extract::k_chunk_rare<<<148 * 8, 128, 0, st>>>(S);
+        extract::k_chunk_rare<<<NUM_SMS * 8, 128, 0, st>>>(S);
         extract::k_rec_fin<<<(unsigned)((nrec + 255) / 256), 256, 0, st>>>(S); LAUNCHED(ctx, 4);
         mark(ctx, "k_rec_post");
         extract::PostParams Q{};
@@ -761,7 +761,7 @@ static int enqueue_stage_a(snfb_ctx* ctx) {
         extract::EmitParams E{};
         E.rec = ctx->d_rec; E.clip = ctx->clip; E.var = ctx->d_var; E.ev = S.ev; E.n_ev = S.n_ev; E.ev_cap = ctx->cap.lead; E.fcnt = ctx->fcnt;
         E.leads = ctx->leads; E.ctr = ctr; E.maxlen = cf.dev_seq_cache_maxlen; E.detect_large_ins = cf.detect_large_ins; E.longinslen = (double)cf.long_ins_length / 2.0;
-        extract::k_emit<<<148 * 16, 128, 0, st>>>(E);
+        extract::k_emit<<<NUM_SMS * 16, 128, 0, st>>>(E);
         mark(ctx, "k_sa");
         extract::SaParams A{};
         A.rec = ctx->d_rec; A.clip = ctx->clip; A.var = ctx->d_var; A.task = b.task; A.contig = b.contig; A.n_contig = ctx->n_contig;
@@ -811,19 +811,19 @@ static int enqueue_stage_b(snfb_ctx* ctx) {
     mark(ctx, "cluster_call");
     // clusters too large for one warp's shared memory go to a block each, next to the warp-per-cluster kernel
     CUDA_TRY(cudaEventRecord(ctx->ev_fork, st)); CUDA_TRY(cudaStreamWaitEvent(ctx->st_side, ctx->ev_fork, 0));
-    cluster::k_cluster_block<<<148, cluster::CB_THREADS, cluster::CB_SMEM, ctx->st_side>>>(b);
-    cluster::k_cluster_warp<cluster::WARP_CAP, cluster::CWM_WARPS, true><<<148 * 2, cluster::CWM_WARPS * 32, cluster::CwCfg<cluster::WARP_CAP, cluster::CWM_WARPS>::smem, ctx->st_side>>>(b);
+    cluster::k_cluster_block<<<NUM_SMS, cluster::CB_THREADS, cluster::CB_SMEM, ctx->st_side>>>(b);
+    cluster::k_cluster_warp<cluster::WARP_CAP, cluster::CWM_WARPS, true><<<NUM_SMS * 2, cluster::CWM_WARPS * 32, cluster::CwCfg<cluster::WARP_CAP, cluster::CWM_WARPS>::smem, ctx->st_side>>>(b);
     CUDA_TRY(cudaEventRecord(ctx->ev_join, ctx->st_side));
-    cluster::k_cluster_warp<cluster::SMALL_CAP, cluster::CWS_WARPS, false><<<148 * 4, cluster::CWS_WARPS * 32, cluster::CwCfg<cluster::SMALL_CAP, cluster::CWS_WARPS>::smem, st>>>(b);
+    cluster::k_cluster_warp<cluster::SMALL_CAP, cluster::CWS_WARPS, false><<<NUM_SMS * 4, cluster::CWS_WARPS * 32, cluster::CwCfg<cluster::SMALL_CAP, cluster::CWS_WARPS>::smem, st>>>(b);
     CUDA_TRY(cudaStreamWaitEvent(st, ctx->ev_join, 0));
     mark(ctx, "emit_cands");
     LAUNCHED(ctx, prims::exclusive_scan(b.cl_nvalid, b.cl_cand_base, b.scan_tmp, &ctr->n_clusters, nb, &ctr->n_cand, st));
     LAUNCHED(ctx, prims::exclusive_scan(b.cl_nlead, b.cl_lead_base, b.scan_tmp, &ctr->n_clusters, nb, &ctr->n_cand_leads, st));
     LAUNCHED(ctx, prims::exclusive_scan(b.cl_nrn, b.cl_rn_base, b.scan_tmp, &ctr->n_clusters, nb, &ctr->n_rnames, st));
-    cluster::k_emit_cands<<<148 * 8, 128, 0, st>>>(b);
+    cluster::k_emit_cands<<<NUM_SMS * 8, 128, 0, st>>>(b);
     mark(ctx, "coverage");
     if (ctx->n_mask) { cluster::k_mask_bp<<<grid_for((unsigned long long)ctx->n_mask * 32, 128), 128, 0, st>>>(b, ctx->b_mask_task.as<uint32_t>(), ctx->n_mask, ctx->task_cov); LAUNCHED(ctx, 1); }
-    cluster::k_coverage<<<148 * 32, 128, 0, st>>>(b); LAUNCHED(ctx, 13);
+    cluster::k_coverage<<<NUM_SMS * 32, 128, 0, st>>>(b); LAUNCHED(ctx, 13);
     // consensus plan: best read per INS candidate, sizes and offsets of the ALT bytes and of the scratch; the candidate records are final after this
     consensus::C& c = ctx->Cc;
     CUDA_TRY(cudaMemsetAsync(c.work_ctr, 0, 64, st));
@@ -868,11 +868,11 @@ static int enqueue_stage_c(snfb_ctx* ctx) {
         c.seq = ctx->seq_arena; c.arena_off = ctx->arena_off;
     }
     mark(ctx, "consensus");
-    consensus::k_prep<<<148 * 8, 128, 0, st>>>(c);
+    consensus::k_prep<<<NUM_SMS * 8, 128, 0, st>>>(c);
     mark(ctx, "consensus_align");
-    consensus::k_align<<<148 * 7, consensus::ALIGN_WARPS * 32, 0, st>>>(c);
+    consensus::k_align<<<NUM_SMS * 7, consensus::ALIGN_WARPS * 32, 0, st>>>(c);
     mark(ctx, "consensus_vote");
-    consensus::k_vote<<<148 * 16, consensus::VOTE_THREADS, 0, st>>>(c); LAUNCHED(ctx, 3);
+    consensus::k_vote<<<NUM_SMS * 16, consensus::VOTE_THREADS, 0, st>>>(c); LAUNCHED(ctx, 3);
     mark(ctx, nullptr);
     CUDA_TRY(cudaGetLastError());
     return 0;
@@ -1070,7 +1070,7 @@ uint64_t snfb_rerun_count(snfb_ctx* ctx) { return ctx ? ctx->reruns : 0; }
 /* developer aid (SNFB_DEBUG set when the ctx ran): per-warp timing of the consensus alignment kernel, 8 words per warp */
 int snfb_debug_dump(snfb_ctx* ctx, uint64_t* out, uint64_t n_words) {
     if (!ctx || !ctx->Cc.dbg || !out) return 1;
-    const uint64_t have = 148ull * 8 * consensus::ALIGN_WARPS * 8; if (n_words > have) n_words = have;
+    const uint64_t have = (uint64_t)NUM_SMS * 8 * consensus::ALIGN_WARPS * 8; if (n_words > have) n_words = have;
     return cudaMemcpy(out, ctx->Cc.dbg, 8 * n_words, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : 1;
 }
 int snfb_pin_host(void* p, size_t bytes) { return cudaHostRegister(p, bytes, cudaHostRegisterDefault) == cudaSuccess ? 0 : 1; }
@@ -1122,9 +1122,9 @@ int snfb_allgather_candidates(snfb_ctx* ctx, uint32_t flags, snfb_gather_view* o
         if (ctx->b_gsend.ensure(cap + 256) || ctx->b_grecv.ensure((size_t)nr * cap + out_cap + 1024)) return fail(ctx, "out of device memory (gather)");
         uint8_t* recv = ctx->b_grecv.as<uint8_t>(); uint8_t* merged = recv + (((size_t)nr * cap + 255) & ~(size_t)255); unsigned long long* d_layout = reinterpret_cast<unsigned long long*>(merged + out_cap);     // layout words live behind the merged arrays
         mark(ctx, "allgather");
-        k_gather_pack<<<148 * 4, 256, 0, st>>>(b.ctr, b.cand, ctx->Cc.alt, b.rnames, b.rn_off_out, b.cand_leads, with_leads, nr > 1 ? ctx->b_gsend.as<uint8_t>() : recv, cap); LAUNCHED(ctx, 1);
+        k_gather_pack<<<NUM_SMS * 4, 256, 0, st>>>(b.ctr, b.cand, ctx->Cc.alt, b.rnames, b.rn_off_out, b.cand_leads, with_leads, nr > 1 ? ctx->b_gsend.as<uint8_t>() : recv, cap); LAUNCHED(ctx, 1);
         if (nr > 1 && g_nccl.AllGather(ctx->b_gsend.p, recv, cap, 0 /* ncclChar */, ctx->comm, st) != 0) return fail(ctx, "ncclAllGather failed");
-        k_gather_merge<<<148 * 4, 256, 0, st>>>(recv, cap, nr, with_leads, merged, out_cap, d_layout); LAUNCHED(ctx, 1);
+        k_gather_merge<<<NUM_SMS * 4, 256, 0, st>>>(recv, cap, nr, with_leads, merged, out_cap, d_layout); LAUNCHED(ctx, 1);
         mark(ctx, nullptr);
         CUDA_TRY(cudaMemcpyAsync(h_layout, d_layout, 64, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(h_hdr, recv, sizeof(GatherHdr), cudaMemcpyDeviceToHost, st));     // slot 0's header; the rest below
@@ -1176,7 +1176,7 @@ int snfb_poa(snfb_ctx* ctx, const snfb_poa_job* jobs, uint32_t n_jobs, const uin
         smax = std::max(smax, poa::scratch_bytes(total, maxl, bw));
     }
     size_t free_b = 0, total_b = 0; cudaMemGetInfo(&free_b, &total_b);
-    size_t nblk = std::min<size_t>(n_jobs, 148 * 2);
+    size_t nblk = std::min<size_t>(n_jobs, NUM_SMS * 2);
     while (nblk > 1 && nblk * smax > free_b / 3) --nblk;
     if (smax > free_b / 2) return fail(ctx, "snfb_poa: a job needs more scratch than the device has free");
     DevBuf d_jobs, d_seqs, d_offs, d_out, d_len, d_scr, d_ctr;
@@ -1222,7 +1222,7 @@ int snfb_combine_groups(snfb_ctx* ctx, const snfb_combine_in* in, snfb_combine_o
     uint32_t max_alt = 16;
     if (use_alt) for (uint32_t i = 0; i < in->n_cand; ++i) { if (in->alt_off[i] + in->alt_len[i] > in->n_alt_bytes) return fail(ctx, "snfb_combine_groups: ALT outside alt[]"); max_alt = std::max(max_alt, in->alt_len[i]); }
     max_alt = (max_alt + 15u) & ~15u;
-    const unsigned blocks = (unsigned)std::min<size_t>((in->n_chain + 3) / 4, 148 * 4);
+    const unsigned blocks = (unsigned)std::min<size_t>((in->n_chain + 3) / 4, NUM_SMS * 4);
     DevBuf b_in, b_state, b_out;
     // inputs in one buffer, group state in one, outputs in one
     Carver ci, cs, co;
@@ -1268,7 +1268,7 @@ int snfb_selftest_edit_distance(snfb_ctx* ctx, const uint8_t* bytes, uint64_t n_
     for (uint32_t i = 0; i < n_pairs; ++i) { if (a_off[i] + a_len[i] > n_bytes || b_off[i] + b_len[i] > n_bytes) return fail(ctx, "snfb_selftest_edit_distance: string outside bytes[]"); max_len = std::max(max_len, std::max(a_len[i], b_len[i])); }
     max_len = (max_len + 15u) & ~15u;
     cudaSetDevice(ctx->device);
-    const unsigned blocks = (unsigned)std::min<uint32_t>((n_pairs + 3) / 4, 148 * 4);
+    const unsigned blocks = (unsigned)std::min<uint32_t>((n_pairs + 3) / 4, NUM_SMS * 4);
     DevBuf d_b, d_o, d_hs, d_out;
     auto done = [&](int r) { d_b.release(); d_o.release(); d_hs.release(); d_out.release(); return r; };
     if (d_b.ensure(n_bytes + 16) | d_o.ensure((size_t)n_pairs * 24 + 64) | d_hs.ensure((size_t)blocks * 4 * max_len + 16) | d_out.ensure((size_t)n_pairs * 4)) return done(fail(ctx, "snfb_selftest_edit_distance: out of device memory"));

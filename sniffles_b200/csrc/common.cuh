@@ -1,4 +1,4 @@
-// common.cuh — shared device helpers of libsnfb200 (sm_100a only).
+// common.cuh — shared device helpers of libsnfb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,6 +7,9 @@
 #include "../../include/snfb.h"
 
 #define FULL 0xffffffffu
+
+// SMs of the H100 SXM: persistent and grid-stride launches are sized in multiples of it
+constexpr int NUM_SMS = 132;
 
 #define CUDA_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { ctx_fail(ctx, #x, cudaGetErrorString(e_)); return 1; } } while (0)
 
@@ -35,6 +38,14 @@ struct DevCounters {
 
 // ---------------------------------------------------------------- small utilities
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
+// stores a struct whose size is a multiple of 16 bytes with 16-byte stores.  The bytes are taken with memcpy, not through a cast
+// pointer: a cast breaks strict aliasing, and the compiler may then read the vectors before the fields are written.
+template <class T> __device__ __forceinline__ void store16(void* dst, const T& v) {
+    static_assert(sizeof(T) % 16 == 0, "store16: size must be a multiple of 16 bytes");
+    uint4 t[sizeof(T) / 16]; memcpy(t, &v, sizeof(T));
+    #pragma unroll
+    for (int k = 0; k < (int)(sizeof(T) / 16); ++k) reinterpret_cast<uint4*>(dst)[k] = t[k];
+}
 __device__ __forceinline__ unsigned lanemask_lt() { unsigned m; asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m)); return m; }
 
 __device__ __forceinline__ uint64_t mix64(uint64_t z) {

@@ -32,8 +32,7 @@ __device__ __forceinline__ bool op_adds_ref(int op) { return (0x18Du >> op) & 1u
 __device__ __forceinline__ bool op_is_event(int op) { return (0x016u >> op) & 1u; }    // I D S      (1,2,4)
 
 __device__ __forceinline__ void store_lead(snfb_lead* dst, const snfb_lead& l) {
-    const uint4* s = reinterpret_cast<const uint4*>(&l); uint4* d = reinterpret_cast<uint4*>(dst);
-    d[0] = s[0]; d[1] = s[1]; d[2] = s[2]; d[3] = s[3];
+    store16(dst, l);
 }
 
 // ---- text helpers (lane-serial; SA tags are short in the compact form aligners write) ----
@@ -298,8 +297,8 @@ __global__ void __launch_bounds__(256) k_rec_index(const IndexParams P) {
     const int nm = (int)c1.x; const uint32_t n = c1.z; const int l_seq = (int)c1.w;
     const unsigned long long cigar_off = (unsigned long long)c2.z | ((unsigned long long)c2.w << 32);
     if ((uint32_t)task >= P.n_task || (cigar_off & 7) || cigar_off + n > P.n_cigar) {      // malformed record (counted by k_validate: the run fails); touch nothing through its offsets
-        RecScan s; s.cig8 = 0; s.n_words = 0; s.pos = pos; s.meta = 0; *reinterpret_cast<uint4*>(P.scan + i) = *reinterpret_cast<const uint4*>(&s);
-        RecClip c; c.alen = 0; c.qas = 0; c.clip_left = 0; c.clip_right = 0; *reinterpret_cast<int4*>(P.clip + i) = *reinterpret_cast<const int4*>(&c);
+        RecScan s; s.cig8 = 0; s.n_words = 0; s.pos = pos; s.meta = 0; store16(P.scan + i, s);
+        RecClip c; c.alen = 0; c.qas = 0; c.clip_left = 0; c.clip_right = 0; store16(P.clip + i, c);
         P.rec_pos[i] = pos; P.rec_flags[i] = 0; P.rec_nm[i] = -1.0; P.rec_end[i] = -1; P.rec_nlead[i] = 0; P.pass_chunks[i] = 0; return;
     }
     P.rec_pos[i] = pos;
@@ -337,9 +336,9 @@ __global__ void __launch_bounds__(256) k_rec_index(const IndexParams P) {
     if (pass && hp > 2) { hp = 0; atomicAdd(&P.ctr->soft_errors, 1ULL); }
     RecScan s; s.cig8 = (uint32_t)(cigar_off >> 3); s.n_words = n; s.pos = pos;
     s.meta = ((uint32_t)task & 0xffffu) | (mapq << 16) | (pass ? RM_PASS : 0u) | (has_nm ? RM_HAS_NM : 0u) | ((pass && (aux & SNFB_AUX_SA)) ? RM_HAS_SA : 0u) | ((pass ? hp : 0u) << 27);
-    *reinterpret_cast<uint4*>(P.scan + i) = *reinterpret_cast<const uint4*>(&s);
+    store16(P.scan + i, s);
     RecClip c; c.alen = alen; c.qas = qas; c.clip_left = clip_left; c.clip_right = clip_right;
-    *reinterpret_cast<int4*>(P.clip + i) = *reinterpret_cast<const int4*>(&c);
+    store16(P.clip + i, c);
     P.rec_flags[i] = pass ? (uint8_t)(RF_PASS | (has_nm ? RF_HAS_NM : 0) | (hp << 2)) : (uint8_t)0;
     P.rec_nm[i] = has_nm ? (double)nm : -1.0;        // k_rec_post turns it into (nm - big) / (alen + 1)
     P.rec_end[i] = -1; P.rec_nlead[i] = 0;
@@ -656,7 +655,7 @@ struct SaParams {
     Seg* seg_scratch;                 // MAXSEG segments per thread of the grid
     snfb_config cfg;
 };
-constexpr int SA_THREADS = 128, SA_BLOCKS = 148 * 8;
+constexpr int SA_THREADS = 128, SA_BLOCKS = NUM_SMS * 8;
 // one thread per record with an SA tag: the text parse is serial per record, so the parallelism is across records.
 // Segments live in a per-thread slice of global scratch (a read has a handful of them; the touched part stays in L2).
 __global__ void __launch_bounds__(SA_THREADS) k_sa(const SaParams P) {
