@@ -367,11 +367,17 @@ struct Event { uint32_t rec; uint32_t len; uint32_t pos_q; int32_t pos_r; uint32
 //     at once) and one OR (E / extension flags).  The loads of 8 groups (128 bytes) are issued before the first is used.
 //   - a segmented warp scan of the sums (a segment starts at the first chunk of a record; a record that continues from the previous
 //     round takes the carry) gives the absolute (query, reference) position at every chunk start.
-//   - chunks holding an E-flagged word are decoded by the whole warp, one chunk at a time in chunk order: lane g reloads group g (just
-//     read: L1 / L2), a scan over the groups gives their positions, lanes whose group holds an E word decode it, apply the region test
-//     (leadprov.py:464-466) and write one Event per SV signature with its final ordinal inside the record (a warp-uniform running count
-//     of the current record).  An extension word alone needs no decode: every I / D / S long enough to need one carries E, and so does
-//     every I / D above 10 bases whenever the NM correction is used (evt_need).
+//   - the round's chunks holding an E-flagged word are decoded together: their groups are laid out over the lanes in chunk order, one
+//     group per lane, in passes of 32 groups (a chunk may continue into the next pass).  A shuffle binary search finds each group's
+//     chunk; the lane reloads the group (just read: L1 / L2) and a scan segmented at chunk starts, seeded with the chunk's start position
+//     (or the previous pass's carry), gives the group's position.  Only lanes whose group holds an E word decode, and only its E words
+//     (group_events: the offset of a word is a masked sum of the words below it; a group with an extension word is decoded op by op),
+//     apply the region test (leadprov.py:464-466), count signatures and big indels.  One scan of the counts over the pass gives the
+//     event slots (one reservation per pass) and, segmented at record starts, each signature's final ordinal inside its record (a record
+//     that continues from an earlier pass or round starts from the warp-uniform running count); the lanes then decode again and write
+//     one Event per signature.  Each chunk's counts go back to the lane that owns it as the difference of the scans over its groups.
+//     An extension word alone needs no decode: every I / D / S long enough to need one carries E, and so does every I / D / S of 11
+//     bases or more (evt_need), which covers the big-indel sum.
 //   - the lane holding a record's last chunk writes its reference end, lead count and "big indel" sum (get_cigar_indels).
 // Event slots: a warp reserves WALK_SLOTS at a time and hands them out in order; what is left when it finishes is retired as holes.
 struct WalkParams {
@@ -425,6 +431,51 @@ __device__ __forceinline__ uint32_t seg_incl_sum(uint32_t v, int h, uint32_t ini
     const uint32_t s = prims::warp_incl_scan(v);
     const uint32_t eh = __shfl_sync(FULL, s - v, h < 0 ? 0 : h);          // lane 0's exclusive prefix is 0
     return init + s - eh;
+}
+
+// the SV signatures of one 16-byte group that holds an E word, in op order: emit(cls, len, q, r) for every I / D / S of at least minsv
+// whose signature lies inside [tk_start, tk_end) (leadprov.py:464-466); (q, r) = the op's read / reference position, the group starts at
+// (q0, r0).  Adds the group's I / D ops above 10 bases to `big` (get_cigar_indels).  Every I / D / S of 11 bases or more carries E and
+// minsv is at least the block's E threshold (evt_need), so the E words are all it has to look at:
+//   - without an extension word, word h is op h: only the E words are visited, the offset of each is the masked sum of the words below it;
+//   - with one, the group is decoded op by op (c16_op).
+template <class Emit>
+__device__ __forceinline__ void group_events(const uint4 v, uint32_t q0, int r0, int minsv, int tk_start, int tk_end, uint32_t& big, Emit&& emit) {
+    const uint32_t ww[4] = { v.x, v.y, v.z, v.w };
+    if ((v.x | v.y | v.z | v.w) & 0x80008000u) {
+        uint32_t q = q0; int r = r0;
+        #pragma unroll
+        for (int x = 0; x < 8; ++x) {
+            unsigned cls, len; c16_op(ww, x, cls, len);
+            if (len > 10u && (cls == C16_I || cls == C16_D)) big += len;
+            if (c16_is_event(cls) && (int)len >= minsv) {
+                const int rsig = cls == C16_D ? r + (int)len : r;
+                if (rsig >= tk_start && rsig < tk_end) emit(cls, len, q, r);
+            }
+            q += len * (cls & 1u); r += (int)(len * ((cls >> 1) & 1u));
+        }
+        return;
+    }
+    // E bit (word bit 14) of half h -> bit h
+    uint32_t em = ((v.x >> 14) & 1u) | ((v.x >> 29) & 2u) | ((v.y >> 12) & 4u) | ((v.y >> 27) & 8u)
+                | ((v.z >> 10) & 16u) | ((v.z >> 25) & 32u) | ((v.w >> 8) & 64u) | ((v.w >> 23) & 128u);
+    for (; em; em &= em - 1u) {
+        const uint32_t h = (uint32_t)__ffs(em) - 1u;
+        const uint32_t w = h < 4u ? (h < 2u ? v.x : v.y) : (h < 6u ? v.z : v.w);
+        const uint32_t x = (w >> (16u * (h & 1u))) & 0xffffu;
+        const unsigned cls = c16_class(x), len = x & C16_LEN_MASK;
+        if (len > 10u && (cls == C16_I || cls == C16_D)) big += len;
+        if (!(c16_is_event(cls) && (int)len >= minsv)) continue;
+        uint32_t aq = 0, ar = 0;                    // the words below h: whole 32-bit words, and the low half of h's own word when h is odd
+        #pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const uint32_t m = 2u * i + 2u <= h ? 0xffffffffu : (2u * i + 1u == h ? 0xffffu : 0u);
+            SNFB_WORD_BODY(ww[i] & m, aq, ar)
+        }
+        const uint32_t q = q0 + (aq & 0xffffu) + (aq >> 16); const int r = r0 + (int)((ar & 0xffffu) + (ar >> 16));
+        const int rsig = cls == C16_D ? r + (int)len : r;
+        if (rsig >= tk_start && rsig < tk_end) emit(cls, len, q, r);
+    }
 }
 
 template <int TILE>
@@ -483,40 +534,49 @@ __global__ void __launch_bounds__(WALK_THREADS, 4) k_cigar_walk(const __grid_con
             const unsigned hm = __ballot_sync(FULL, head) & (lanemask_lt() | (1u << lane));
             const int h = hm ? 31 - __clz(hm) : -1;
             const uint32_t pq = seg_incl_sum(vq, h, h < 0 ? carry.x : 0u) - vq, pr = seg_incl_sum(vr, h, h < 0 ? carry.y : rs[j].z) - vr;
-            // flagged chunks, one at a time in chunk order, by the whole warp
+            // the flagged chunks' groups, one per lane in chunk order, in passes of 32 (a chunk may continue into the next pass)
             uint32_t my_n = 0, my_big = 0;                   // events / big-indel sum of this lane's chunk
-            for (unsigned fl = __ballot_sync(FULL, flags != 0); fl; fl &= fl - 1u) {
-                const int src = __ffs(fl) - 1;
-                const uint32_t f_g0 = __shfl_sync(FULL, g0, src), f_q = __shfl_sync(FULL, pq, src), f_r = __shfl_sync(FULL, pr, src);
-                const int f_ng = __shfl_sync(FULL, ng, src);
-                const uint32_t f_rec = t0 + (uint32_t)__shfl_sync(FULL, j, src);
-                const snfb_task& tk = P.task[rs[__shfl_sync(FULL, j, src)].w & 0xffffu];
-                const int tk_start = tk.start, tk_end = tk.end;
-                const uint4 v = (int)lane < f_ng ? __ldg(cig4 + f_g0 + lane) : make_uint4(0u, 0u, 0u, 0u);
+            const uint32_t fng = flags ? (uint32_t)ng : 0u;
+            const uint32_t fin = prims::warp_incl_scan(fng), fex = fin - fng, ftot = __shfl_sync(FULL, fin, 31);
+            uint32_t cq = 0, cr = 0;                         // group position at the end of the previous pass (warp-uniform)
+            for (uint32_t p0 = 0; p0 < ftot; p0 += 32) {
+                const uint32_t x = p0 + lane;
+                const bool gv = x < ftot;
+                int o = 0;                                   // the owner: the last lane whose first group is <= x (lanes without a flagged chunk own none)
+                #pragma unroll
+                for (int s = 16; s; s >>= 1) { const uint32_t e = __shfl_sync(FULL, fex, o + s); if (e <= x) o += s; }
+                const uint32_t gi = x - __shfl_sync(FULL, fex, o), o_g0 = __shfl_sync(FULL, g0, o), o_pq = __shfl_sync(FULL, pq, o), o_pr = __shfl_sync(FULL, pr, o);
+                const int o_j = __shfl_sync(FULL, j, o);
+                const uint4 v = gv ? __ldg(cig4 + o_g0 + gi) : make_uint4(0u, 0u, 0u, 0u);     // just read by the owner: L1 / L2
                 const uint2 a = group_sums(v);
-                uint32_t q = f_q + prims::warp_incl_scan(a.x) - a.x; int r = (int)(f_r + prims::warp_incl_scan(a.y) - a.y);
-                const bool rb = ((v.x | v.y | v.z | v.w) & 0x40004000u) != 0;
-                const uint32_t ww[4] = { v.x, v.y, v.z, v.w };
-                uint32_t n = 0, big = 0;
-                if (rb) {                                    // count the group's signatures
-                    int r2 = r;
-                    #pragma unroll
-                    for (int x = 0; x < 8; ++x) {
-                        unsigned cls, len; c16_op(ww, x, cls, len);
-                        if (len > 10u && (cls == C16_I || cls == C16_D)) big += len;                // get_cigar_indels, minoplen 10
-                        if (c16_is_event(cls) && (int)len >= P.minsv) {
-                            const int rsig = cls == C16_D ? r2 + (int)len : r2;
-                            if (rsig >= tk_start && rsig < tk_end) ++n;                             // the signature stays inside the task's region
-                        }
-                        r2 += (int)(len * ((cls >> 1) & 1u));
-                    }
+                const unsigned gh = __ballot_sync(FULL, gv && gi == 0) & (lanemask_lt() | (1u << lane));
+                const int hg = gh ? 31 - __clz(gh) : -1;
+                const uint32_t q = seg_incl_sum(a.x, hg, hg < 0 ? cq : o_pq) - a.x, r = seg_incl_sum(a.y, hg, hg < 0 ? cr : o_pr) - a.y;
+                cq = __shfl_sync(FULL, q + a.x, 31); cr = __shfl_sync(FULL, r + a.y, 31);
+                const uint32_t f_rec = t0 + (uint32_t)o_j;
+                int tk_start = 0, tk_end = 0; uint32_t n = 0, big = 0;
+                if (gv && (((v.x | v.y | v.z | v.w) & 0x40004000u) != 0)) {      // count the group's signatures
+                    const snfb_task& tk = P.task[rs[o_j].w & 0xffffu];
+                    tk_start = tk.start; tk_end = tk.end;
+                    group_events(v, q, (int)r, P.minsv, tk_start, tk_end, big, [&](unsigned, unsigned, uint32_t, int) { ++n; });
                 }
-                const uint32_t n_incl = prims::warp_incl_scan(n), n_tot = __shfl_sync(FULL, n_incl, 31);
-                const uint32_t big_tot = __reduce_add_sync(FULL, big);
-                if (lane == (uint32_t)src) { my_n = n_tot; my_big = big_tot; }
+                const uint32_t n_incl = prims::warp_incl_scan(n), n_ex = n_incl - n, n_tot = __shfl_sync(FULL, n_incl, 31);
+                const uint32_t b_incl = prims::warp_incl_scan(big);
+                // this pass's share of each flagged chunk goes back to its owner lane: the scans' difference over the chunk's lanes
+                const uint32_t lo = fex > p0 ? fex - p0 : 0u, hi = fin - p0 < 32u ? fin - p0 : 32u;          // lanes [lo, hi) of this pass
+                const bool mine = fng && fin > p0 && fex < p0 + 32u;
+                const uint32_t hi_n = __shfl_sync(FULL, n_incl, (hi - 1u) & 31u), lo_n = __shfl_sync(FULL, n_ex, lo & 31u);
+                const uint32_t hi_b = __shfl_sync(FULL, b_incl, (hi - 1u) & 31u), lo_b = __shfl_sync(FULL, b_incl - big, lo & 31u);
+                if (mine) { my_n += hi_n - lo_n; my_big += hi_b - lo_b; }
                 if (n_tot) {
-                    const uint32_t base = f_rec == run_rec ? run_cnt : 0u;
-                    run_rec = f_rec; run_cnt = base + n_tot;
+                    // ordinals: a segmented count that starts at every record's first group of the pass; a record that continues
+                    // from an earlier pass or round starts from the running count
+                    const uint32_t prev_rec = __shfl_up_sync(FULL, f_rec, 1);
+                    const unsigned rh = __ballot_sync(FULL, gv && (lane == 0 ? f_rec != run_rec : f_rec != prev_rec)) & (lanemask_lt() | (1u << lane));
+                    const int hr = rh ? 31 - __clz(rh) : -1;
+                    const uint32_t ord = (hr < 0 ? run_cnt : 0u) + n_ex - __shfl_sync(FULL, n_ex, hr < 0 ? 0 : hr);
+                    const uint32_t lastv = ftot - p0 < 32u ? ftot - p0 - 1u : 31u;
+                    run_rec = __shfl_sync(FULL, f_rec, lastv); run_cnt = __shfl_sync(FULL, ord + n, lastv);
                     // the s_left reserved slots first, then a new reservation
                     const uint32_t avail = s_left;
                     unsigned long long nb = 0; uint32_t blk = 0;
@@ -526,22 +586,13 @@ __global__ void __launch_bounds__(WALK_THREADS, 4) k_cigar_walk(const __grid_con
                         nb = __shfl_sync(FULL, nb, 0);
                     }
                     if (n) {                                 // decode the group again and write its signatures
-                        uint32_t t = n_incl - n;
-                        int r2 = r;
-                        #pragma unroll
-                        for (int x = 0; x < 8; ++x) {
-                            unsigned cls, len; c16_op(ww, x, cls, len);
-                            if (c16_is_event(cls) && (int)len >= P.minsv) {
-                                const int rsig = cls == C16_D ? r2 + (int)len : r2;
-                                if (rsig >= tk_start && rsig < tk_end) {
-                                    const unsigned long long slot = t < avail ? s_cur + t : nb + (t - avail);
-                                    if (slot < P.ev_cap) { uint4* dst = reinterpret_cast<uint4*>(P.ev + slot); dst[0] = make_uint4(f_rec, len, q, (uint32_t)r2); dst[1] = make_uint4(((base + t) & 0xffffu) | (cls << 16), 0u, 0u, 0u); }
-                                    else ++overflow;
-                                    ++t;
-                                }
-                            }
-                            q += len * (cls & 1u); r2 += (int)(len * ((cls >> 1) & 1u));
-                        }
+                        uint32_t t = n_ex, k = ord, big_again = 0;
+                        group_events(v, q, (int)r, P.minsv, tk_start, tk_end, big_again, [&](unsigned cls, unsigned len, uint32_t eq, int er) {
+                            const unsigned long long slot = t < avail ? s_cur + t : nb + (t - avail);
+                            if (slot < P.ev_cap) { uint4* dst = reinterpret_cast<uint4*>(P.ev + slot); dst[0] = make_uint4(f_rec, len, eq, (uint32_t)er); dst[1] = make_uint4((k & 0xffffu) | (cls << 16), 0u, 0u, 0u); }
+                            else ++overflow;
+                            ++t; ++k;
+                        });
                     }
                     if (n_tot > avail) { s_cur = nb + (n_tot - avail); s_left = blk - (n_tot - avail); } else { s_cur += n_tot; s_left -= n_tot; }
                 }
