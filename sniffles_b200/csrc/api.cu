@@ -295,48 +295,30 @@ int snfb_set_config(snfb_ctx* ctx, const snfb_config* cfg) {
     ctx->cfg = *cfg; ctx->have_cfg = true; ctx->stage_a_done = ctx->stage_b_done = ctx->stage_c_done = false; return 0;
 }
 
-// ---- BAM CIGAR words -> CIGAR16 (include/snfb.h).  Host code; the only place the 32-bit form is read. ----
-static inline int c16_group_words(uint32_t len) { return len < (1u << 11) ? 1 : (len < (1u << 23) ? 2 : 3); }
-static const uint8_t C16_CLASS[9] = { 3, 1, 2, 6, 5, 4, 0, 3, 3 };     // M I D N S H P = X
-// number of 16-bit words of one record, pad words included (a group never straddles an 8-word boundary); 0 = bad op
-static inline uint64_t c16_count(const uint32_t* cg, uint32_t n, bool* bad) {
-    uint64_t k = 0;
-    for (uint32_t i = 0; i < n; ++i) {
-        if ((cg[i] & 15u) > 8u) { *bad = true; return 0; }
-        const int g = c16_group_words(cg[i] >> 4);
-        if ((k & 7) + g > 8) k = (k + 7) & ~7ull;
-        k += g;
-    }
-    return k;
-}
-static inline uint64_t c16_write(const uint32_t* cg, uint32_t n, uint16_t* out, uint32_t evt_min) {      // returns the words written (= c16_count)
-    uint64_t k = 0;
-    for (uint32_t i = 0; i < n; ++i) {
-        const uint32_t len = cg[i] >> 4; const int g = c16_group_words(len); const unsigned cls = C16_CLASS[cg[i] & 15u];
-        if ((k & 7) + g > 8) { while (k & 7) out[k++] = 0; }
-        const unsigned e = ((cls == 1 || cls == 2 || cls == 5) && len >= evt_min) ? 0x4000u : 0u;      // E: an I / D / S the streaming kernel has to look at
-        out[k++] = (uint16_t)(e | (cls << 11) | (len & 0x7ffu));
-        if (g >= 2) out[k++] = (uint16_t)(0x8000u | (1u << 12) | ((len >> 11) & 0xfffu));
-        if (g >= 3) out[k++] = (uint16_t)(0x8000u | (2u << 12) | ((len >> 23) & 0xfffu));
-    }
-    return k;
-}
+// ---- BAM CIGAR words -> CIGAR16 on the host: the ingest encoder run with one lane.  The only place the 32-bit form is read. ----
 // pass 1: off[i] = first word of record i in the 16-bit arena (every record starts a 16-byte group); false when an op code is unknown
 static bool c16_offsets(const snfb_rec* rec_in, uint64_t n_rec, const uint32_t* cigar32, std::vector<uint64_t>& off) {
     off.assign(n_rec + 1, 0);
+    const uint8_t* raw = reinterpret_cast<const uint8_t*>(cigar32);
     bool bad = false;
     #pragma omp parallel for schedule(static) reduction(|| : bad)
-    for (long long i = 0; i < (long long)n_rec; ++i) { bool b = false; const uint64_t w = c16_count(cigar32 + rec_in[i].cigar_off, rec_in[i].n_cigar, &b); bad = bad || b; off[i + 1] = (w + 7) & ~7ull; }
+    for (long long i = 0; i < (long long)n_rec; ++i) {
+        long long ref; int b = 0;
+        const uint32_t w = ingest::c16_convert<1>(raw, 4ull * rec_in[i].cigar_off, rec_in[i].n_cigar, nullptr, 0, 0, &ref, &b);
+        bad = bad || b; off[i + 1] = (w + 7) & ~7ull;
+    }
     if (bad) return false;
     for (uint64_t i = 0; i < n_rec; ++i) off[i + 1] += off[i];
     return true;
 }
 // pass 2: the words and the rewritten records
 static void c16_fill(const snfb_rec* rec_in, uint64_t n_rec, const uint32_t* cigar32, const std::vector<uint64_t>& off, snfb_rec* rec_out, uint16_t* out16, uint32_t evt_min) {
+    const uint8_t* raw = reinterpret_cast<const uint8_t*>(cigar32);
     #pragma omp parallel for schedule(static)
     for (long long i = 0; i < (long long)n_rec; ++i) {
         uint16_t* dst = out16 + off[i]; const uint64_t span = off[i + 1] - off[i];
-        const uint64_t k = c16_write(cigar32 + rec_in[i].cigar_off, rec_in[i].n_cigar, dst, evt_min);
+        long long ref; int bad = 0;      // c16_offsets has rejected a block with an unknown op
+        const uint64_t k = ingest::c16_convert<1>(raw, 4ull * rec_in[i].cigar_off, rec_in[i].n_cigar, dst, evt_min, 0, &ref, &bad);
         if (k < span) memset(dst + k, 0, 2 * (span - k));
         snfb_rec r = rec_in[i]; r.n_cigar = (uint32_t)k; r.cigar_off = off[i];
         rec_out[i] = r;

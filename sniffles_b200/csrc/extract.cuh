@@ -11,6 +11,7 @@
 //   build_leadtab region filter                                       leadprov.py:464-468
 #pragma once
 #include "common.cuh"
+#include "cigar16.h"
 
 namespace extract {
 
@@ -246,14 +247,6 @@ __device__ __noinline__ unsigned process_sa(const snfb_config* __restrict__ cfgp
 //   k_emit  one thread per Event: the 64-byte lead.
 //   k_sa    one thread per record with an SA tag: Lead.for_bnd + read_itersplits.
 // ================================================================================================
-// CIGAR16 (include/snfb.h): base word = [15] 0 | [14] E | [13:11] class | [10:0] length & 0x7ff; class bit 0 (word bit 11) = advances the
-// read, class bit 1 (word bit 12) = advances the reference; E = an I / D / S of at least the block's event length (what the streaming
-// kernel must look at).  Extension word = [15] 1 | [14:12] level (1, 2) | [11:0] payload, adding payload << (11 + 12 * (level - 1)).
-constexpr unsigned C16_I = 1, C16_D = 2, C16_M = 3, C16_H = 4, C16_S = 5;
-constexpr unsigned C16_LEN_BITS = 11, C16_LEN_MASK = 0x7ffu, C16_E = 0x4000u;
-__device__ __forceinline__ bool c16_is_event(unsigned cls) { return (0x26u >> cls) & 1u; }        // I D S
-__device__ __forceinline__ unsigned c16_class(unsigned w) { return (w >> C16_LEN_BITS) & 7u; }
-__device__ __forceinline__ unsigned c16_ext_add(unsigned e) { return (e & 0xfffu) << (C16_LEN_BITS + 12u * (((e >> 12) & 7u) - 1u)); }
 
 // the op at word h of the eight 16-bit words one lane holds (cls 0 / len 0 where a pad, P or extension word sits).  Groups never
 // straddle a 16-byte boundary, so this is lane-local.
@@ -262,11 +255,11 @@ __device__ __forceinline__ void c16_op(const uint32_t (&ww)[4], int h, unsigned&
     #pragma unroll
     for (int e = 0; e < 3; ++e) x[e] = h + e < 8 ? (ww[(h + e) >> 1] >> (16 * ((h + e) & 1))) & 0xffffu : 0u;
     unsigned c = 0, l = 0;
-    if (!(x[0] & 0x8000u)) {
-        c = c16_class(x[0]); l = x[0] & C16_LEN_MASK;
-        if (x[1] & 0x8000u) {
+    if (!(x[0] & C16_EXT)) {
+        c = c16_word_class(x[0]); l = x[0] & C16_LEN_MASK;
+        if (x[1] & C16_EXT) {
             l += c16_ext_add(x[1]);
-            if (x[2] & 0x8000u) l += c16_ext_add(x[2]);
+            if (x[2] & C16_EXT) l += c16_ext_add(x[2]);
         }
     }
     cls = c; len = l;
@@ -312,17 +305,17 @@ __device__ __forceinline__ bool index_record(const IndexParams& P, uint32_t i) {
     { bool first = true; uint32_t k = 0;
       while (k < n) {
           const unsigned w = __ldg(cg + k); if (w == 0) { ++k; continue; }
-          unsigned len = w & C16_LEN_MASK; const unsigned cls = c16_class(w); uint32_t k2 = k + 1;
-          while (k2 < n) { const unsigned e = __ldg(cg + k2); if (!(e & 0x8000u)) break; len += c16_ext_add(e); ++k2; }
+          unsigned len = w & C16_LEN_MASK; const unsigned cls = c16_word_class(w); uint32_t k2 = k + 1;
+          while (k2 < n) { const unsigned e = __ldg(cg + k2); if (!(e & C16_EXT)) break; len += c16_ext_add(e); ++k2; }
           if (first) { if (cls == C16_S || cls == C16_H) clip_left = (int)len; first = false; fe = k2; }
           if (cls == C16_S) qas += (int)len; else if (cls != C16_H) break;
           k = k2;
       } }
     { bool last = true; long k = (long)n - 1;
       while (k >= (long)fe) {
-          long b = k; while (b > (long)fe && (__ldg(cg + b) & 0x8000u)) --b;
+          long b = k; while (b > (long)fe && (__ldg(cg + b) & C16_EXT)) --b;
           const unsigned w = __ldg(cg + b); if (w == 0) { k = b - 1; continue; }
-          unsigned len = w & C16_LEN_MASK; const unsigned cls = c16_class(w);
+          unsigned len = w & C16_LEN_MASK; const unsigned cls = c16_word_class(w);
           for (long e2 = b + 1; e2 <= k; ++e2) { const unsigned e = __ldg(cg + e2); len += c16_ext_add(e); }
           if (last) { if (cls == C16_S || cls == C16_H) clip_right = (int)len; last = false; }
           if (cls == C16_S) qae -= (int)len; else if (cls != C16_H) break;
@@ -395,12 +388,11 @@ constexpr unsigned WALK_SLOTS = 64;                                     // per w
 // lowers the E-bit threshold of a CIGAR16 arena in place (a config that cares about shorter events than the block was packed for)
 __global__ void k_reflag(uint16_t* __restrict__ cigar, unsigned long long n_words, unsigned evt_min) {
     for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n_words; i += (unsigned long long)gridDim.x * blockDim.x) {
-        const unsigned w = cigar[i]; if (w & 0x8000u) continue;
-        const unsigned cls = c16_class(w);
-        if (!c16_is_event(cls) || (w & C16_E)) continue;
-        bool big = (w & C16_LEN_MASK) >= evt_min;
-        if (!big && (i & 7) != 7) big = (cigar[i + 1] & 0x8000u) != 0;          // an extension word follows: the length is at least 2048
-        if (big) cigar[i] = (uint16_t)(w | C16_E);
+        const unsigned w = cigar[i]; if (w & (C16_EXT | C16_E)) continue;
+        uint32_t len = w & C16_LEN_MASK;
+        if (len < evt_min && (i & 7) != 7 && (cigar[i + 1] & C16_EXT)) len = 1u << C16_LEN_BITS;      // an extension word follows: the op is at least that long
+        const unsigned e = c16_e_flag(c16_word_class(w), len, evt_min);
+        if (e) cigar[i] = (uint16_t)(w | e);
     }
 }
 
@@ -463,7 +455,7 @@ __device__ __forceinline__ void group_events(const uint4 v, uint32_t q0, int r0,
         const uint32_t h = (uint32_t)__ffs(em) - 1u;
         const uint32_t w = h < 4u ? (h < 2u ? v.x : v.y) : (h < 6u ? v.z : v.w);
         const uint32_t x = (w >> (16u * (h & 1u))) & 0xffffu;
-        const unsigned cls = c16_class(x), len = x & C16_LEN_MASK;
+        const unsigned cls = c16_word_class(x), len = x & C16_LEN_MASK;
         if (len > 10u && (cls == C16_I || cls == C16_D)) big += len;
         if (!(c16_is_event(cls) && (int)len >= minsv)) continue;
         uint32_t aq = 0, ar = 0;                    // the words below h: whole 32-bit words, and the low half of h's own word when h is odd

@@ -7,15 +7,14 @@
 // address and broadcast), so no lane ever waits for a broadcast, and the parts that ARE data parallel — filling the look-up
 // tables, LZ77 match copies, stored blocks, byte copies — are split across the lanes.  With NL = 1 the same code is plain
 // sequential C++: tests/native/ingest_host.cpp compiles this header with g++ and checks it against zlib on the CPU (test
-// infrastructure; the product only ever instantiates NL = 32 inside kernels).
+// infrastructure).  The product instantiates NL = 32 inside kernels, and c16_convert<1> for the host CIGAR16 conversion (api.cu).
 #pragma once
 #include <stdint.h>
+#include "cigar16.h"            // also defines SNFB_HD
 #if defined(__CUDACC__)
-#define SNFB_HD __host__ __device__ __forceinline__
 #define SNFB_HDN __host__ __device__ __noinline__
 #else
 #include <string.h>
-#define SNFB_HD inline
 #define SNFB_HDN inline
 #endif
 
@@ -354,9 +353,8 @@ SNFB_HD void parse_record(const uint8_t* raw, uint64_t body, uint32_t bs, RawRec
     o->n_cig = n_cig; o->status = ST_OK;
 }
 
-// ---------------------------------------------------------------- BAM CIGAR words -> CIGAR16 (include/snfb.h; the layout snfb_pack_cigar16 writes)
-SNFB_HD int c16_words(uint32_t len) { return len < (1u << 11) ? 1 : (len < (1u << 23) ? 2 : 3); }
-SNFB_HD unsigned c16_class(unsigned op) { return (unsigned)((0x330456213ull >> (4 * op)) & 15ull); }      // M I D N S H P = X -> 3 1 2 6 5 4 0 3 3
+// ---------------------------------------------------------------- BAM CIGAR words -> CIGAR16 (cigar16.h)
+// The one CIGAR16 encoder: the ingest kernels run it with 32 lanes, snfb_pack_cigar16 and snfb_load_records with one.
 // Convert the n BAM CIGAR words at raw[src ..] ; out == nullptr only counts.  Returns the number of 16-bit words written (pads
 // inside the record included, not rounded up); *reflen = reference bases the CIGAR covers; *bad set when an op code is unknown.
 template <int NL>
@@ -366,11 +364,10 @@ SNFB_HD uint32_t c16_convert(const uint8_t* raw, uint64_t src, uint32_t n, uint1
         const uint32_t i = base + lane; const bool valid = i < n;
         const uint32_t w = valid ? ld32u(raw, src + 4ull * i) : 0u; const uint32_t len = w >> 4; const unsigned code = w & 15u;
         if (valid && code > 8u) bad_op = true;
-        const unsigned cls = c16_class(code > 8u ? 6u : code);
-        const int g = valid ? c16_words(len) : 0;
-        if (valid && (cls & 2u)) ref += len;            // class bit 1 (= bit 12 of the word): the op advances the reference (M, D, N)
-        const unsigned e = ((cls == 1u || cls == 2u || cls == 5u) && len >= evt_min) ? 0x4000u : 0u;
-        const uint16_t w0 = (uint16_t)(e | (cls << 11) | (len & 0x7ffu));
+        const unsigned cls = c16_op_class(code > 8u ? 6u : code);
+        const int g = valid ? c16_op_words(len) : 0;
+        if (valid && (cls & 2u)) ref += len;            // class bit 1: the op advances the reference (M, D, N)
+        const uint16_t w0 = c16_base_word(cls, len, evt_min);
         const uint32_t cnt = n - base < (uint32_t)NL ? n - base : (uint32_t)NL;
         if (!warp_any<NL>(g > 1)) {                     // 32 short ops: one word each, no group can straddle
             if (valid && out) out[k + lane] = w0;
@@ -381,8 +378,8 @@ SNFB_HD uint32_t c16_convert(const uint8_t* raw, uint64_t src, uint32_t n, uint1
                 if ((k & 7u) + (uint32_t)gj > 8u) { const uint32_t k8 = (k + 7u) & ~7u; if (out && lane == 0) for (uint32_t z = k; z < k8; ++z) out[z] = 0; k = k8; }
                 if ((uint32_t)lane == j && out) {
                     out[k] = w0;
-                    if (g >= 2) out[k + 1] = (uint16_t)(0x8000u | (1u << 12) | ((len >> 11) & 0xfffu));
-                    if (g >= 3) out[k + 2] = (uint16_t)(0x8000u | (2u << 12) | ((len >> 23) & 0xfffu));
+                    if (g >= 2) out[k + 1] = c16_ext_word(len, 1);
+                    if (g >= 3) out[k + 2] = c16_ext_word(len, 2);
                 }
                 k += (uint32_t)gj;
             }

@@ -24,7 +24,7 @@ sys.path[:0] = [ROOT, os.path.join(ROOT, "oracle", "pyref")]
 logging.disable(logging.CRITICAL)
 
 import harness  # noqa: E402
-from sniffles_b200 import bampack, synth  # noqa: E402
+from sniffles_b200 import bamio, synth  # noqa: E402
 
 FIXTURES = {
     # name: (synth.generate kwargs, reference CLI args)
@@ -86,8 +86,15 @@ def make_bam_vectors():
     data = os.path.join(harness.REFERENCE_SRC, "tests", "data")
     blocks, expect = [], []
     for fn in ("hg008.bam", "hg002.bam"):
-        contigs, recs = bampack.read_bam(os.path.join(data, fn))
-        blk = bampack.pack(contigs, recs, with_seq=False)
+        f = bamio.BamFile(os.path.join(data, fn))
+        tasks, recs = [], []                # one task per contig that has records ([0, len-1], as the reference plans them: sniffles:313-358)
+        for c, (name, length) in enumerate(f.contigs):
+            got = list(f.fetch(name, 0, length))
+            if got:
+                recs.extend((len(tasks), r) for r in got)
+                tasks.append((c, 0, length - 1, len(tasks)))
+        blk = bamio.pack_records(f.contigs, recs, tasks, with_seq=False)
+        f.close()
         for i in range(len(blk.rec)):
             rd = harness.DuckRead(blk, i)
             ld = Lead.for_bnd(0, rd)

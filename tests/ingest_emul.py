@@ -14,7 +14,7 @@ from sniffles_b200 import abi
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, "native", "ingest_host.cpp")
 _SO = os.path.join(_HERE, "native", "libingest_host.so")
-_CORE = os.path.join(os.path.dirname(_HERE), "sniffles_b200", "csrc", "ingest_core.h")
+_CORE = [os.path.join(os.path.dirname(_HERE), "sniffles_b200", "csrc", f) for f in ("ingest_core.h", "cigar16.h")]
 _L = None
 
 RAWREC_DTYPE = np.dtype([("body", "<u8"), ("cig_src", "<u8"), ("seq_src", "<u8"), ("sa_src", "<u8"), ("body_len", "<u4"), ("n_cig", "<u4"), ("sa_len", "<u4"),
@@ -25,7 +25,7 @@ RAWREC_DTYPE = np.dtype([("body", "<u8"), ("cig_src", "<u8"), ("seq_src", "<u8")
 def lib():
     global _L
     if _L is None:
-        if not os.path.exists(_SO) or os.path.getmtime(_SO) < max(os.path.getmtime(_SRC), os.path.getmtime(_CORE)):
+        if not os.path.exists(_SO) or os.path.getmtime(_SO) < max(os.path.getmtime(p) for p in [_SRC, *_CORE]):
             subprocess.check_call(["g++", "-O2", "-fPIC", "-shared", "-Wall", "-o", _SO, _SRC])
         L = C.CDLL(_SO)
         L.ingest_host_inflate.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]

@@ -1,5 +1,7 @@
 """CIGAR16 (include/snfb.h): snfb_pack_cigar16 is host code, so the format is checked without a GPU:
-every op survives the round trip, groups never straddle a 16-byte boundary, records start on one."""
+every op survives the round trip, groups never straddle a 16-byte boundary, records start on one.
+`check_record` decodes with this file's own reading of the format, independent of sniffles_b200/csrc/cigar16.h; the ingest tests
+check the device encoder's words with it as well."""
 import numpy as np
 import pytest
 
@@ -8,23 +10,45 @@ from sniffles_b200 import abi, binding, synth
 CLASS = [3, 1, 2, 6, 5, 4, 0, 3, 3]          # M I D N S H P = X
 
 
-E = [[]]
-
-
 def decode(words):
-    ops = []
-    E[0] = []
+    """CIGAR16 words -> [(length, class, E)]; pad words are skipped.  An op's extension words follow it directly, level 1 then 2."""
+    ops, level = [], 0          # the level the next extension word must have (0: none may come)
     for k, w in enumerate(int(x) for x in words):
         if w & 0x8000:
             assert k % 8 != 0, "an extension word starts a 16-byte group"
-            assert ops, "extension word without a base word"
-            ln, c = ops[-1]
-            ops[-1] = (ln + ((w & 0xfff) << (11 + 12 * (((w >> 12) & 7) - 1))), c)
+            assert level and (w >> 12) & 7 == level, "extension word without its base word or out of order"
+            ln, c, e = ops[-1]
+            ops[-1] = (ln + ((w & 0xfff) << (11 + 12 * (level - 1))), c, e)
+            level = 2 if level == 1 else 0
         elif w != 0:
-            ln, c = w & 0x7ff, (w >> 11) & 7
-            ops.append((ln, c))
-            E[0].append((len(ops) - 1, bool(w & 0x4000)))
+            ops.append((w & 0x7ff, (w >> 11) & 7, bool(w & 0x4000)))
+            level = 1
+        else:
+            level = 0
     return ops
+
+
+def n_words(cigar32):
+    """words of one record: 1, 2 or 3 per op (length below 2^11, 2^23, or more), and pad words only where a group would straddle 16 bytes"""
+    k = 0
+    for w in cigar32:
+        ln = int(w) >> 4
+        g = 1 if ln < 1 << 11 else 2 if ln < 1 << 23 else 3
+        if k % 8 + g > 8:
+            k = (k + 7) // 8 * 8
+        k += g
+    return k
+
+
+def check_record(words, cigar32, evt_min=11):
+    """one record's CIGAR16 words (from its first word to its last op's last word) against its BAM CIGAR words"""
+    assert len(words) == n_words(cigar32)
+    got = decode(words)
+    want = [(int(w) >> 4, CLASS[int(w) & 15]) for w in cigar32]
+    want = [(ln, c) for ln, c in want if not (ln == 0 and c == 0)]        # a zero-length P is a pad word
+    assert [(ln, c) for ln, c, _ in got] == want
+    for ln, c, e in got:          # E bit: an I / D / S of at least evt_min bases
+        assert e == (c in (1, 2, 5) and ln >= evt_min), (ln, c, e)
 
 
 def block_of(cigars):
@@ -42,12 +66,8 @@ def check(rec, cigar32):
     assert len(c16) % 8 == 0
     for r, r16 in zip(rec, rec16):
         assert int(r16["cigar_off"]) % 8 == 0
-        want = [(int(w) >> 4, CLASS[int(w) & 15]) for w in cigar32[int(r["cigar_off"]):int(r["cigar_off"]) + int(r["n_cigar"])]]
-        want = [(ln, c) for ln, c in want if not (ln == 0 and c == 0)]
-        got = decode(c16[int(r16["cigar_off"]):int(r16["cigar_off"]) + int(r16["n_cigar"])])
-        assert got == want
-        for k, e in E[0]:          # E bit: an I / D / S of at least 11 bases
-            assert e == (got[k][1] in (1, 2, 5) and got[k][0] >= 11), (got[k], e)
+        o, n = int(r16["cigar_off"]), int(r16["n_cigar"])
+        check_record(c16[o:o + n], cigar32[int(r["cigar_off"]):int(r["cigar_off"]) + int(r["n_cigar"])])
         for f in ("task", "pos", "flag", "mapq", "l_seq", "seq_off", "var_off", "nm"):
             assert r[f] == r16[f]
     return rec16, c16

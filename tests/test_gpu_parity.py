@@ -28,7 +28,8 @@ def test_config1_shape():
     assert len(got.cand) > 20
 
 
-@pytest.mark.parametrize("args", [(), ("--mosaic",), ("--no-qc",), ("--repeat",), ("--minsvlen", "30")])
+# --minsvlen 8 screens for events below the E threshold the block was packed with: the library re-flags the arena (k_reflag)
+@pytest.mark.parametrize("args", [(), ("--mosaic",), ("--no-qc",), ("--repeat",), ("--minsvlen", "30"), ("--minsvlen", "8")])
 def test_config2_scaled(args):
     _run(synth.config_block(2, 0.004), *args)
 
