@@ -441,9 +441,6 @@ typedef struct snfb_combine_out {
     int32_t*  cov_non;        /* [n_cand][n_samples]; -1 where the sample is included (never probed) */
 } snfb_combine_out;
 int         snfb_combine_groups(snfb_ctx* ctx, const snfb_combine_in* in, snfb_combine_out* out);
-/* developer aid: with SNFB_DEBUG set in the environment the consensus alignment kernel records, per warp, busy cycles / elapsed cycles / items /
- * longest item (cycles, consensus length, read length); returns 1 when nothing was recorded */
-int         snfb_debug_dump(snfb_ctx* ctx, uint64_t* out, uint64_t n_words);
 /* self-check of the exact statistics.stdev arithmetic (host build of the routine the kernels use): the correctly rounded sqrt(P / Q) for
  * P = p_hi * 2^64 + p_lo; slow != 0 selects the limb-by-limb restatement of CPython's _float_sqrt_of_frac, 0 the verified fast path */
 double      snfb_selftest_sqrt_frac(uint64_t p_hi, uint64_t p_lo, uint64_t q, int slow);

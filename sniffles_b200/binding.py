@@ -16,7 +16,7 @@ EXPORTS = ["snfb_version", "snfb_sizeof", "snfb_hash_name", "snfb_ctx_create", "
            "snfb_load_records", "snfb_extract_leads", "snfb_cluster_call", "snfb_consensus", "snfb_run",
            "snfb_last_timings", "snfb_device_candidates", "snfb_device_alt", "snfb_launch_count",
            "snfb_pin_host", "snfb_unpin_host", "snfb_pack_cigar16", "snfb_rerun_count", "snfb_coverage_bins",
-           "snfb_nccl_unique_id", "snfb_comm_init", "snfb_allgather_candidates", "snfb_selftest_sqrt_frac", "snfb_debug_dump", "snfb_poa", "snfb_combine_groups", "snfb_selftest_edit_distance",
+           "snfb_nccl_unique_id", "snfb_comm_init", "snfb_allgather_candidates", "snfb_selftest_sqrt_frac", "snfb_poa", "snfb_combine_groups", "snfb_selftest_edit_distance",
            "snfb_load_bam", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf"]
 
 
@@ -59,7 +59,6 @@ def lib():
         L.snfb_nccl_unique_id.argtypes = [C.c_void_p]
         L.snfb_comm_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
         L.snfb_allgather_candidates.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(abi.GatherView)]
-        L.snfb_debug_dump.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
         L.snfb_poa.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
         L.snfb_combine_groups.argtypes = [C.c_void_p, C.POINTER(abi.CombineIn), C.POINTER(abi.CombineOut)]
         L.snfb_selftest_edit_distance.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]

@@ -138,7 +138,6 @@ static void mark(snfb_ctx* ctx, const char* name, uint64_t bytes = 0) {
     cudaEventRecord(ctx->ev[ctx->n_ev], ctx->st);
     ctx->ev_name[ctx->n_ev] = name; ctx->ev_bytes[ctx->n_ev] = bytes; ++ctx->n_ev;
 }
-#define LAUNCHED(ctx, k) ((ctx)->launches += (k))
 static int grid_for(unsigned long long n, int threads) { unsigned long long g = (n + threads - 1) / threads; if (g < 1) g = 1; if (g > (uint64_t)NUM_SMS * 32) g = (uint64_t)NUM_SMS * 32; return (int)g; }
 static int bits_for(uint32_t n) { int b = 0; while ((1ull << b) < n) ++b; return b; }
 
@@ -218,20 +217,13 @@ __global__ void k_gather_merge(const uint8_t* recv, unsigned long long cap, int 
     if (tid == 0) reinterpret_cast<uint32_t*>(out + o_ro)[tot.n_cand] = (uint32_t)tot.n_rn;
 }
 
-// lanes per BGZF block of the DEFLATE kernel: SNFB_INFLATE_LANES = 32, 16 or 8 (measured default below)
-template <int NL> static void launch_inflate_nl(snfb_ctx* ctx, const ingest::BgzfBlock* d_blk, unsigned nb, ingest::IngestCounters* d_ctr) {
-    static bool attr = false;
-    const size_t smem = ingest::inflate_smem_bytes<NL>();
-    if (!attr) { cudaFuncSetAttribute(ingest::k_inflate<NL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
-    const unsigned per_block = ingest::INF_WARPS * (32 / NL);
+// the DEFLATE kernel over nb BGZF blocks: as many blocks per SM as the tables' shared memory allows (at most 8)
+static void launch_inflate(snfb_ctx* ctx, const ingest::BgzfBlock* d_blk, unsigned nb, ingest::IngestCounters* d_ctr) {
+    const size_t smem = ingest::INF_SMEM_BYTES;
+    const unsigned per_block = ingest::INF_WARPS * (32 / ingest::INF_LANES);
     const unsigned resident = (unsigned)std::max<size_t>(1, std::min<size_t>(8, (220 * 1024) / (smem + 1024)));
     const unsigned grid = std::min<unsigned>((nb + per_block - 1) / per_block, (unsigned)NUM_SMS * resident);
-    ingest::k_inflate<NL><<<grid, ingest::INF_WARPS * 32, smem, ctx->st>>>(ctx->b_comp.as<uint8_t>(), d_blk, nb, ctx->b_raw.as<uint8_t>(), d_ctr);
-}
-static void launch_inflate(snfb_ctx* ctx, const ingest::BgzfBlock* d_blk, unsigned nb, ingest::IngestCounters* d_ctr) {
-    static int lanes = 0;
-    if (!lanes) { const char* e = getenv("SNFB_INFLATE_LANES"); lanes = e ? atoi(e) : 16; if (lanes != 32 && lanes != 16 && lanes != 8) lanes = 16; }
-    if (lanes == 32) launch_inflate_nl<32>(ctx, d_blk, nb, d_ctr); else if (lanes == 16) launch_inflate_nl<16>(ctx, d_blk, nb, d_ctr); else launch_inflate_nl<8>(ctx, d_blk, nb, d_ctr);
+    launch(ctx->launches, ingest::k_inflate, grid, ingest::INF_WARPS * 32, smem, ctx->st, ctx->b_comp.as<uint8_t>(), d_blk, nb, ctx->b_raw.as<uint8_t>(), d_ctr);
 }
 
 extern "C" {
@@ -477,7 +469,7 @@ int snfb_inflate_bgzf(snfb_ctx* ctx, const uint8_t* bgzf, uint64_t n_bytes, uint
     CUDA_TRY(cudaMemsetAsync(d_ctr, 0, sizeof(ingest::IngestCounters), ctx->st));
     CUDA_TRY(cudaMemcpyAsync(d_blk, blocks.data(), sizeof(ingest::BgzfBlock) * nb, cudaMemcpyHostToDevice, ctx->st));
     mark(ctx, "inflate", n_bytes + raw_len);
-    if (nb) { launch_inflate(ctx, d_blk, (unsigned)nb, d_ctr); LAUNCHED(ctx, 1); }
+    if (nb) launch_inflate(ctx, d_blk, (unsigned)nb, d_ctr);
     mark(ctx, nullptr);
     ingest::IngestCounters hc;
     CUDA_TRY(cudaMemcpyAsync(&hc, d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, ctx->st));
@@ -534,11 +526,11 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
     CUDA_TRY(cudaMemcpyAsync(d_blk, blocks.data(), sizeof(ingest::BgzfBlock) * nb, cudaMemcpyHostToDevice, st));
     if (ns) CUDA_TRY(cudaMemcpyAsync(d_span, spans.data(), sizeof(ingest::Span) * ns, cudaMemcpyHostToDevice, st));
     mark(ctx, "inflate", in->n_bytes + raw_len);
-    if (nb) { launch_inflate(ctx, d_blk, (unsigned)nb, d_ctr); LAUNCHED(ctx, 1); }
+    if (nb) launch_inflate(ctx, d_blk, (unsigned)nb, d_ctr);
     mark(ctx, "walk_records", 0);
     if (ns) {
-        ingest::k_walk<<<(unsigned)((ns + 127) / 128), 128, 0, st>>>(raw, raw_len, d_span, (unsigned)ns, 0, span_cnt, nullptr, nullptr, 0, d_ctr); LAUNCHED(ctx, 1);
-        LAUNCHED(ctx, prims::exclusive_scan(span_cnt, span_base, scan_tmp0, nullptr, ns, &d_ctr->n_raw, st));
+        launch(ctx->launches, ingest::k_walk, (unsigned)((ns + 127) / 128), 128, 0, st, raw, raw_len, d_span, (unsigned)ns, 0, span_cnt, nullptr, nullptr, 0, d_ctr);
+        prims::exclusive_scan(ctx->launches, span_cnt, span_base, scan_tmp0, nullptr, ns, &d_ctr->n_raw, st);
     }
     if (ctx->h_ing.ensure(2 * sizeof(ingest::IngestCounters))) return fail(ctx, "out of pinned memory");
     ingest::IngestCounters* hc = ctx->h_ing.as<ingest::IngestCounters>();
@@ -565,15 +557,15 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
     uint64_t n_rec = 0, n_groups = 0, n_var16 = 0, n_seq16 = 0;
     if (n_raw) {
         const unsigned warp_grid = (unsigned)std::min<uint64_t>((n_raw + 7) / 8, (uint64_t)NUM_SMS * 16);
-        ingest::k_walk<<<(unsigned)((ns + 127) / 128), 128, 0, st>>>(raw, raw_len, d_span, (unsigned)ns, 1, span_cnt, span_base, recs, n_raw, d_ctr);
+        launch(ctx->launches, ingest::k_walk, (unsigned)((ns + 127) / 128), 128, 0, st, raw, raw_len, d_span, (unsigned)ns, 1, span_cnt, span_base, recs, n_raw, d_ctr);
         mark(ctx, "parse_records", 0);
-        ingest::k_parse<<<(unsigned)((n_raw + 127) / 128), 128, 0, st>>>(raw, recs, (unsigned)n_raw, ctx->b_task.as<snfb_task>(), d_ctr);
+        launch(ctx->launches, ingest::k_parse, (unsigned)((n_raw + 127) / 128), 128, 0, st, raw, recs, (unsigned)n_raw, ctx->b_task.as<snfb_task>(), d_ctr);
         mark(ctx, "record_sizes", 0);
-        ingest::k_rec_sizes<<<warp_grid, 256, 0, st>>>(raw, recs, (unsigned)n_raw, ctx->b_task.as<snfb_task>(), evt, keep, groups, var16, seq16, d_ctr); LAUNCHED(ctx, 3);
-        LAUNCHED(ctx, prims::exclusive_scan(keep, idx, scan_tmp, nullptr, n_raw, &d_ctr->n_keep, st));
-        LAUNCHED(ctx, prims::exclusive_scan(groups, grp_off, scan_tmp, nullptr, n_raw, &d_ctr->n_groups, st));
-        LAUNCHED(ctx, prims::exclusive_scan(var16, var_off, scan_tmp, nullptr, n_raw, &d_ctr->n_var, st));
-        LAUNCHED(ctx, prims::exclusive_scan(seq16, seq_off, scan_tmp, nullptr, n_raw, &d_ctr->n_seq16, st));
+        launch(ctx->launches, ingest::k_rec_sizes, warp_grid, 256, 0, st, raw, recs, (unsigned)n_raw, ctx->b_task.as<snfb_task>(), evt, keep, groups, var16, seq16, d_ctr);
+        prims::exclusive_scan(ctx->launches, keep, idx, scan_tmp, nullptr, n_raw, &d_ctr->n_keep, st);
+        prims::exclusive_scan(ctx->launches, groups, grp_off, scan_tmp, nullptr, n_raw, &d_ctr->n_groups, st);
+        prims::exclusive_scan(ctx->launches, var16, var_off, scan_tmp, nullptr, n_raw, &d_ctr->n_var, st);
+        prims::exclusive_scan(ctx->launches, seq16, seq_off, scan_tmp, nullptr, n_raw, &d_ctr->n_seq16, st);
         CUDA_TRY(cudaMemcpyAsync(hc, d_ctr, sizeof(*hc), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
         if (hc->malformed || hc->bad_cigar) return fail(ctx, std::to_string(hc->malformed) + " malformed BAM record(s), " + std::to_string(hc->bad_cigar) + " with a CIGAR operation the path does not know");
@@ -586,7 +578,7 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
     CUDA_TRY(cudaMemsetAsync(ctx->b_cigar.as<uint16_t>() + 8 * n_groups, 0, 2 * 24, st));
     if (n_raw) {
         const unsigned warp_grid = (unsigned)std::min<uint64_t>((n_raw + 7) / 8, (uint64_t)NUM_SMS * 16);
-        ingest::k_pack<<<warp_grid, 256, 0, st>>>(raw, recs, (unsigned)n_raw, evt, keep, idx, grp_off, groups, var_off, seq_off, ctx->b_rec.as<snfb_rec>(), ctx->b_cigar.as<uint16_t>(), ctx->b_var.as<uint8_t>(), ctx->b_seq.as<uint8_t>()); LAUNCHED(ctx, 1);
+        launch(ctx->launches, ingest::k_pack, warp_grid, 256, 0, st, raw, recs, (unsigned)n_raw, evt, keep, idx, grp_off, groups, var_off, seq_off, ctx->b_rec.as<snfb_rec>(), ctx->b_cigar.as<uint16_t>(), ctx->b_var.as<uint8_t>(), ctx->b_seq.as<uint8_t>());
     }
     mark(ctx, nullptr);
     ctx->n_ev_load = ctx->n_ev;
@@ -650,7 +642,6 @@ static void carve_c(snfb_ctx* ctx, Carver& c) {
     cc.alt_off = c.take<uint32_t>(k.cand + 1); cc.scr_off = c.take<uint32_t>(k.cand + 1); cc.work_big = c.take<uint32_t>(k.cand + 1); cc.work_small = c.take<uint32_t>(k.cand + 1); cc.work_ctr = c.take<uint32_t>(64);
     cc.items_big = c.take<consensus::C::Item>(k.item + 1); cc.items_small = c.take<consensus::C::Item>(k.item + 1); cc.tiles = c.take<uint2>(k.tile + 1);
     cc.alt = c.take<uint8_t>(k.alt + 64); cc.scr = c.take<uint8_t>(k.scr16 * 16 + 64);
-    cc.dbg = getenv("SNFB_DEBUG") ? c.take<unsigned long long>(NUM_SMS * 9 * consensus::ALIGN_WARPS * 8 + 8) : nullptr;
     ctx->seq_req = c.take<consensus::SeqReq>(k.req + 1); ctx->seq_arena = c.take<uint8_t>(k.req16 * 16 + 64);
 }
 static int ensure_arenas(snfb_ctx* ctx) {
@@ -707,57 +698,56 @@ static int enqueue_stage_a(snfb_ctx* ctx) {
     if (evt_need(ctx) < ctx->evt_min) {
         // the block's E bits were set for longer events than this configuration looks at: lower the threshold in place
         if (ctx->on_device) return fail(ctx, "the device-resident CIGAR16 arena was packed with a larger event length than the configuration needs: repack with snfb_pack_cigar16(evt_min)");
-        extract::k_reflag<<<NUM_SMS * 8, 256, 0, st>>>(const_cast<uint16_t*>(ctx->d_cigar), ctx->n_cigar, evt_need(ctx)); LAUNCHED(ctx, 1);
+        launch(ctx->launches, extract::k_reflag, NUM_SMS * 8, 256, 0, st, const_cast<uint16_t*>(ctx->d_cigar), ctx->n_cigar, evt_need(ctx));
         ctx->evt_min = evt_need(ctx);
     }
     mark(ctx, "k_rec_index");
     if (nrec) {
-        k_validate<<<(unsigned)((nrec + 255) / 256), 256, 0, st>>>(ctx->d_rec, (uint32_t)nrec, nt, ctx->n_cigar, ctx->n_var, ctx->n_seq, ctx->seq_on_demand ? 0 : 1, ctr);
+        launch(ctx->launches, k_validate, (unsigned)((nrec + 255) / 256), 256, 0, st, ctx->d_rec, (uint32_t)nrec, nt, ctx->n_cigar, ctx->n_var, ctx->n_seq, ctx->seq_on_demand ? 0 : 1, ctr);
         extract::IndexParams I{};
         I.rec = ctx->d_rec; I.cigar = ctx->d_cigar; I.task = b.task; I.n_rec = (uint32_t)nrec; I.n_task = nt; I.rec_pos = ctx->rec_pos; I.task_first = ctx->task_first; I.task_last = ctx->task_last;
         I.scan = ctx->scanrec; I.clip = ctx->clip; I.rec_end = ctx->rec_end; I.rec_flags = ctx->rec_flags; I.rec_nm = ctx->rec_nm; I.rec_nlead = ctx->rec_nlead; I.ctr = ctr;
         I.mapq_min = cf.mapq; I.alen_min = cf.min_alignment_length; I.excl = cf.exclude_flags; I.want_nm = (cf.qc_nm_measure || cf.phase) ? 1 : 0; I.n_cigar = ctx->n_cigar;
         I.sa_list = ctx->sa_list; I.n_sa = &ctr->n_sa;
-        extract::k_rec_index<<<(unsigned)((nrec + 255) / 256), 256, 0, st>>>(I); LAUNCHED(ctx, 2);
+        launch(ctx->launches, extract::k_rec_index, (unsigned)((nrec + 255) / 256), 256, 0, st, I);
         // the CIGAR walk: bytes = the CIGAR16 arena (bench.py counts the passing records' groups)
         mark(ctx, "k_scan", 2 * ctx->n_cigar);
-        if (nrec >= extract::WALK_WIDE_MIN) extract::k_cigar_walk<32><<<extract::WALK_BLOCKS, extract::WALK_THREADS, 0, st>>>(S);
-        else extract::k_cigar_walk<1><<<extract::WALK_BLOCKS, extract::WALK_THREADS, 0, st>>>(S);
-        LAUNCHED(ctx, 1);
+        if (nrec >= extract::WALK_WIDE_MIN) launch(ctx->launches, extract::k_cigar_walk<32>, extract::WALK_BLOCKS, extract::WALK_THREADS, 0, st, S);
+        else launch(ctx->launches, extract::k_cigar_walk<1>, extract::WALK_BLOCKS, extract::WALK_THREADS, 0, st, S);
         mark(ctx, "k_rec_post");
         extract::PostParams Q{};
         Q.scan = I.scan; Q.clip = I.clip; Q.task = b.task; Q.n_rec = (uint32_t)nrec; Q.rec_end = ctx->rec_end; Q.rec_big = ctx->rec_big; Q.rec_nm = ctx->rec_nm;
         Q.task_reads = ctx->task_reads; Q.task_cov_bp = ctx->task_cov; Q.task_maxspan = ctx->task_span;
-        extract::k_rec_post<<<(unsigned)((nrec + 255) / 256), 256, 0, st>>>(Q);
+        launch(ctx->launches, extract::k_rec_post, (unsigned)((nrec + 255) / 256), 256, 0, st, Q);
         mark(ctx, "k_emit");
         extract::EmitParams E{};
         E.rec = ctx->d_rec; E.clip = ctx->clip; E.var = ctx->d_var; E.ev = S.ev; E.n_ev = S.n_ev; E.ev_cap = ctx->cap.lead;
         E.leads = ctx->leads; E.ctr = ctr; E.maxlen = cf.dev_seq_cache_maxlen; E.detect_large_ins = cf.detect_large_ins; E.longinslen = (double)cf.long_ins_length / 2.0;
-        extract::k_emit<<<NUM_SMS * 16, 128, 0, st>>>(E);
+        launch(ctx->launches, extract::k_emit, NUM_SMS * 16, 128, 0, st, E);
         mark(ctx, "k_sa");
         extract::SaParams A{};
         A.rec = ctx->d_rec; A.clip = ctx->clip; A.var = ctx->d_var; A.task = b.task; A.contig = b.contig; A.n_contig = ctx->n_contig;
         A.sa_list = ctx->sa_list; A.n_sa = &ctr->n_sa; A.rec_end = ctx->rec_end; A.rec_nlead = ctx->rec_nlead; A.leads = E.leads; A.lead_cap = ctx->cap.lead; A.ctr = ctr; A.cfg = cf; A.seg_scratch = ctx->sa_seg;
-        extract::k_sa<<<extract::SA_BLOCKS, extract::SA_THREADS, 0, st>>>(A);
+        launch(ctx->launches, extract::k_sa, extract::SA_BLOCKS, extract::SA_THREADS, 0, st, A);
         mark(ctx, "k_task_nm");
         const int cpt = (int)((nrec + extract::NM_CHUNK - 1) / extract::NM_CHUNK);
-        extract::k_nm_partial<<<dim3(cpt, nt), 256, 0, st>>>(ctx->rec_flags, ctx->rec_nm, ctx->task_first, ctx->task_last, ctx->nm_part, ctx->nm_cnt);
-        extract::k_task_nm<<<nt, 256, 0, st>>>(ctx->task_first, ctx->task_last, ctx->nm_part, ctx->nm_cnt, cpt, ctx->task_nm); LAUNCHED(ctx, 8);
+        launch(ctx->launches, extract::k_nm_partial, dim3(cpt, nt), 256, 0, st, ctx->rec_flags, ctx->rec_nm, ctx->task_first, ctx->task_last, ctx->nm_part, ctx->nm_cnt);
+        launch(ctx->launches, extract::k_task_nm, nt, 256, 0, st, ctx->task_first, ctx->task_last, ctx->nm_part, ctx->nm_cnt, cpt, ctx->task_nm);
     }
     mark(ctx, "scan_rec_leads");
-    LAUNCHED(ctx, prims::exclusive_scan(ctx->rec_nlead, ctx->rec_lead_off, ctx->scan_tmp_r, nullptr, nrec, &ctr->n_leads, st));
+    prims::exclusive_scan(ctx->launches, ctx->rec_nlead, ctx->rec_lead_off, ctx->scan_tmp_r, nullptr, nrec, &ctr->n_leads, st);
     const unsigned long long nb = b.n_bound; const int g = grid_for(nb, 256);
     mark(ctx, "sort_leads");
-    cluster::k_scatter_keys<<<g, 256, 0, st>>>(b);
+    launch(ctx->launches, cluster::k_scatter_keys, g, 256, 0, st, b);
     prims::RadixTemp rt{ ctx->radix_hist, b.scan_tmp };
     bool first = true;
-    LAUNCHED(ctx, 1 + prims::radix_sort(b.key0, b.val0, b.key1, b.val1, rt, &ctr->n_leads, nb, cluster::TASK_SHIFT + bits_for(ctx->n_task), &first, st));
+    prims::radix_sort(ctx->launches, b.key0, b.val0, b.key1, b.val1, rt, &ctr->n_leads, nb, cluster::TASK_SHIFT + bits_for(ctx->n_task), &first, st);
     b.skey = first ? b.key0 : b.key1; b.sval = first ? b.val0 : b.val1;
     mark(ctx, "bins");
-    cluster::k_bin_heads<<<g, 256, 0, st>>>(b);
-    LAUNCHED(ctx, prims::exclusive_scan(b.flag, b.scan, b.scan_tmp, &ctr->n_leads, nb, &ctr->n_bins, st));
-    cluster::k_bin_build<<<g, 256, 0, st>>>(b);
-    cluster::k_bin_stats<<<g, 256, 0, st>>>(b); LAUNCHED(ctx, 3);
+    launch(ctx->launches, cluster::k_bin_heads, g, 256, 0, st, b);
+    prims::exclusive_scan(ctx->launches, b.flag, b.scan, b.scan_tmp, &ctr->n_leads, nb, &ctr->n_bins, st);
+    launch(ctx->launches, cluster::k_bin_build, g, 256, 0, st, b);
+    launch(ctx->launches, cluster::k_bin_stats, g, 256, 0, st, b);
     mark(ctx, nullptr);
     CUDA_TRY(cudaGetLastError());
     return 0;
@@ -767,43 +757,43 @@ static int enqueue_stage_b(snfb_ctx* ctx) {
     cluster::B& b = ctx->B; DevCounters* ctr = b.ctr; cudaStream_t st = ctx->st;
     const unsigned long long nb = b.n_bound; const int g = grid_for(nb, 128);
     mark(ctx, "kept_bins");
-    LAUNCHED(ctx, prims::exclusive_scan(b.bin_nl, b.kl_off, b.scan_tmp, &ctr->n_bins, nb, &ctr->n_kl, st));
-    LAUNCHED(ctx, prims::exclusive_scan(b.bin_nlong, b.kll_off, b.scan_tmp, &ctr->n_bins, nb, &ctr->n_kll, st));
-    LAUNCHED(ctx, prims::exclusive_scan(b.bin_kept, b.kb_idx, b.scan_tmp, &ctr->n_bins, nb, &ctr->n_kbins, st));
-    cluster::k_kbin_build<<<g, 128, 0, st>>>(b);
-    cluster::k_gather_kept<<<grid_for(nb, 256), 256, 0, st>>>(b);
+    prims::exclusive_scan(ctx->launches, b.bin_nl, b.kl_off, b.scan_tmp, &ctr->n_bins, nb, &ctr->n_kl, st);
+    prims::exclusive_scan(ctx->launches, b.bin_nlong, b.kll_off, b.scan_tmp, &ctr->n_bins, nb, &ctr->n_kll, st);
+    prims::exclusive_scan(ctx->launches, b.bin_kept, b.kb_idx, b.scan_tmp, &ctr->n_bins, nb, &ctr->n_kbins, st);
+    launch(ctx->launches, cluster::k_kbin_build, g, 128, 0, st, b);
+    launch(ctx->launches, cluster::k_gather_kept, grid_for(nb, 256), 256, 0, st, b);
     mark(ctx, "merge_chains");
-    cluster::k_seg_heads<<<g, 128, 0, st>>>(b);
-    LAUNCHED(ctx, prims::exclusive_scan(b.flag, b.scan, b.scan_tmp, &ctr->n_kbins, nb, &ctr->n_segs, st));
-    cluster::k_seg_build<<<g, 128, 0, st>>>(b);
-    cluster::k_merge<<<g, 128, 0, st>>>(b);
-    cluster::k_verify_cuts<<<g, 128, 0, st>>>(b);
-    LAUNCHED(ctx, prims::exclusive_scan(b.flag, b.scan, b.scan_tmp, &ctr->n_kbins, nb, &ctr->n_clusters, st));
-    cluster::k_cluster_build<<<g, 128, 0, st>>>(b);
+    launch(ctx->launches, cluster::k_seg_heads, g, 128, 0, st, b);
+    prims::exclusive_scan(ctx->launches, b.flag, b.scan, b.scan_tmp, &ctr->n_kbins, nb, &ctr->n_segs, st);
+    launch(ctx->launches, cluster::k_seg_build, g, 128, 0, st, b);
+    launch(ctx->launches, cluster::k_merge, g, 128, 0, st, b);
+    launch(ctx->launches, cluster::k_verify_cuts, g, 128, 0, st, b);
+    prims::exclusive_scan(ctx->launches, b.flag, b.scan, b.scan_tmp, &ctr->n_kbins, nb, &ctr->n_clusters, st);
+    launch(ctx->launches, cluster::k_cluster_build, g, 128, 0, st, b);
     mark(ctx, "cluster_call");
     // clusters too large for one warp's shared memory go to a block each, next to the warp-per-cluster kernel
     CUDA_TRY(cudaEventRecord(ctx->ev_fork, st)); CUDA_TRY(cudaStreamWaitEvent(ctx->st_side, ctx->ev_fork, 0));
-    cluster::k_cluster_block<<<NUM_SMS, cluster::CB_THREADS, cluster::CB_SMEM, ctx->st_side>>>(b);
-    cluster::k_cluster_warp<cluster::WARP_CAP, cluster::CWM_WARPS, true><<<NUM_SMS * 2, cluster::CWM_WARPS * 32, cluster::CwCfg<cluster::WARP_CAP, cluster::CWM_WARPS>::smem, ctx->st_side>>>(b);
+    launch(ctx->launches, cluster::k_cluster_block, NUM_SMS, cluster::CB_THREADS, cluster::CB_SMEM, ctx->st_side, b);
+    launch(ctx->launches, cluster::k_cluster_warp<cluster::WARP_CAP, cluster::CWM_WARPS, true>, NUM_SMS * 2, cluster::CWM_WARPS * 32, cluster::CwCfg<cluster::WARP_CAP, cluster::CWM_WARPS>::smem, ctx->st_side, b);
     CUDA_TRY(cudaEventRecord(ctx->ev_join, ctx->st_side));
-    cluster::k_cluster_warp<cluster::SMALL_CAP, cluster::CWS_WARPS, false><<<NUM_SMS * 4, cluster::CWS_WARPS * 32, cluster::CwCfg<cluster::SMALL_CAP, cluster::CWS_WARPS>::smem, st>>>(b);
+    launch(ctx->launches, cluster::k_cluster_warp<cluster::SMALL_CAP, cluster::CWS_WARPS, false>, NUM_SMS * 4, cluster::CWS_WARPS * 32, cluster::CwCfg<cluster::SMALL_CAP, cluster::CWS_WARPS>::smem, st, b);
     CUDA_TRY(cudaStreamWaitEvent(st, ctx->ev_join, 0));
     mark(ctx, "emit_cands");
-    LAUNCHED(ctx, prims::exclusive_scan(b.cl_nvalid, b.cl_cand_base, b.scan_tmp, &ctr->n_clusters, nb, &ctr->n_cand, st));
-    LAUNCHED(ctx, prims::exclusive_scan(b.cl_nlead, b.cl_lead_base, b.scan_tmp, &ctr->n_clusters, nb, &ctr->n_cand_leads, st));
-    LAUNCHED(ctx, prims::exclusive_scan(b.cl_nrn, b.cl_rn_base, b.scan_tmp, &ctr->n_clusters, nb, &ctr->n_rnames, st));
-    cluster::k_emit_cands<<<NUM_SMS * 8, 128, 0, st>>>(b);
+    prims::exclusive_scan(ctx->launches, b.cl_nvalid, b.cl_cand_base, b.scan_tmp, &ctr->n_clusters, nb, &ctr->n_cand, st);
+    prims::exclusive_scan(ctx->launches, b.cl_nlead, b.cl_lead_base, b.scan_tmp, &ctr->n_clusters, nb, &ctr->n_cand_leads, st);
+    prims::exclusive_scan(ctx->launches, b.cl_nrn, b.cl_rn_base, b.scan_tmp, &ctr->n_clusters, nb, &ctr->n_rnames, st);
+    launch(ctx->launches, cluster::k_emit_cands, NUM_SMS * 8, 128, 0, st, b);
     mark(ctx, "coverage");
-    if (ctx->n_mask) { cluster::k_mask_bp<<<grid_for((unsigned long long)ctx->n_mask * 32, 128), 128, 0, st>>>(b, ctx->b_mask_task.as<uint32_t>(), ctx->n_mask, ctx->task_cov); LAUNCHED(ctx, 1); }
-    cluster::k_coverage<<<NUM_SMS * 32, 128, 0, st>>>(b); LAUNCHED(ctx, 13);
+    if (ctx->n_mask) launch(ctx->launches, cluster::k_mask_bp, grid_for((unsigned long long)ctx->n_mask * 32, 128), 128, 0, st, b, ctx->b_mask_task.as<uint32_t>(), ctx->n_mask, ctx->task_cov);
+    launch(ctx->launches, cluster::k_coverage, NUM_SMS * 32, 128, 0, st, b);
     // consensus plan: best read per INS candidate, sizes and offsets of the ALT bytes and of the scratch; the candidate records are final after this
     consensus::C& c = ctx->Cc;
     CUDA_TRY(cudaMemsetAsync(c.work_ctr, 0, 64, st));
     mark(ctx, "consensus_plan");
-    consensus::k_plan<<<grid_for(ctx->cap.cand, 128), 128, 0, st>>>(c);
-    LAUNCHED(ctx, prims::exclusive_scan(c.alt_len, c.alt_off, b.scan_tmp, &ctr->n_cand, ctx->cap.cand, &ctr->n_alt_bytes, st));
-    LAUNCHED(ctx, prims::exclusive_scan(c.scr_len, c.scr_off, b.scan_tmp, &ctr->n_cand, ctx->cap.cand, &ctr->n_seq_bytes, st));
-    consensus::k_plan_finish<<<grid_for(ctx->cap.cand, 128), 128, 0, st>>>(c); LAUNCHED(ctx, 2);
+    launch(ctx->launches, consensus::k_plan, grid_for(ctx->cap.cand, 128), 128, 0, st, c);
+    prims::exclusive_scan(ctx->launches, c.alt_len, c.alt_off, b.scan_tmp, &ctr->n_cand, ctx->cap.cand, &ctr->n_alt_bytes, st);
+    prims::exclusive_scan(ctx->launches, c.scr_len, c.scr_off, b.scan_tmp, &ctr->n_cand, ctx->cap.cand, &ctr->n_seq_bytes, st);
+    launch(ctx->launches, consensus::k_plan_finish, grid_for(ctx->cap.cand, 128), 128, 0, st, c);
     mark(ctx, nullptr);
     CUDA_TRY(cudaGetLastError());
     return 0;
@@ -817,7 +807,7 @@ static int enqueue_stage_c(snfb_ctx* ctx) {
         // the device lists the base slices it will read, the host gathers exactly those bytes from its arena into pinned staging,
         // one H2D copy brings them in (PCIe bytes ~ algorithmic bytes instead of the whole arena).  This path needs the host in the loop.
         mark(ctx, "seq_requests");
-        consensus::k_seq_requests<<<grid_for(ctx->cap.cand, 128), 128, 0, st>>>(c, ctx->seq_req, ctx->cap.req, ctx->arena_off, &ctr->n_req, &ctr->n_req_units); LAUNCHED(ctx, 1);
+        launch(ctx->launches, consensus::k_seq_requests, grid_for(ctx->cap.cand, 128), 128, 0, st, c, ctx->seq_req, ctx->cap.req, ctx->arena_off, &ctr->n_req, &ctr->n_req_units);
         mark(ctx, nullptr);
         CUDA_TRY(cudaMemcpyAsync(ctx->h_fin, ctr, sizeof(DevCounters), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
@@ -840,11 +830,11 @@ static int enqueue_stage_c(snfb_ctx* ctx) {
         c.seq = ctx->seq_arena; c.arena_off = ctx->arena_off;
     }
     mark(ctx, "consensus");
-    consensus::k_prep<<<NUM_SMS * 8, 128, 0, st>>>(c);
+    launch(ctx->launches, consensus::k_prep, NUM_SMS * 8, 128, 0, st, c);
     mark(ctx, "consensus_align");
-    consensus::k_align<<<NUM_SMS * 7, consensus::ALIGN_WARPS * 32, 0, st>>>(c);
+    launch(ctx->launches, consensus::k_align, NUM_SMS * 7, consensus::ALIGN_WARPS * 32, 0, st, c);
     mark(ctx, "consensus_vote");
-    consensus::k_vote<<<NUM_SMS * 16, consensus::VOTE_THREADS, 0, st>>>(c); LAUNCHED(ctx, 3);
+    launch(ctx->launches, consensus::k_vote, NUM_SMS * 16, consensus::VOTE_THREADS, 0, st, c);
     mark(ctx, nullptr);
     CUDA_TRY(cudaGetLastError());
     return 0;
@@ -898,7 +888,7 @@ static int fill_lead_view(snfb_ctx* ctx, snfb_lead_view* out) {
     if (ctx->h_leads.ensure(sizeof(snfb_lead) * (nl + 1)) || ctx->h_task_reads.ensure(4 * nt) || ctx->h_task_nm.ensure(8 * nt) || ctx->h_rec_nm.ensure(8 * (ctx->n_rec + 1)))
         return fail(ctx, "out of memory for the lead view");
     if (nl) {
-        k_gather_leads<<<grid_for(nl, 256), 256, 0, ctx->st>>>(ctx->leads, ctx->B.sval, ctx->sorted_leads, &ctx->B.ctr->n_leads, ctx->cap.lead); LAUNCHED(ctx, 1);
+        launch(ctx->launches, k_gather_leads, grid_for(nl, 256), 256, 0, ctx->st, ctx->leads, ctx->B.sval, ctx->sorted_leads, &ctx->B.ctr->n_leads, ctx->cap.lead);
         CUDA_TRY(cudaMemcpyAsync(ctx->h_leads.p, ctx->sorted_leads, sizeof(snfb_lead) * nl, cudaMemcpyDeviceToHost, ctx->st));
     }
     CUDA_TRY(cudaMemcpyAsync(ctx->h_task_reads.p, ctx->task_reads, 4 * nt, cudaMemcpyDeviceToHost, ctx->st));
@@ -1041,12 +1031,6 @@ int snfb_device_alt(snfb_ctx* ctx, void** dptr, uint64_t* n_bytes) {
 uint64_t snfb_launch_count(snfb_ctx* ctx) { return ctx ? ctx->launches : 0; }
 double snfb_selftest_sqrt_frac(uint64_t p_hi, uint64_t p_lo, uint64_t q, int slow) { const u128 P = ((u128)p_hi << 64) | p_lo; return slow ? sqrt_frac_rn_slow(P, q) : sqrt_frac_rn(P, q); }
 uint64_t snfb_rerun_count(snfb_ctx* ctx) { return ctx ? ctx->reruns : 0; }
-/* developer aid (SNFB_DEBUG set when the ctx ran): per-warp timing of the consensus alignment kernel, 8 words per warp */
-int snfb_debug_dump(snfb_ctx* ctx, uint64_t* out, uint64_t n_words) {
-    if (!ctx || !ctx->Cc.dbg || !out) return 1;
-    const uint64_t have = (uint64_t)NUM_SMS * 8 * consensus::ALIGN_WARPS * 8; if (n_words > have) n_words = have;
-    return cudaMemcpy(out, ctx->Cc.dbg, 8 * n_words, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : 1;
-}
 int snfb_pin_host(void* p, size_t bytes) { return cudaHostRegister(p, bytes, cudaHostRegisterDefault) == cudaSuccess ? 0 : 1; }
 int snfb_unpin_host(void* p) { return cudaHostUnregister(p) == cudaSuccess ? 0 : 1; }
 
@@ -1096,9 +1080,9 @@ int snfb_allgather_candidates(snfb_ctx* ctx, uint32_t flags, snfb_gather_view* o
         if (ctx->b_gsend.ensure(cap + 256) || ctx->b_grecv.ensure((size_t)nr * cap + out_cap + 1024)) return fail(ctx, "out of device memory (gather)");
         uint8_t* recv = ctx->b_grecv.as<uint8_t>(); uint8_t* merged = recv + (((size_t)nr * cap + 255) & ~(size_t)255); unsigned long long* d_layout = reinterpret_cast<unsigned long long*>(merged + out_cap);     // layout words live behind the merged arrays
         mark(ctx, "allgather");
-        k_gather_pack<<<NUM_SMS * 4, 256, 0, st>>>(b.ctr, b.cand, ctx->Cc.alt, b.rnames, b.rn_off_out, b.cand_leads, with_leads, nr > 1 ? ctx->b_gsend.as<uint8_t>() : recv, cap); LAUNCHED(ctx, 1);
+        launch(ctx->launches, k_gather_pack, NUM_SMS * 4, 256, 0, st, b.ctr, b.cand, ctx->Cc.alt, b.rnames, b.rn_off_out, b.cand_leads, with_leads, nr > 1 ? ctx->b_gsend.as<uint8_t>() : recv, cap);
         if (nr > 1 && g_nccl.AllGather(ctx->b_gsend.p, recv, cap, 0 /* ncclChar */, ctx->comm, st) != 0) return fail(ctx, "ncclAllGather failed");
-        k_gather_merge<<<NUM_SMS * 4, 256, 0, st>>>(recv, cap, nr, with_leads, merged, out_cap, d_layout); LAUNCHED(ctx, 1);
+        launch(ctx->launches, k_gather_merge, NUM_SMS * 4, 256, 0, st, recv, cap, nr, with_leads, merged, out_cap, d_layout);
         mark(ctx, nullptr);
         CUDA_TRY(cudaMemcpyAsync(h_layout, d_layout, 64, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(h_hdr, recv, sizeof(GatherHdr), cudaMemcpyDeviceToHost, st));     // slot 0's header; the rest below
@@ -1163,7 +1147,7 @@ int snfb_poa(snfb_ctx* ctx, const snfb_poa_job* jobs, uint32_t n_jobs, const uin
     poa::Params P{}; P.jobs = d_jobs.as<poa::Job>(); P.n_jobs = n_jobs; P.seqs = d_seqs.as<uint8_t>(); P.offs = d_offs.as<int>(); P.out = d_out.as<uint8_t>(); P.out_len = d_len.as<int>();
     P.scratch = d_scr.as<uint8_t>(); P.scratch_per_block = smax; P.next_job = d_ctr.as<unsigned>();
     mark(ctx, "poa");
-    poa::k_poa<<<(unsigned)nblk, poa::THREADS, 0, st>>>(P); LAUNCHED(ctx, 1);
+    launch(ctx->launches, poa::k_poa, (unsigned)nblk, poa::THREADS, 0, st, P);
     mark(ctx, nullptr);
     cudaMemcpyAsync(out, d_out.p, out_bytes, cudaMemcpyDeviceToHost, st); cudaMemcpyAsync(out_len, d_len.p, 4 * (size_t)n_jobs, cudaMemcpyDeviceToHost, st);
     const cudaError_t e = cudaStreamSynchronize(st);
@@ -1226,7 +1210,7 @@ int snfb_combine_groups(snfb_ctx* ctx, const snfb_combine_in* in, snfb_combine_o
     if (use_alt) { up(P.alt, in->alt, in->n_alt_bytes); up(P.alt_off, in->alt_off, 8 * n); up(P.alt_len, in->alt_len, 4 * n); }
     cudaMemsetAsync(P.next_chain, 0, 16, st);
     mark(ctx, "combine_groups");
-    combine::k_combine<<<blocks, 128, 0, st>>>(P); LAUNCHED(ctx, 1);
+    launch(ctx->launches, combine::k_combine, blocks, 128, 0, st, P);
     mark(ctx, nullptr);
     cudaMemcpyAsync(out->cand_group, P.cand_group, 4 * n, cudaMemcpyDeviceToHost, st); cudaMemcpyAsync(out->emit_chunk, P.emit_chunk, 4 * n, cudaMemcpyDeviceToHost, st);
     cudaMemcpyAsync(out->emit_ord, P.emit_ord, 4 * n, cudaMemcpyDeviceToHost, st); cudaMemcpyAsync(out->cov_non, P.cov_non, 4 * n * S, cudaMemcpyDeviceToHost, st);
@@ -1250,7 +1234,7 @@ int snfb_selftest_edit_distance(snfb_ctx* ctx, const uint8_t* bytes, uint64_t n_
     cudaStream_t st = ctx->st;
     cudaMemcpyAsync(d_b.p, bytes, n_bytes, cudaMemcpyHostToDevice, st); cudaMemcpyAsync(ao, a_off, 8 * (size_t)n_pairs, cudaMemcpyHostToDevice, st); cudaMemcpyAsync(bo, b_off, 8 * (size_t)n_pairs, cudaMemcpyHostToDevice, st);
     cudaMemcpyAsync(al, a_len, 4 * (size_t)n_pairs, cudaMemcpyHostToDevice, st); cudaMemcpyAsync(bl, b_len, 4 * (size_t)n_pairs, cudaMemcpyHostToDevice, st);
-    combine::k_edit_selftest<<<blocks, 128, 0, st>>>(d_b.as<uint8_t>(), ao, al, bo, bl, n_pairs, d_hs.as<int8_t>(), max_len, d_out.as<int>()); LAUNCHED(ctx, 1);
+    launch(ctx->launches, combine::k_edit_selftest, blocks, 128, 0, st, d_b.as<uint8_t>(), ao, al, bo, bl, n_pairs, d_hs.as<int8_t>(), max_len, d_out.as<int>());
     cudaMemcpyAsync(out, d_out.p, 4 * (size_t)n_pairs, cudaMemcpyDeviceToHost, st);
     const cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return done(fail(ctx, std::string("snfb_selftest_edit_distance: ") + cudaGetErrorString(e)));
@@ -1271,7 +1255,7 @@ int snfb_coverage_bins(snfb_ctx* ctx, uint32_t task, int binsize, const double**
     uint32_t lohi[2];
     CUDA_TRY(cudaMemcpyAsync(&lohi[0], ctx->task_first + task, 4, cudaMemcpyDeviceToHost, ctx->st)); CUDA_TRY(cudaMemcpyAsync(&lohi[1], ctx->task_last + task, 4, cudaMemcpyDeviceToHost, ctx->st));
     CUDA_TRY(cudaStreamSynchronize(ctx->st));
-    if (nb && lohi[1] > lohi[0]) { k_cov_bins<<<grid_for(lohi[1] - lohi[0], 256), 256, 0, ctx->st>>>(ctx->rec_pos, ctx->rec_end, ctx->rec_flags, lohi[0], lohi[1], binsize, L, nb, acc.as<unsigned long long>()); LAUNCHED(ctx, 1); }
+    if (nb && lohi[1] > lohi[0]) launch(ctx->launches, k_cov_bins, grid_for(lohi[1] - lohi[0], 256), 256, 0, ctx->st, ctx->rec_pos, ctx->rec_end, ctx->rec_flags, lohi[0], lohi[1], binsize, L, nb, acc.as<unsigned long long>());
     unsigned long long* raw = reinterpret_cast<unsigned long long*>(ctx->h_cov_bins.as<uint8_t>() + 8 * (size_t)(nb + 1));
     CUDA_TRY(cudaMemcpyAsync(raw, acc.p, 8 * (size_t)nb, cudaMemcpyDeviceToHost, ctx->st));
     CUDA_TRY(cudaStreamSynchronize(ctx->st));

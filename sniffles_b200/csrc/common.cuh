@@ -13,6 +13,9 @@ constexpr int NUM_SMS = 132;
 
 #define CUDA_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { ctx_fail(ctx, #x, cudaGetErrorString(e_)); return 1; } } while (0)
 
+// every kernel of the library is launched here, so the launch counter n (snfb_launch_count) counts exactly the launches made
+template <class... P, class... A> inline void launch(uint64_t& n, void (*k)(P...), dim3 g, dim3 b, size_t smem, cudaStream_t st, A... a) { k<<<g, b, smem, st>>>(a...); ++n; }
+
 typedef unsigned __int128 u128;
 
 // ---------------------------------------------------------------- device-side run state

@@ -27,7 +27,6 @@ struct C {
     // item pipeline: one (candidate, supporting read) pair per warp, one (candidate, column tile) per block
     struct Item { uint32_t cand; uint32_t k; uint32_t row; uint32_t rd_off; };
     Item* items_big; Item* items_small; uint2* tiles; unsigned long long item_cap, tile_cap;
-    unsigned long long* dbg;          // optional (SNFB_DEBUG): per warp of k_align [busy cycles, end time, items, longest item cycles, its L, its Lo]
     DevCounters* ctr; snfb_config cfg;
 };
 
@@ -353,10 +352,8 @@ __global__ void __launch_bounds__(128) k_prep(C c) {
 
 // one (candidate, supporting read) item by the cooperating group g; hi / hj / hcl / run_st / run_len hold `cap` ints each
 template <typename G>
-__device__ __forceinline__ void align_item(const C& c, const C::Item it, const G g, int* hi, int* hj, int* hcl, int* run_st, int* run_len, int cap, unsigned long long* d_ph) {
+__device__ __forceinline__ void align_item(const C& c, const C::Item it, const G g, int* hi, int* hj, int* hcl, int* run_st, int* run_len, int cap) {
     const int tid = g.tid; constexpr int NT = G::NTHR; const int klen = 6;
-    long long d_pt = c.dbg ? clock64() : 0;
-    #define PHASE(k) if (c.dbg) { const long long n_ = clock64(); d_ph[k] += (unsigned long long)(n_ - d_pt); d_pt = n_; }
     const uint32_t ci = it.cand; const uint32_t L = c.alt_len[ci];
     if ((unsigned long long)c.scr_off[ci] + c.scr_len[ci] > c.scr_cap16) return;
     const snfb_cand* cd = &c.cand[ci];
@@ -369,7 +366,6 @@ __device__ __forceinline__ void align_item(const C& c, const C::Item it, const G
     const long skip = c.cfg.consensus_kmer_skip_base + (long)__dmul_rn((double)L, c.cfg.consensus_kmer_skip_seqlen_mult);
     unpack_lead(c, cd->lead_off + it.k, rd, tid, NT);
     g.sync();
-    PHASE(0)
     // (1) anchor hits in j order (table lives in global scratch, L2 resident); four k-mers per thread in flight
     int nh = 0;
     const long nk = Lo - klen > 0 ? (Lo - klen + skip - 1) / skip : 0;
@@ -395,7 +391,6 @@ __device__ __forceinline__ void align_item(const C& c, const C::Item it, const G
     }
     if (nh > cap) nh = cap;
     g.sync();
-    PHASE(1)
     // (2) anchor automaton (consensus.py:306-338) in closed form: a hit is accepted iff its i exceeds every earlier hit's i
     //     (the accepted hits are the left-to-right maxima), and len(conseq) before accepted hit m is
     //     min(L, c0 + j[m-1] - j[0]) because every step appends min(j step, room left).  Compacted in place.
@@ -416,7 +411,6 @@ __device__ __forceinline__ void align_item(const C& c, const C::Item it, const G
     long span = skip > 12 ? segments_pass<8>(hi, hj, hcl, na, c0, j0, (long)L, rd, best, tid, NT) : segments_pass<1>(hi, hj, hcl, na, c0, j0, (long)L, rd, best, tid, NT);
     span = g.sum(span);
     g.sync();
-    PHASE(2)
     // (3b) dash-free runs (= chains of copied segments) survive only with identity > 0.5 and more than 5 matches
     //      (consensus.py:343-360); decided on the segment list before anything is written.  A non-empty dashed segment
     //      ends a run; run ids are prefix counts of those, the per-run sums are accumulated in shared memory.
@@ -441,7 +435,6 @@ __device__ __forceinline__ void align_item(const C& c, const C::Item it, const G
         }
         g.sync();
     }
-    PHASE(3)
     // (3c) the row: every copied segment lands at row[cs + t] = rd[lj + t] with cs - lj = c0 - j0 for all of them, so the row is
     //      one shifted copy of the read between the first and the last anchor (coalesced words), dashes outside, and the
     //      rejected segments dashed afterwards
@@ -468,8 +461,6 @@ __device__ __forceinline__ void align_item(const C& c, const C::Item it, const G
     }
     if (tid == 0) acc[it.row] = __ddiv_rn((double)span, (double)L) > 0.2;
     g.sync();
-    PHASE(4)
-    #undef PHASE
 }
 
 // Heavy items (long insertions) first, the whole block on one item (the longest insertion's reads are the tail of the step);
@@ -479,30 +470,23 @@ __global__ void __launch_bounds__(ALIGN_WARPS * 32, 7) k_align(C c) {
     __shared__ int sm[5][ALIGN_WARPS * MAXHIT_LIGHT]; __shared__ int s_red[2 * ALIGN_WARPS]; __shared__ uint32_t s_q;
     static_assert(ALIGN_WARPS * MAXHIT_LIGHT >= MAXHIT, "a block item needs MAXHIT entries");
     const int lane = lane_id(), warp = threadIdx.x >> 5;
-    unsigned long long d_busy = 0, d_items = 0, d_ph[5] = { 0, 0, 0, 0, 0 }; const long long d_start = c.dbg ? clock64() : 0;
     const uint32_t nb = (uint32_t)min((unsigned long long)c.work_ctr[4], c.item_cap), ns = (uint32_t)min((unsigned long long)c.work_ctr[5], c.item_cap);
     for (;;) {
         __syncthreads();
         if (threadIdx.x == 0) s_q = atomicAdd(&c.work_ctr[6], 1u);
         __syncthreads();
         const uint32_t q = s_q; if (q >= nb) break;
-        const long long t0 = c.dbg ? clock64() : 0;
         BlockGrp<ALIGN_WARPS> g; g.tid = threadIdx.x; g.red = s_red;
-        align_item(c, c.items_big[q], g, sm[0], sm[1], sm[2], sm[3], sm[4], ALIGN_WARPS * MAXHIT_LIGHT, d_ph);
-        if (c.dbg) { d_busy += (unsigned long long)(clock64() - t0); if (warp == 0) ++d_items; }
+        align_item(c, c.items_big[q], g, sm[0], sm[1], sm[2], sm[3], sm[4], ALIGN_WARPS * MAXHIT_LIGHT);
     }
     __syncthreads();
     for (;;) {
         uint32_t q = 0; if (lane == 0) q = atomicAdd(&c.work_ctr[7], 1u);
         q = __shfl_sync(FULL, q, 0);
         if (q >= ns) break;
-        const long long t0 = c.dbg ? clock64() : 0;
         WarpGrp g; g.tid = lane; const int o = warp * MAXHIT_LIGHT;
-        align_item(c, c.items_small[q], g, sm[0] + o, sm[1] + o, sm[2] + o, sm[3] + o, sm[4] + o, MAXHIT_LIGHT, d_ph);
-        if (c.dbg) { d_busy += (unsigned long long)(clock64() - t0); ++d_items; }
+        align_item(c, c.items_small[q], g, sm[0] + o, sm[1] + o, sm[2] + o, sm[3] + o, sm[4] + o, MAXHIT_LIGHT);
     }
-    if (c.dbg && lane == 0) { unsigned long long* o = c.dbg + (size_t)(blockIdx.x * ALIGN_WARPS + warp) * 8;
-        o[0] = d_busy; o[1] = (unsigned long long)(clock64() - d_start); o[2] = d_items; o[3] = d_ph[0]; o[4] = d_ph[1]; o[5] = d_ph[2]; o[6] = d_ph[3]; o[7] = d_ph[4]; }
 }
 
 // column vote (consensus.py:365-380), one block per (candidate, 4096-column tile); every thread takes four adjacent columns

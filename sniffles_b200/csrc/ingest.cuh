@@ -2,9 +2,9 @@
 // Replaces the host decode behind `bam.fetch(contig, start, end)` (parallel.py:95-98, leadprov.py:488): only the BGZF bytes cross
 // PCIe; inflate, record decode, filtering to the task's region, the CG long-CIGAR escape and the CIGAR16 packing run here.
 //
-//   k_inflate<NL>  NL = 32 / 16 / 8 lanes per BGZF block (ingest_core.h inflate_stream<NL>; 16 by default): the Huffman tables of a block in
+//   k_inflate      16 lanes per BGZF block (ingest_core.h inflate_stream<16>): the Huffman tables of a block in
 //                  shared memory, the scalar decode executed redundantly by the block's lanes, match copies / table fills / stored blocks split
-//                  across them; two or four blocks share a warp's instruction stream wherever they run the same path
+//                  across them; the two blocks of a warp share its instruction stream wherever they run the same path
 //   k_walk         one thread per span (a record-aligned range of the inflated stream, cut at the BAI's linear-index anchors):
 //                  follows the block_size chain, first to count, then to write the record offsets
 //   k_parse        one thread per raw record: fixed fields, aux walk (NM, HP, PS, SA, CG), task filter on contig and end
@@ -23,27 +23,28 @@ struct Span { unsigned long long ubeg, uend; unsigned task; unsigned _pad; };   
 struct IngestCounters { unsigned long long bad_blocks, first_bad_block, first_bad_code, bad_chain, malformed, bad_cigar, n_raw, n_keep, n_groups, n_var, n_seq16; };
 
 constexpr int INF_WARPS = 8;
+// lanes per BGZF block: two blocks per warp (their decodes share the warp's instruction stream where they run the same path — a
+// literal-heavy stream mostly does — and diverge where they do not)
+constexpr int INF_LANES = 16;
+constexpr size_t INF_SMEM_BYTES = sizeof(WarpTables) * INF_WARPS * (32 / INF_LANES);      // one WarpTables per block being decoded
+static_assert(INF_SMEM_BYTES <= 48 * 1024, "k_inflate's tables must fit the default dynamic shared memory limit (48 KB)");
 
-// NL lanes per BGZF block: 32 = one block per warp, 16 / 8 = two / four blocks per warp (their decodes share the warp's instruction
-// stream where they run the same path — a literal-heavy stream mostly does — and diverge where they do not)
-template <int NL>
 __global__ void __launch_bounds__(INF_WARPS * 32) k_inflate(const uint8_t* __restrict__ comp, const BgzfBlock* __restrict__ blocks, unsigned n_blocks, uint8_t* __restrict__ raw, IngestCounters* ctr) {
     extern __shared__ __align__(16) uint8_t inflate_smem[];
-    constexpr int GPW = 32 / NL;                              // groups per warp
+    constexpr int GPW = 32 / INF_LANES;                       // groups per warp
     WarpTables* tables = reinterpret_cast<WarpTables*>(inflate_smem);
-    const int w = threadIdx.x >> 5, g = (threadIdx.x & 31) / NL, lane = (threadIdx.x & 31) % NL;
-    const unsigned gmask = NL == 32 ? 0xffffffffu : (((1u << (NL & 31)) - 1u) << (g * NL));
+    const int w = threadIdx.x >> 5, g = (threadIdx.x & 31) / INF_LANES, lane = (threadIdx.x & 31) % INF_LANES;
+    const unsigned gmask = ((1u << INF_LANES) - 1u) << (g * INF_LANES);
     WarpTables* T = tables + (w * GPW + g);
     const unsigned stride = gridDim.x * INF_WARPS * GPW;
     for (unsigned b = (blockIdx.x * INF_WARPS + w) * GPW + g; b < n_blocks; b += stride) {
         const BgzfBlock B = blocks[b];
         uint32_t produced = 0;
-        int rc = inflate_stream<NL>(comp, B.in_off, B.in_off + B.in_len, raw + B.out_off, B.isize, T, lane, gmask, &produced);
+        int rc = inflate_stream<INF_LANES>(comp, B.in_off, B.in_off + B.in_len, raw + B.out_off, B.isize, T, lane, gmask, &produced);
         if (rc == INF_OK && produced != B.isize) rc = INF_LENGTH_MISMATCH;
         if (rc != INF_OK && lane == 0) { if (atomicAdd(&ctr->bad_blocks, 1ULL) == 0) { ctr->first_bad_block = b; ctr->first_bad_code = (unsigned long long)rc; } }
     }
 }
-template <int NL> constexpr size_t inflate_smem_bytes() { return sizeof(WarpTables) * INF_WARPS * (32 / NL); }
 
 // mode 0: span_cnt[s] = records in the span; mode 1: rec_body[base[s] + k] / rec_bs / rec_task
 __global__ void k_walk(const uint8_t* __restrict__ raw, unsigned long long raw_len, const Span* __restrict__ spans, unsigned n_spans, int mode,

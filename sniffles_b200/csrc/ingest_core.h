@@ -7,7 +7,7 @@
 // address and broadcast), so no lane ever waits for a broadcast, and the parts that ARE data parallel — filling the look-up
 // tables, LZ77 match copies, stored blocks, byte copies — are split across the lanes.  With NL = 1 the same code is plain
 // sequential C++: tests/native/ingest_host.cpp compiles this header with g++ and checks it against zlib on the CPU (test
-// infrastructure).  The product instantiates NL = 32 inside kernels, and c16_convert<1> for the host CIGAR16 conversion (api.cu).
+// infrastructure).  The kernels instantiate inflate_stream<16> and c16_convert<32>, the host CIGAR16 conversion (api.cu) c16_convert<1>.
 #pragma once
 #include <stdint.h>
 #include "cigar16.h"            // also defines SNFB_HD

@@ -73,15 +73,14 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_scan_down(const uint32_t* __re
 }
 
 // exclusive scan of in[0..n) into out (may alias in); total (u64) to *total_out if not null.
-// tmp must hold ceil(n_bound / SCAN_TILE) u32.
-inline int exclusive_scan(const uint32_t* in, uint32_t* out, uint32_t* tmp, const unsigned long long* n_ptr, unsigned long long n_bound,
+// tmp must hold ceil(n_bound / SCAN_TILE) u32.  Launches are counted in `launches`.
+inline void exclusive_scan(uint64_t& launches, const uint32_t* in, uint32_t* out, uint32_t* tmp, const unsigned long long* n_ptr, unsigned long long n_bound,
                            unsigned long long* total_out, cudaStream_t st) {
-    if (n_bound == 0) { if (total_out) cudaMemsetAsync(total_out, 0, 8, st); return 0; }
+    if (n_bound == 0) { if (total_out) cudaMemsetAsync(total_out, 0, 8, st); return; }
     int ntiles = (int)((n_bound + SCAN_TILE - 1) / SCAN_TILE);
-    k_scan_reduce<<<ntiles, SCAN_THREADS, 0, st>>>(in, tmp, n_ptr, n_bound);
-    k_scan_tiles<<<1, SCAN_THREADS, 0, st>>>(tmp, ntiles, total_out);
-    k_scan_down<<<ntiles, SCAN_THREADS, 0, st>>>(in, out, tmp, n_ptr, n_bound);
-    return 3;
+    launch(launches, k_scan_reduce, ntiles, SCAN_THREADS, 0, st, in, tmp, n_ptr, n_bound);
+    launch(launches, k_scan_tiles, 1, SCAN_THREADS, 0, st, tmp, ntiles, total_out);
+    launch(launches, k_scan_down, ntiles, SCAN_THREADS, 0, st, in, out, tmp, n_ptr, n_bound);
 }
 inline size_t scan_tmp_elems(unsigned long long n_bound) { return (size_t)((n_bound + SCAN_TILE - 1) / SCAN_TILE) + 1; }
 
@@ -147,21 +146,20 @@ __global__ void __launch_bounds__(RS_THREADS) k_radix_scatter(const uint64_t* __
 struct RadixTemp { uint32_t* hist; uint32_t* scan_tmp; };
 inline size_t radix_hist_elems(unsigned long long n_bound) { return (size_t)256 * (size_t)((n_bound + RS_TILE - 1) / RS_TILE) + 256; }
 
-// sorts (k0,v0) by the key bits [0, bits); result ends in (k0,v0) when `*in_first` is true, else in (k1,v1)
-inline int radix_sort(uint64_t* k0, uint32_t* v0, uint64_t* k1, uint32_t* v1, RadixTemp tmp, const unsigned long long* n_ptr, unsigned long long n_bound,
+// sorts (k0,v0) by the key bits [0, bits); result ends in (k0,v0) when `*in_first` is true, else in (k1,v1).  Launches are counted in `launches`.
+inline void radix_sort(uint64_t& launches, uint64_t* k0, uint32_t* v0, uint64_t* k1, uint32_t* v1, RadixTemp tmp, const unsigned long long* n_ptr, unsigned long long n_bound,
                        int bits, bool* in_first, cudaStream_t st) {
-    *in_first = true; int launches = 0;
-    if (n_bound == 0) return 0;
+    *in_first = true;
+    if (n_bound == 0) return;
     int nblk = (int)((n_bound + RS_TILE - 1) / RS_TILE);
     for (int shift = 0; shift < bits; shift += 8) {
         const uint64_t* ki = *in_first ? k0 : k1; const uint32_t* vi = *in_first ? v0 : v1;
         uint64_t* ko = *in_first ? k1 : k0; uint32_t* vo = *in_first ? v1 : v0;
-        k_radix_hist<<<nblk, RS_THREADS, 0, st>>>(ki, tmp.hist, n_ptr, n_bound, shift, nblk);
-        launches += 2 + exclusive_scan(tmp.hist, tmp.hist, tmp.scan_tmp, nullptr, (unsigned long long)256 * nblk, nullptr, st);
-        k_radix_scatter<<<nblk, RS_THREADS, 0, st>>>(ki, vi, ko, vo, tmp.hist, n_ptr, n_bound, shift, nblk);
+        launch(launches, k_radix_hist, nblk, RS_THREADS, 0, st, ki, tmp.hist, n_ptr, n_bound, shift, nblk);
+        exclusive_scan(launches, tmp.hist, tmp.hist, tmp.scan_tmp, nullptr, (unsigned long long)256 * nblk, nullptr, st);
+        launch(launches, k_radix_scatter, nblk, RS_THREADS, 0, st, ki, vi, ko, vo, tmp.hist, n_ptr, n_bound, shift, nblk);
         *in_first = !*in_first;
     }
-    return launches;
 }
 
 }  // namespace prims
