@@ -328,7 +328,9 @@ int         snfb_run(snfb_ctx* ctx, snfb_lead_view* leads, snfb_cand_view* cands
  * (16 lanes of a warp per block), follows the block_size chain of every span, decodes the records, keeps those `bam.fetch(contig, start,
  * end)` would return for the span's task (task.contig is the BAM reference id), restores CIGARs of more than 65535 operations
  * from the CG:B,I tag, and writes snfb_rec + CIGAR16 + names/SA + 4-bit bases exactly as snfb_load_records expects them.
- * The BGZF CRC32 is not verified (a corrupt block is caught by the DEFLATE decoder or the inflated size).  Tables (tasks, contigs,
+ * Every block is checked as htslib checks it: its DEFLATE stream must decode, to exactly ISIZE bytes, whose CRC-32 equals the
+ * block's trailer; a failing block fails the call and the error names the lowest failing block, its code and its byte offset in
+ * `bgzf` (code 10 = CRC32 mismatch: a damaged block that still decodes).  Tables (tasks, contigs,
  * tandem repeats, N mask) have the meaning they have in snfb_records. */
 typedef struct snfb_bam_span {
     uint64_t cbeg, cend;      /* byte offsets of BGZF block starts inside bgzf[] */

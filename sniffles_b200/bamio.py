@@ -48,8 +48,14 @@ class BgzfReader:
         if bsize is None:
             raise ValueError("BGZF block without a BC field")
         cdata = self.f.read(bsize - 12 - xlen - 8)
-        self.f.read(8)
+        trailer = self.f.read(8)
         data = zlib.decompress(cdata, -15)
+        # the gzip trailer, checked as htslib checks it: a damaged block can still inflate to ISIZE bytes, but not to the same CRC-32
+        crc, isize = struct.unpack("<II", trailer) if len(trailer) == 8 else (None, None)
+        if isize != len(data):
+            raise ValueError(f"BGZF block at file offset {coffset}: inflated size {len(data)} differs from ISIZE {isize}")
+        if crc != zlib.crc32(data):
+            raise ValueError(f"BGZF block at file offset {coffset}: CRC32 mismatch")
         self._cache = (coffset, data, bsize)
         return data, bsize
 

@@ -438,7 +438,7 @@ static int walk_bgzf(snfb_ctx* ctx, const uint8_t* z, uint64_t n, std::vector<in
         while (e + 4 <= xend) { const uint32_t slen = z[e + 2] | (z[e + 3] << 8); if (z[e] == 66 && z[e + 1] == 67 && slen == 2 && e + 6 <= xend) bsize = (z[e + 4] | (z[e + 5] << 8)) + 1u; e += 4 + slen; }
         if (!bsize || bsize < 12 + xlen + 8 || o + bsize > n) return fail(ctx, "BGZF block without a BC field or truncated");
         ingest::BgzfBlock b; b.in_off = o + 12 + xlen; b.in_len = bsize - 12 - xlen - 8;
-        memcpy(&b.isize, z + o + bsize - 4, 4); b.out_off = uo;
+        memcpy(&b.crc, z + o + bsize - 8, 4); memcpy(&b.isize, z + o + bsize - 4, 4); b.out_off = uo; b._pad = 0;
         if (b.isize > 65536u) return fail(ctx, "BGZF block claims more than 64 KiB of data");
         blocks.push_back(b); cstart.push_back(o);
         uo += b.isize; o += bsize;
@@ -454,6 +454,13 @@ static int inflate_to_device(snfb_ctx* ctx, const uint8_t* z, uint64_t n, std::v
     CUDA_TRY(cudaMemsetAsync(ctx->b_comp.as<uint8_t>() + n, 0, 64, ctx->st));
     CUDA_TRY(cudaMemsetAsync(ctx->b_raw.as<uint8_t>() + *raw_len, 0, 64, ctx->st));
     return 0;
+}
+
+// the error of a k_inflate launch with failed blocks: their count, and the lowest failing block with its byte offset in the caller's buffer
+static int inflate_failed(snfb_ctx* ctx, const ingest::IngestCounters& hc, const std::vector<uint64_t>& cstart) {
+    const unsigned long long first = ~hc.first_bad_inv, b = first >> 8, code = first & 255u;
+    return fail(ctx, "inflate: " + std::to_string(hc.bad_blocks) + " BGZF block(s) failed to decode (first: block " + std::to_string(b) + ", code " + std::to_string(code)
+                     + (code == ingest::INF_CRC_MISMATCH ? ", CRC32 mismatch" : "") + ", at byte " + std::to_string(cstart[b]) + " of the buffer)");
 }
 
 int snfb_inflate_bgzf(snfb_ctx* ctx, const uint8_t* bgzf, uint64_t n_bytes, uint8_t* out, uint64_t out_cap, uint64_t* out_len) {
@@ -474,7 +481,7 @@ int snfb_inflate_bgzf(snfb_ctx* ctx, const uint8_t* bgzf, uint64_t n_bytes, uint
     ingest::IngestCounters hc;
     CUDA_TRY(cudaMemcpyAsync(&hc, d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, ctx->st));
     CUDA_TRY(cudaStreamSynchronize(ctx->st));
-    if (hc.bad_blocks) return fail(ctx, "inflate: " + std::to_string(hc.bad_blocks) + " BGZF block(s) failed to decode (first: block " + std::to_string(hc.first_bad_block) + ", code " + std::to_string(hc.first_bad_code) + ")");
+    if (hc.bad_blocks) return inflate_failed(ctx, hc, cstart);
     if (out) {
         if (out_cap < raw_len) return fail(ctx, "snfb_inflate_bgzf: output buffer too small");
         CUDA_TRY(cudaMemcpy(out, ctx->b_raw.p, raw_len, cudaMemcpyDeviceToHost));
@@ -536,7 +543,7 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
     ingest::IngestCounters* hc = ctx->h_ing.as<ingest::IngestCounters>();
     CUDA_TRY(cudaMemcpyAsync(hc, d_ctr, sizeof(*hc), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
-    if (hc->bad_blocks) return fail(ctx, "inflate: " + std::to_string(hc->bad_blocks) + " BGZF block(s) failed to decode (first: block " + std::to_string(hc->first_bad_block) + ", code " + std::to_string(hc->first_bad_code) + ")");
+    if (hc->bad_blocks) return inflate_failed(ctx, *hc, cstart);
     if (hc->bad_chain) return fail(ctx, "BAM record chain broken in " + std::to_string(hc->bad_chain) + " span(s): a span does not start or end on a record boundary, or the data is truncated");
     const uint64_t n_raw = hc->n_raw;
     if (n_raw >= (1ull << 28)) return fail(ctx, "too many records in one block (2^28)");

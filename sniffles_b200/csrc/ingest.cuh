@@ -4,7 +4,8 @@
 //
 //   k_inflate      16 lanes per BGZF block (ingest_core.h inflate_stream<16>): the Huffman tables of a block in
 //                  shared memory, the scalar decode executed redundantly by the block's lanes, match copies / table fills / stored blocks split
-//                  across them; the two blocks of a warp share its instruction stream wherever they run the same path
+//                  across them; the two blocks of a warp share its instruction stream wherever they run the same path; then the same
+//                  lanes check the block's CRC-32 (crc32_group<16>)
 //   k_walk         one thread per span (a record-aligned range of the inflated stream, cut at the BAI's linear-index anchors):
 //                  follows the block_size chain, first to count, then to write the record offsets
 //   k_parse        one thread per raw record: fixed fields, aux walk (NM, HP, PS, SA, CG), task filter on contig and end
@@ -18,21 +19,29 @@
 
 namespace ingest {
 
-struct BgzfBlock { unsigned long long in_off; unsigned in_len; unsigned isize; unsigned long long out_off; };      // DEFLATE payload in the compressed buffer, its inflated size, where it lands
+// DEFLATE payload in the compressed buffer, its inflated size and CRC-32 (the block's gzip trailer), where it lands
+struct BgzfBlock { unsigned long long in_off; unsigned in_len; unsigned isize; unsigned long long out_off; unsigned crc; unsigned _pad; };
 struct Span { unsigned long long ubeg, uend; unsigned task; unsigned _pad; };                                      // record-aligned range of the inflated stream owned by one task
-struct IngestCounters { unsigned long long bad_blocks, first_bad_block, first_bad_code, bad_chain, malformed, bad_cigar, n_raw, n_keep, n_groups, n_var, n_seq16; };
+// first_bad_inv = ~(block << 8 | INF_* code) of the lowest failing block: an atomicMax of the complement, so the zeroed counters need no
+// other initial value and the block reported does not depend on which group failed first
+struct IngestCounters { unsigned long long bad_blocks, first_bad_inv, bad_chain, malformed, bad_cigar, n_raw, n_keep, n_groups, n_var, n_seq16; };
 
 constexpr int INF_WARPS = 8;
 // lanes per BGZF block: two blocks per warp (their decodes share the warp's instruction stream where they run the same path — a
 // literal-heavy stream mostly does — and diverge where they do not)
 constexpr int INF_LANES = 16;
-constexpr size_t INF_SMEM_BYTES = sizeof(WarpTables) * INF_WARPS * (32 / INF_LANES);      // one WarpTables per block being decoded
+// the CRC tables once per thread block, then one WarpTables per block being decoded.  41,088 B: launch_inflate still sizes its grid for 5 thread blocks per SM
+constexpr size_t INF_SMEM_BYTES = sizeof(CrcTables) + sizeof(WarpTables) * INF_WARPS * (32 / INF_LANES);
 static_assert(INF_SMEM_BYTES <= 48 * 1024, "k_inflate's tables must fit the default dynamic shared memory limit (48 KB)");
 
+// every block is decoded, checked against its ISIZE, then against its CRC-32
 __global__ void __launch_bounds__(INF_WARPS * 32) k_inflate(const uint8_t* __restrict__ comp, const BgzfBlock* __restrict__ blocks, unsigned n_blocks, uint8_t* __restrict__ raw, IngestCounters* ctr) {
     extern __shared__ __align__(16) uint8_t inflate_smem[];
     constexpr int GPW = 32 / INF_LANES;                       // groups per warp
-    WarpTables* tables = reinterpret_cast<WarpTables*>(inflate_smem);
+    CrcTables* crc_tab = reinterpret_cast<CrcTables*>(inflate_smem);
+    WarpTables* tables = reinterpret_cast<WarpTables*>(inflate_smem + sizeof(CrcTables));
+    crc_tables_fill(crc_tab, threadIdx.x, blockDim.x);
+    __syncthreads();
     const int w = threadIdx.x >> 5, g = (threadIdx.x & 31) / INF_LANES, lane = (threadIdx.x & 31) % INF_LANES;
     const unsigned gmask = ((1u << INF_LANES) - 1u) << (g * INF_LANES);
     WarpTables* T = tables + (w * GPW + g);
@@ -42,7 +51,8 @@ __global__ void __launch_bounds__(INF_WARPS * 32) k_inflate(const uint8_t* __res
         uint32_t produced = 0;
         int rc = inflate_stream<INF_LANES>(comp, B.in_off, B.in_off + B.in_len, raw + B.out_off, B.isize, T, lane, gmask, &produced);
         if (rc == INF_OK && produced != B.isize) rc = INF_LENGTH_MISMATCH;
-        if (rc != INF_OK && lane == 0) { if (atomicAdd(&ctr->bad_blocks, 1ULL) == 0) { ctr->first_bad_block = b; ctr->first_bad_code = (unsigned long long)rc; } }
+        if (rc == INF_OK && crc32_group<INF_LANES>(raw + B.out_off, B.isize, crc_tab, lane, gmask) != B.crc) rc = INF_CRC_MISMATCH;
+        if (rc != INF_OK && lane == 0) { atomicAdd(&ctr->bad_blocks, 1ULL); atomicMax(&ctr->first_bad_inv, ~(((unsigned long long)b << 8) | (unsigned)rc)); }
     }
 }
 

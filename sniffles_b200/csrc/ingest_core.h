@@ -6,8 +6,9 @@
 // the same values (bit buffer, positions, symbols live in registers, identical in every lane; table look-ups hit one shared-memory
 // address and broadcast), so no lane ever waits for a broadcast, and the parts that ARE data parallel — filling the look-up
 // tables, LZ77 match copies, stored blocks, byte copies — are split across the lanes.  With NL = 1 the same code is plain
-// sequential C++: tests/native/ingest_host.cpp compiles this header with g++ and checks it against zlib on the CPU (test
-// infrastructure).  The kernels instantiate inflate_stream<16> and c16_convert<32>, the host CIGAR16 conversion (api.cu) c16_convert<1>.
+// sequential C++: tests/native/ingest_host.cpp and crc_host.cpp compile this header with g++ and check it against zlib on the CPU (test
+// infrastructure).  The kernels instantiate inflate_stream<16>, crc32_group<16> and c16_convert<32>, the host CIGAR16 conversion (api.cu)
+// c16_convert<1>.
 #pragma once
 #include <stdint.h>
 #include "cigar16.h"            // also defines SNFB_HD
@@ -75,7 +76,8 @@ struct WarpTables {
     uint8_t lens[320];                          // code lengths being read
 };
 
-enum { INF_OK = 0, INF_BAD_BLOCK_TYPE = 1, INF_BAD_STORED = 2, INF_BAD_CODE = 3, INF_OVERSUBSCRIBED = 4, INF_BAD_SYMBOL = 5, INF_BAD_DISTANCE = 6, INF_OUTPUT_OVERRUN = 7, INF_INPUT_OVERRUN = 8, INF_LENGTH_MISMATCH = 9 };
+enum { INF_OK = 0, INF_BAD_BLOCK_TYPE = 1, INF_BAD_STORED = 2, INF_BAD_CODE = 3, INF_OVERSUBSCRIBED = 4, INF_BAD_SYMBOL = 5, INF_BAD_DISTANCE = 6, INF_OUTPUT_OVERRUN = 7, INF_INPUT_OVERRUN = 8, INF_LENGTH_MISMATCH = 9,
+       INF_CRC_MISMATCH = 10 };
 
 // A decoding group = NL lanes of a warp (NL = 32: the whole warp; NL = 16 / 8: two / four BGZF blocks per warp, each decoded by its own
 // lanes with its own tables — the groups share the warp's instruction stream wherever they happen to take the same path, and
@@ -275,6 +277,103 @@ SNFB_HD int inflate_stream(const uint8_t* in, uint64_t ipos, uint64_t iend, uint
     *out_len = op;
     if (!err && (ovr || 4u * iw - (uint32_t)(bc >> 3) > iend_rel)) err = INF_INPUT_OVERRUN;
     return err;
+}
+
+// ---------------------------------------------------------------- CRC-32 of an inflated block (the gzip trailer every BGZF block carries)
+// zlib's CRC-32: reflected polynomial 0xEDB88320, initial value and final XOR 0xFFFFFFFF.  A DEFLATE stream can be damaged and still
+// decode to ISIZE bytes (any byte of a stored block, many bit flips in a Huffman-coded one); the CRC is what catches those, as htslib does.
+constexpr uint32_t CRC_POLY = 0xEDB88320u;
+struct CrcTables {
+    uint32_t t[4][256];         // slice-by-4: t[k][b] = CRC register after byte b followed by k zero bytes
+    uint32_t x8pow[32];         // x^(8 * 2^k) mod P: multiplying by it moves a CRC past 2^k bytes
+};
+SNFB_HD uint32_t crc_byte_step(uint32_t c) { for (int k = 0; k < 8; ++k) c = (c >> 1) ^ (CRC_POLY & (0u - (c & 1u))); return c; }
+// fill the tables with threads tid = 0 .. nthreads - 1 (the caller synchronises them before use)
+SNFB_HD void crc_tables_fill(CrcTables* C, int tid, int nthreads) {
+    for (int i = tid; i < 256; i += nthreads) {
+        uint32_t c = crc_byte_step((uint32_t)i); C->t[0][i] = c;
+        for (int k = 1; k < 4; ++k) { c = (c >> 8) ^ crc_byte_step(c & 0xffu); C->t[k][i] = c; }
+    }
+    if (tid == 0) {
+        // x^8 squared k times, in the reflected representation (x^0 = 0x80000000); zlib's x2n_table from its entry 3 on
+        const uint32_t x8pow[32] = { 0x00800000u, 0x00008000u, 0xedb88320u, 0xb1e6b092u, 0xa06a2517u, 0xed627daeu, 0x88d14467u, 0xd7bbfe6au,
+                                     0xec447f11u, 0x8e7ea170u, 0x6427800eu, 0x4d47bae0u, 0x09fe548fu, 0x83852d0fu, 0x30362f1au, 0x7b5a9cc3u,
+                                     0x31fec169u, 0x9fec022au, 0x6c8dedc4u, 0x15d6874du, 0x5fde7a4eu, 0xbad90e37u, 0x2e4e5eefu, 0x4eaba214u,
+                                     0xa8a472c0u, 0x429a969eu, 0x148d302au, 0xc40ba6d0u, 0xc4e22c3cu, 0x40000000u, 0x20000000u, 0x08000000u };
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+        for (int k = 0; k < 32; ++k) C->x8pow[k] = x8pow[k];
+    }
+}
+// a * b mod P in the reflected representation (zlib's multmodp): at most 32 steps, fewer when a's low-order terms are zero
+SNFB_HD uint32_t crc_multmodp(uint32_t a, uint32_t b) {
+    uint32_t p = 0;
+    for (uint32_t m = 1u << 31; m; m >>= 1) {
+        if (a & m) { p ^= b; if (!(a & (m - 1u))) break; }
+        b = (b >> 1) ^ (CRC_POLY & (0u - (b & 1u)));
+    }
+    return p;
+}
+// CRC of A || B from crc(A), crc(B) and len(B) (zlib's crc32_combine): crc(A) times x^(8 len(B)), plus crc(B)
+SNFB_HD uint32_t crc32_combine(uint32_t crc_a, uint32_t crc_b, uint32_t len_b, const uint32_t* x8pow) {
+    uint32_t xn = 1u << 31;
+    for (int k = 0; len_b; ++k, len_b >>= 1) if (len_b & 1u) xn = crc_multmodp(x8pow[k], xn);
+    return crc_multmodp(xn, crc_a) ^ crc_b;
+}
+SNFB_HD uint32_t crc_word_step(uint32_t c, const CrcTables* C) { return C->t[3][c & 0xffu] ^ C->t[2][(c >> 8) & 0xffu] ^ C->t[1][(c >> 16) & 0xffu] ^ C->t[0][c >> 24]; }
+SNFB_HD uint32_t ld32a(const uint8_t* p) {            // 4-byte aligned load
+#if defined(__CUDA_ARCH__)
+    return *reinterpret_cast<const uint32_t*>(p);
+#else
+    uint32_t v; memcpy(&v, p, 4); return v;
+#endif
+}
+struct U32x4 { uint32_t x, y, z, w; };
+SNFB_HD U32x4 ld128a(const uint8_t* p) {             // 16-byte aligned load
+#if defined(__CUDA_ARCH__)
+    const uint4 v = *reinterpret_cast<const uint4*>(p);
+    return { v.x, v.y, v.z, v.w };
+#else
+    U32x4 v; memcpy(&v, p, 16); return v;
+#endif
+}
+// CRC-32 of p[0 .. n), p at any alignment: bytes up to the first 16-byte boundary, then one 16-byte load per four table steps, then
+// words, then bytes
+SNFB_HD uint32_t crc32_slice(const uint8_t* p, uint32_t n, const CrcTables* C) {
+    uint32_t c = 0xffffffffu, i = 0;
+    for (; i < n && ((uintptr_t)(p + i) & 15u); ++i) c = (c >> 8) ^ C->t[0][(c ^ p[i]) & 0xffu];
+    for (; i + 16u <= n; i += 16u) {
+        const U32x4 v = ld128a(p + i);
+        c = crc_word_step(c ^ v.x, C); c = crc_word_step(c ^ v.y, C); c = crc_word_step(c ^ v.z, C); c = crc_word_step(c ^ v.w, C);
+    }
+    for (; i + 4u <= n; i += 4u) c = crc_word_step(c ^ ld32a(p + i), C);
+    for (; i < n; ++i) c = (c >> 8) ^ C->t[0][(c ^ p[i]) & 0xffu];
+    return ~c;
+}
+SNFB_HD uint32_t group_shfl_xor(uint32_t v, int d, unsigned gmask) {
+#if defined(__CUDA_ARCH__)
+    return __shfl_xor_sync(gmask, v, d);
+#else
+    (void)d; (void)gmask; return v;
+#endif
+}
+// CRC-32 of out[0 .. n) by the NL lanes of a decoding group; every lane calls it and every lane gets the result.  Each lane takes one
+// contiguous slice (whole 256-byte units, so that the lengths joined below have few set bits), and the slices' CRCs are joined in
+// log2(NL) butterfly steps: the lower half of each pair is A, the upper half B.
+template <int NL>
+SNFB_HD uint32_t crc32_group(const uint8_t* out, uint32_t n, const CrcTables* C, int lane, unsigned gmask) {
+    group_sync(gmask);                                 // the bytes were written by every lane of the group
+    const uint32_t per = ((n + NL - 1) / NL + 255u) & ~255u;
+    const uint32_t beg = (uint32_t)lane * per < n ? (uint32_t)lane * per : n, end = n - beg > per ? beg + per : n;
+    uint32_t crc = crc32_slice(out + beg, end - beg, C), len = end - beg;
+    for (int d = 1; d < NL; d <<= 1) {
+        const uint32_t o_crc = group_shfl_xor(crc, d, gmask), o_len = group_shfl_xor(len, d, gmask);
+        const bool upper = (lane & d) != 0;
+        crc = crc32_combine(upper ? o_crc : crc, upper ? crc : o_crc, upper ? len : o_len, C->x8pow);
+        len += o_len;
+    }
+    return crc;
 }
 
 // ---------------------------------------------------------------- BAM records (SAM spec §4.2)
