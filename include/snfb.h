@@ -353,6 +353,13 @@ int         snfb_ingest_fetch(snfb_ctx* ctx, snfb_rec* rec, uint16_t* cigar16, u
 /* inflate whole BGZF blocks on the device and return the inflated stream (tests / inspection).  Returns 0 and *out_len = bytes;
  * out may be NULL to get the size only. */
 int         snfb_inflate_bgzf(snfb_ctx* ctx, const uint8_t* bgzf, uint64_t n_bytes, uint8_t* out, uint64_t out_cap, uint64_t* out_len);
+/* compress host bytes in[0 .. n_in) into BGZF on the device and return the members in host memory (what `bgzip` / pysam.tabix_index
+ * write for a .vcf.gz): the input is cut into blocks of 0xff00 bytes (the last may be shorter), each an independent gzip member with the
+ * BC extra field, one DEFLATE block (stored, fixed or dynamic Huffman, whichever is smallest) and the CRC-32 + ISIZE trailer.  The bytes
+ * are a pure function of the input.  out_cap must be at least ceil(n_in / 0xff00) * 65536; *out_len = bytes written; coffset[k] (may be
+ * NULL) = byte offset of member k in out.  The BGZF EOF marker is not appended.  Device buffers belong to the context and grow on
+ * demand; n_in is limited to 65535 blocks (~4 GiB) per call.  Records a "deflate" timing mark (snfb_last_timings). */
+int         snfb_deflate_bgzf(snfb_ctx* ctx, const uint8_t* in, uint64_t n_in, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* coffset);
 /* device-time accounting of the last run: per-kernel milliseconds from CUDA events on
  * the ctx stream; names[i] is a static string.  Returns the number of entries. */
 int         snfb_last_timings(snfb_ctx* ctx, const char** names, float* ms, uint64_t* bytes, int cap);

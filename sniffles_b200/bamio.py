@@ -418,6 +418,115 @@ def pack_records(contigs, recs, tasks, with_seq=True, tandem_repeats=None) -> Re
                        tr=np.asarray(tr_flat, dtype="<i4"), contig_names=names, aligned_bp=0)
 
 
+def bin_index(records, n_ref):
+    """The BAI-layout tables of coordinate-sorted records (SAM spec §5.2; tabix uses the same layout): `records` yields (ref, beg, end, v0,
+    v1) = the reference index, the 0-based half-open interval and the virtual offsets of the record's first byte and of the byte after it.
+    Returns per reference (bins, linear index, stats): bins = {bin: [(v0, v1) chunks]} in order of first use, adjacent chunks of a bin
+    merged; the linear index = per 16 kb window the smallest v0 of a record overlapping it, empty windows inheriting the previous offset;
+    stats = [first v0, last v1, record count] (pseudo-bin 37450), first v0 None for a reference without records."""
+    tabs = [({}, [], [None, None, 0]) for _ in range(n_ref)]
+    for rid, pos, end, v0, v1 in records:
+        bins, lin, st = tabs[rid]
+        ch = bins.setdefault(reg2bin(pos, end), [])
+        if ch and ch[-1][1] == v0:
+            ch[-1] = (ch[-1][0], v1)
+        else:
+            ch.append((v0, v1))
+        for w in range(pos >> 14, ((end - 1) >> 14) + 1):
+            while len(lin) <= w:
+                lin.append(0)
+            if lin[w] == 0:
+                lin[w] = v0
+        st[0] = v0 if st[0] is None else st[0]
+        st[1] = v1
+        st[2] += 1
+    for _, lin, _ in tabs:
+        for w in range(1, len(lin)):                   # empty windows inherit the previous offset
+            if lin[w] == 0:
+                lin[w] = lin[w - 1]
+    return tabs
+
+
+def _bai_ref_bytes(bins, lin, st) -> bytes:
+    """one reference of a BAI / TBI index: bins with their chunks, the pseudo-bin 37450, the linear index"""
+    out = [struct.pack("<i", len(bins) + (1 if st[2] else 0))]
+    for b, ch in bins.items():
+        out.append(struct.pack("<Ii", b, len(ch)) + b"".join(struct.pack("<QQ", v0, v1) for v0, v1 in ch))
+    if st[2]:
+        out.append(struct.pack("<Ii", 37450, 2) + struct.pack("<QQ", st[0], st[1]) + struct.pack("<QQ", st[2], 0))
+    out.append(struct.pack("<i", len(lin)) + struct.pack(f"<{len(lin)}Q", *lin))
+    return b"".join(out)
+
+
+_TBI_MAX = 1 << 29                                     # TBI's bins cover [0, 2^29)
+
+
+def _vcf_interval(fields):
+    """0-based half-open interval of a VCF line as htslib's tbx_parse1 derives it for the VCF preset (htslib tbx.c): beg = POS - 1;
+    end = beg + len(REF), replaced by INFO END= (at the start of INFO or after a ';') when present and not '.', or by beg + 1 when that
+    END <= beg"""
+    beg = int(fields[1]) - 1
+    end = beg + len(fields[3]) if len(fields) > 3 else beg + 1
+    info = fields[7] if len(fields) > 7 else ""
+    s = info[4:] if info.startswith("END=") else (info.split(";END=", 1)[1] if ";END=" in info else None)
+    if s and s[0] != ".":
+        k = 1 if s[0] in "+-" else 0
+        while k < len(s) and s[k].isdigit():
+            k += 1
+        if k and s[:k] not in "+-":
+            e = int(s[:k])
+            end = e if e > beg else beg + 1
+    return beg, end
+
+
+def tabix_index(text: bytes, coffsets) -> bytes:
+    """The uncompressed body of the .tbi index (tabix spec) of a VCF whose text was cut into BGZF members of 0xff00 bytes starting at
+    the file offsets `coffsets` — what `pysam.tabix_index(..., preset="vcf")` writes.  Byte u of the text has the virtual offset
+    coffsets[u // 0xff00] << 16 | u % 0xff00; the end of a text that fills its last block is (last block << 16 | 0xff00), as htslib's
+    bgzf_tell reports it.  Lines starting with '#' are skipped; intervals follow _vcf_interval.  Raises ValueError, naming the line, for a
+    contig that reappears after another one, a POS below the previous POS of the contig, or an interval beyond 2^29 — the input tabix
+    refuses."""
+    blk = 0xff00
+
+    def voff(u):
+        k = u // blk
+        if k == len(coffsets) and k and u % blk == 0:
+            return (coffsets[k - 1] << 16) | blk
+        return (coffsets[k] << 16) | (u % blk)
+    names, ids, placed = [], {}, []
+    last_rid, last_beg = -1, -1
+    u, n = 0, len(text)
+    lineno = 0
+    while u < n:
+        e = text.find(b"\n", u)
+        e = n if e < 0 else e + 1
+        line = text[u:e].rstrip(b"\r\n")
+        lineno += 1
+        if line and not line.startswith(b"#"):
+            f = line.decode().split("\t")
+            try:
+                beg, end = _vcf_interval(f)
+            except (ValueError, IndexError):
+                raise ValueError(f"line {lineno}: cannot parse the position of {line[:80]!r}") from None
+            rid = ids.get(f[0])
+            if rid is None:
+                rid = ids[f[0]] = len(names)
+                names.append(f[0])
+            elif rid != last_rid:
+                raise ValueError(f"line {lineno}: contig {f[0]!r} reappears after {names[last_rid]!r}: the VCF is not sorted ({line[:80]!r})")
+            if rid == last_rid and beg < last_beg:
+                raise ValueError(f"line {lineno}: POS {beg + 1} after POS {last_beg + 1} on {f[0]!r}: the VCF is not sorted ({line[:80]!r})")
+            if beg < 0 or end > _TBI_MAX:
+                raise ValueError(f"line {lineno}: interval {beg}..{end} on {f[0]!r} lies outside the 2^29 range of a TBI index ({line[:80]!r})")
+            placed.append((rid, beg, end, voff(u), voff(e)))
+            last_rid, last_beg = rid, beg
+        u = e
+    nm = b"".join(x.encode() + b"\0" for x in names)
+    out = [b"TBI\1", struct.pack("<8i", len(names), 2, 1, 2, 0, ord("#"), 0, len(nm)), nm]   # n_ref, VCF preset: format, col_seq/beg/end, meta, skip
+    out += [_bai_ref_bytes(*t) for t in bin_index(placed, len(names))]
+    return b"".join(out)
+
+
 # ------------------------------------------------------------------------------------------------ writer (tests / benchmark inputs)
 def _bgzf_block(data: bytes, level: int = 6) -> bytes:
     c = zlib.compressobj(level, zlib.DEFLATED, -15)
@@ -439,8 +548,7 @@ def write_bam(path, blk: RecordBlock, block_bytes=0xff00, level=6, qual_seed=Non
         head += struct.pack("<i", len(n) + 1) + n.encode() + b"\0" + struct.pack("<i", int(c["length"]))
     out = open(path, "wb")
     buf, coff = bytearray(), 0
-    index_tabs = [({}, []) for _ in names]
-    stats = [[None, None, 0] for _ in names]
+    placed = []                                        # (ref, beg, end, v0, v1) of every record
 
     def flush():
         nonlocal buf, coff
@@ -503,32 +611,15 @@ def write_bam(path, blk: RecordBlock, block_bytes=0xff00, level=6, qual_seed=Non
         else:
             buf += data
         v1 = (coff << 16) | len(buf)
-        bins, lin = index_tabs[rid]
-        ch = bins.setdefault(reg2bin(pos, end), [])
-        if ch and ch[-1][1] == v0:
-            ch[-1] = (ch[-1][0], v1)
-        else:
-            ch.append((v0, v1))
-        for w in range(pos >> 14, ((end - 1) >> 14) + 1):
-            while len(lin) <= w:
-                lin.append(0)
-            if lin[w] == 0:
-                lin[w] = v0
-        st = stats[rid]
-        st[0] = v0 if st[0] is None else st[0]
-        st[1] = v1
-        st[2] += 1
+        placed.append((rid, pos, end, v0, v1))
     flush()
     out.write(_BGZF_EOF)
     out.close()
-    for _, lin in index_tabs:
-        for w in range(1, len(lin)):                   # empty windows inherit the previous offset
-            if lin[w] == 0:
-                lin[w] = lin[w - 1]
+    tabs = bin_index(placed, len(names))
     if index == "csi":
         body = b"CSI\1" + struct.pack("<iii", 14, 5, 0) + struct.pack("<i", len(names))
         level_first = [((1 << (3 * l)) - 1) // 7 for l in range(6)]
-        for (bins, lin), st in zip(index_tabs, stats):
+        for bins, lin, st in tabs:
             body += struct.pack("<i", len(bins) + (1 if st[2] else 0))
             for b, ch in bins.items():
                 lvl = max(l for l in range(6) if level_first[l] <= b)
@@ -542,15 +633,5 @@ def write_bam(path, blk: RecordBlock, block_bytes=0xff00, level=6, qual_seed=Non
             f.write(_BGZF_EOF)
         return path, path + ".csi"
     with open(path + ".bai", "wb") as f:
-        f.write(b"BAI\1" + struct.pack("<i", len(names)))
-        for (bins, lin), st in zip(index_tabs, stats):
-            nb = len(bins) + (1 if st[2] else 0)
-            f.write(struct.pack("<i", nb))
-            for b, ch in bins.items():
-                f.write(struct.pack("<Ii", b, len(ch)))
-                for v0, v1 in ch:
-                    f.write(struct.pack("<QQ", v0, v1))
-            if st[2]:
-                f.write(struct.pack("<Ii", 37450, 2) + struct.pack("<QQ", st[0], st[1]) + struct.pack("<QQ", st[2], 0))
-            f.write(struct.pack("<i", len(lin)) + struct.pack(f"<{len(lin)}Q", *lin))
+        f.write(b"BAI\1" + struct.pack("<i", len(names)) + b"".join(_bai_ref_bytes(*t) for t in tabs))
     return path, path + ".bai"

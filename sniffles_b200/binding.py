@@ -17,7 +17,7 @@ EXPORTS = ["snfb_version", "snfb_sizeof", "snfb_hash_name", "snfb_ctx_create", "
            "snfb_last_timings", "snfb_device_candidates", "snfb_device_alt", "snfb_launch_count",
            "snfb_pin_host", "snfb_unpin_host", "snfb_pack_cigar16", "snfb_rerun_count", "snfb_coverage_bins",
            "snfb_nccl_unique_id", "snfb_comm_init", "snfb_allgather_candidates", "snfb_selftest_sqrt_frac", "snfb_poa", "snfb_combine_groups", "snfb_selftest_edit_distance",
-           "snfb_load_bam", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf"]
+           "snfb_load_bam", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf", "snfb_deflate_bgzf"]
 
 
 def lib():
@@ -42,6 +42,7 @@ def lib():
         L.snfb_ingest_sizes.argtypes = [C.c_void_p, C.c_void_p]
         L.snfb_ingest_fetch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.snfb_inflate_bgzf.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+        L.snfb_deflate_bgzf.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.c_void_p]
         L.snfb_extract_leads.argtypes = [C.c_void_p, C.POINTER(abi.LeadView)]
         L.snfb_cluster_call.argtypes = [C.c_void_p, C.POINTER(abi.CandView)]
         L.snfb_consensus.argtypes = [C.c_void_p, C.POINTER(abi.SeqView)]
@@ -208,6 +209,16 @@ class Context:
         out = np.zeros(max(int(n.value), 1), "u1")
         self._check(self._lib.snfb_inflate_bgzf(self._h, bgzf.ctypes.data, len(bgzf), out.ctypes.data, len(out), C.byref(n)), "snfb_inflate_bgzf")
         return out[:int(n.value)].tobytes()
+
+    def deflate_bgzf(self, data) -> tuple:
+        """bytes -> (BGZF members, their byte offsets), compressed on the device (snfb_deflate_bgzf); no EOF marker is appended"""
+        src = np.frombuffer(bytes(data), "u1")
+        nb = (len(src) + 0xff00 - 1) // 0xff00
+        out = np.empty(max(nb * 65536, 1), "u1")
+        coff = np.zeros(max(nb, 1), "<u8")
+        n = C.c_uint64()
+        self._check(self._lib.snfb_deflate_bgzf(self._h, src.ctypes.data, len(src), out.ctypes.data, len(out), C.byref(n), coff.ctypes.data), "snfb_deflate_bgzf")
+        return out[:int(n.value)].tobytes(), [int(x) for x in coff[:nb]]
 
     def run(self, want_leads=True, want_cands=True, want_seqs=True, copy=True) -> Result:
         lv, cv, sv = abi.LeadView(), abi.CandView(), abi.SeqView()

@@ -25,6 +25,7 @@
 #include "poa.cuh"
 #include "combine.cuh"
 #include "ingest.cuh"
+#include "bgzf_write.cuh"
 
 struct DevBuf {
     void* p = nullptr; size_t cap = 0;
@@ -97,6 +98,7 @@ struct snfb_ctx {
     DevBuf b_rec, b_cigar, b_var, b_seq, b_task, b_contig, b_tr, b_trp, b_mask, b_mask_off, b_mask_task;
     HostBuf h_c16, h_rec16;        // BAM32 host input converted to CIGAR16 before the upload
     DevBuf b_comp, b_raw, b_ing; HostBuf h_ing; uint64_t ing_sizes[8] = {0, 0, 0, 0, 0, 0, 0, 0}; bool from_bam = false;      // device BAM ingest: BGZF bytes, inflated stream, work arrays
+    DevBuf b_zin, b_zslot, b_zout, b_zwork;          // BGZF compression: input bytes, 64 KiB member slots, packed members, sizes / offsets / candidate scratch
     std::vector<snfb_task> tasks;
     // capacities and the three arenas carved by them
     Caps cap; bool force_no_cuts = false;
@@ -257,6 +259,7 @@ int snfb_ctx_create(int device, snfb_ctx** out) {
     cudaFuncSetAttribute(cluster::k_cluster_warp<cluster::SMALL_CAP, cluster::CWS_WARPS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cluster::CwCfg<cluster::SMALL_CAP, cluster::CWS_WARPS>::smem);
     cudaFuncSetAttribute(cluster::k_cluster_warp<cluster::WARP_CAP, cluster::CWM_WARPS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cluster::CwCfg<cluster::WARP_CAP, cluster::CWM_WARPS>::smem);
     cudaFuncSetAttribute(cluster::k_cluster_block, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cluster::CB_SMEM);
+    cudaFuncSetAttribute(bgzfw::k_deflate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bgzfw::DEF_SMEM_BYTES);
     *out = ctx; return 0;
 }
 
@@ -266,7 +269,8 @@ void snfb_ctx_destroy(snfb_ctx* ctx) {
     cudaStreamSynchronize(ctx->st); cudaStreamSynchronize(ctx->st_copy); cudaStreamSynchronize(ctx->st_side);
     if (ctx->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(ctx->comm);
     DevBuf* bufs[] = { &ctx->b_rec, &ctx->b_cigar, &ctx->b_var, &ctx->b_seq, &ctx->b_task, &ctx->b_contig, &ctx->b_tr, &ctx->b_trp, &ctx->b_mask, &ctx->b_mask_off, &ctx->b_mask_task,
-                       &ctx->b_ctr, &ctx->arena_r, &ctx->arena_l, &ctx->arena_c, &ctx->b_gsend, &ctx->b_grecv, &ctx->b_comp, &ctx->b_raw, &ctx->b_ing };
+                       &ctx->b_ctr, &ctx->arena_r, &ctx->arena_l, &ctx->arena_c, &ctx->b_gsend, &ctx->b_grecv, &ctx->b_comp, &ctx->b_raw, &ctx->b_ing,
+                       &ctx->b_zin, &ctx->b_zslot, &ctx->b_zout, &ctx->b_zwork };
     for (DevBuf* b : bufs) b->release();
     HostBuf* hb[] = { &ctx->h_c16, &ctx->h_rec16, &ctx->h_seq_req, &ctx->h_seq_arena, &ctx->h_ctr_buf, &ctx->h_leads, &ctx->h_task_reads, &ctx->h_task_nm, &ctx->h_rec_nm, &ctx->h_cand, &ctx->h_cand_leads,
                       &ctx->h_rnames, &ctx->h_rn_off, &ctx->h_task_cov, &ctx->h_task_cov_raw, &ctx->h_alt, &ctx->h_cov_bins, &ctx->h_gather, &ctx->h_ing };
@@ -486,6 +490,46 @@ int snfb_inflate_bgzf(snfb_ctx* ctx, const uint8_t* bgzf, uint64_t n_bytes, uint
         if (out_cap < raw_len) return fail(ctx, "snfb_inflate_bgzf: output buffer too small");
         CUDA_TRY(cudaMemcpy(out, ctx->b_raw.p, raw_len, cudaMemcpyDeviceToHost));
     }
+    return 0;
+}
+
+int snfb_deflate_bgzf(snfb_ctx* ctx, const uint8_t* in, uint64_t n_in, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* coffset) {
+    if (!ctx || !out_len || (n_in && (!in || !out))) return 1;
+    cudaSetDevice(ctx->device);
+    const uint64_t nb = (n_in + deflate::BLOCK_IN - 1) / deflate::BLOCK_IN;
+    if (nb > 65535) return fail(ctx, "snfb_deflate_bgzf: more than 65535 BGZF blocks (~4 GiB) in one call: split the input");
+    if (out_cap < nb * deflate::MEMBER_MAX) return fail(ctx, "snfb_deflate_bgzf: out_cap must be at least ceil(n_in / 0xff00) * 65536");
+    ctx->n_ev = 0;
+    *out_len = 0;
+    if (nb == 0) return 0;
+    const unsigned grid = (unsigned)std::min<uint64_t>(nb, (uint64_t)NUM_SMS);
+    Carver m; uint32_t* sizes = m.take<uint32_t>(nb + 1); uint32_t* offs = m.take<uint32_t>(nb + 1); uint32_t* tmp = m.take<uint32_t>(prims::scan_tmp_elems(nb));
+    unsigned long long* total = m.take<unsigned long long>(1); uint16_t* scratch = m.take<uint16_t>(2ull * deflate::BLOCK_IN * grid);
+    if (ctx->b_zin.ensure(n_in + 64) || ctx->b_zslot.ensure(nb * deflate::MEMBER_MAX) || ctx->b_zout.ensure(nb * deflate::MEMBER_MAX) || ctx->b_zwork.ensure(m.off + 256))
+        return fail(ctx, "out of device memory (BGZF compression)");
+    m.base = ctx->b_zwork.as<uint8_t>(); m.off = 0;
+    sizes = m.take<uint32_t>(nb + 1); offs = m.take<uint32_t>(nb + 1); tmp = m.take<uint32_t>(prims::scan_tmp_elems(nb));
+    total = m.take<unsigned long long>(1); scratch = m.take<uint16_t>(2ull * deflate::BLOCK_IN * grid);
+    cudaStream_t st = ctx->st;
+    mark(ctx, "h2d_deflate", n_in);
+    CUDA_TRY(cudaMemcpyAsync(ctx->b_zin.p, in, n_in, cudaMemcpyHostToDevice, st));
+    mark(ctx, "deflate", n_in);
+    launch(ctx->launches, bgzfw::k_deflate, grid, bgzfw::DEF_THREADS, bgzfw::DEF_SMEM_BYTES, st, ctx->b_zin.as<const uint8_t>(), (unsigned long long)n_in, (unsigned)nb, scratch,
+           ctx->b_zslot.as<uint8_t>(), sizes);
+    prims::exclusive_scan(ctx->launches, sizes, offs, tmp, nullptr, nb, total, st);
+    launch(ctx->launches, bgzfw::k_pack, (unsigned)std::min<uint64_t>(nb, (uint64_t)NUM_SMS * 16), 256, 0, st, ctx->b_zslot.as<const uint8_t>(), sizes, offs, (unsigned)nb, ctx->b_zout.as<uint8_t>());
+    mark(ctx, "d2h_deflate", 0);
+    unsigned long long n_out = 0;
+    std::vector<uint32_t> h_offs(nb);
+    CUDA_TRY(cudaMemcpyAsync(&n_out, total, sizeof(n_out), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(h_offs.data(), offs, 4 * nb, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaMemcpyAsync(out, ctx->b_zout.p, n_out, cudaMemcpyDeviceToHost, st));
+    mark(ctx, nullptr);
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaGetLastError());
+    if (coffset) for (uint64_t k = 0; k < nb; ++k) coffset[k] = h_offs[k];
+    *out_len = n_out;
     return 0;
 }
 

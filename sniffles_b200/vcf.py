@@ -13,7 +13,10 @@ reference's `VCF.write_header` / `VCF.write_call` (/root/reference/src/sniffles/
 
 The FASTA reader is any object with `fetch(contig, start, end) -> str` (pysam.FastaFile duck type); none is needed for
 symbolic / sequence-free output.  Genotype columns follow format_genotype (vcf.py:50-79)."""
+import io
 from collections import Counter
+
+from . import bamio
 
 AMBIGUOUS = str.maketrans("RYSWKMBDHV", "N" * 10)          # util.py:169-170
 
@@ -214,3 +217,45 @@ class VCFWriter:
                                              call.qual if call.qual is not None else ".", call.filter, ";".join(parts), self.genotype_format] + cols))
         self.call_count += 1
         return 1
+
+
+class BgzfIndexedOutput:
+    """Text handle for a `--vcf out.vcf.gz` (sniffles:229-244, :573-584): VCFWriter writes into it unchanged; `close()` compresses the
+    text into BGZF members with `compress(bytes) -> (members, coffsets)` (binding.Context.deflate_bgzf on the product path), then writes
+    `path` (members + the BGZF EOF marker) and `path + ".tbi"` (bamio.tabix_index, compressed the same way) — the pair
+    `pysam.tabix_index(..., preset="vcf")` leaves.  When the index refuses the text (unsorted lines, a reappearing contig, a position
+    beyond 2^29) the ValueError propagates and neither file is written."""
+
+    def __init__(self, path, compress):
+        self.path, self.compress = path, compress
+        self._buf = io.StringIO()
+
+    def write(self, text):
+        return self._buf.write(text)
+
+    def close(self):
+        if self._buf is None:
+            return
+        text = self._buf.getvalue().encode()
+        self._buf = None
+        z, coffsets = self.compress(text)
+        tbi, _ = self.compress(bamio.tabix_index(text, coffsets))
+        with open(self.path, "wb") as f:
+            f.write(z + bamio._BGZF_EOF)
+        with open(self.path + ".tbi", "wb") as f:
+            f.write(tbi + bamio._BGZF_EOF)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, exc_type, exc, tb):
+        if exc_type is None:
+            self.close()
+
+
+def open_output(config, ctx):
+    """the handle VCFWriter writes `config.vcf` through: a plain text file, or for a .gz / .bgz name (config.vcf_output_bgz) a
+    BgzfIndexedOutput compressed on the device of `ctx` (sniffles:250, :575-583)"""
+    if not config.vcf_output_bgz:
+        return open(config.vcf, "w")
+    return BgzfIndexedOutput(config.vcf, ctx.deflate_bgzf)
