@@ -27,37 +27,38 @@
 #include "ingest.cuh"
 #include "bgzf_write.cuh"
 
-struct DevBuf {
+// one owning allocation of device memory, or of pinned host memory when Pinned; freed by the destructor
+template <bool Pinned> struct Buf {
     void* p = nullptr; size_t cap = 0;
+    Buf() = default;
+    Buf(const Buf&) = delete; Buf& operator=(const Buf&) = delete;
+    ~Buf() { release(); }
+    // grows only; the old allocation is freed before the new one is made, so the peak holds one of them
     int ensure(size_t bytes) {
         if (bytes <= cap) return 0;
-        if (p) cudaFree(p);
-        p = nullptr; cap = 0;
+        release();
         size_t want = bytes + bytes / 8 + 256;
-        if (cudaMalloc(&p, want) != cudaSuccess) { p = nullptr; cudaGetLastError(); return 1; }
+        if ((Pinned ? cudaMallocHost(&p, want) : cudaMalloc(&p, want)) != cudaSuccess) { p = nullptr; cudaGetLastError(); return 1; }
         cap = want; return 0;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <class T> T* as() { return reinterpret_cast<T*>(p); }
+private:
+    void release() { if (p) { if (Pinned) cudaFreeHost(p); else cudaFree(p); } p = nullptr; cap = 0; }
 };
-struct HostBuf {
-    void* p = nullptr; size_t cap = 0;
-    int ensure(size_t bytes) {
-        if (bytes <= cap) return 0;
-        if (p) cudaFreeHost(p);
-        p = nullptr; cap = 0;
-        size_t want = bytes + bytes / 8 + 256;
-        if (cudaMallocHost(&p, want) != cudaSuccess) { p = nullptr; cudaGetLastError(); return 1; }
-        cap = want; return 0;
-    }
-    void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
-    template <class T> T* as() { return reinterpret_cast<T*>(p); }
-};
+using DevBuf = Buf<false>;
+using HostBuf = Buf<true>;
 // one allocation carved into 256-byte aligned arrays: a measuring pass, then an assigning pass over the same list
 struct Carver {
     uint8_t* base = nullptr; size_t off = 0;
     template <class T> T* take(size_t n) { const size_t o = off; off += (n * sizeof(T) + 255) & ~(size_t)255; return base ? reinterpret_cast<T*>(base + o) : nullptr; }
 };
+// runs the layout lay(Carver&) to measure, grows buf to fit, runs it again over buf to assign the pointers; nonzero when out of memory
+template <bool Pinned, class Lay> static int carve(Buf<Pinned>& buf, Lay&& lay) {
+    Carver m; lay(m);
+    if (buf.ensure(m.off + 256)) return 1;
+    Carver a; a.base = buf.template as<uint8_t>(); lay(a);
+    return 0;
+}
 
 constexpr int MAX_TIMINGS = 64;
 
@@ -97,13 +98,12 @@ struct snfb_ctx {
     const snfb_rec* d_rec = nullptr; const uint16_t* d_cigar = nullptr; const uint8_t* d_var = nullptr; const uint8_t* d_seq = nullptr;
     DevBuf b_rec, b_cigar, b_var, b_seq, b_task, b_contig, b_tr, b_trp, b_mask, b_mask_off, b_mask_task;
     HostBuf h_c16, h_rec16;        // BAM32 host input converted to CIGAR16 before the upload
-    DevBuf b_comp, b_raw, b_ing; HostBuf h_ing; uint64_t ing_sizes[8] = {0, 0, 0, 0, 0, 0, 0, 0}; bool from_bam = false;      // device BAM ingest: BGZF bytes, inflated stream, work arrays
+    DevBuf b_comp, b_raw, b_ing, b_ing_work; HostBuf h_ing; uint64_t ing_sizes[8] = {0, 0, 0, 0, 0, 0, 0, 0}; bool from_bam = false;      // device BAM ingest: BGZF bytes, inflated stream, block / span tables, per-raw-record work arrays
     DevBuf b_zin, b_zslot, b_zout, b_zwork;          // BGZF compression: input bytes, 64 KiB member slots, packed members, sizes / offsets / candidate scratch
     std::vector<snfb_task> tasks;
     // capacities and the three arenas carved by them
     Caps cap; bool force_no_cuts = false;
     DevBuf b_ctr, arena_r, arena_l, arena_c;            // counters; per-record arrays; per-lead arrays (stages A + B); stage C
-    uint64_t arena_r_for = 0, arena_r_cigar = 0; Caps arena_l_for, arena_c_for; uint32_t arena_r_tasks = 0;
     // per-record (arena_r)
     int32_t* rec_pos; int32_t* rec_end; uint8_t* rec_flags; double* rec_nm; uint32_t* rec_nlead; uint32_t* rec_lead_off; uint32_t* sa_list; extract::RecScan* scanrec; extract::RecClip* clip; int32_t* rec_big;
     uint32_t* task_first; uint32_t* task_last; uint32_t* task_reads; unsigned long long* task_cov; int32_t* task_span; double* task_nm; double* nm_part; unsigned* nm_cnt; extract::Seg* sa_seg; uint32_t* scan_tmp_r;
@@ -118,7 +118,7 @@ struct snfb_ctx {
     HostBuf h_ctr_buf; DevCounters* h_mid = nullptr; DevCounters* h_fin = nullptr; uint32_t* h_work = nullptr;
     HostBuf h_leads, h_task_reads, h_task_nm, h_rec_nm, h_cand, h_cand_leads, h_rnames, h_rn_off, h_task_cov, h_task_cov_raw, h_alt, h_cov_bins;
     // gather
-    void* comm = nullptr; int rank = 0, nranks = 1; DevBuf b_gsend, b_grecv; HostBuf h_gather; unsigned long long gather_cap = 0;
+    void* comm = nullptr; int rank = 0, nranks = 1; DevBuf b_gsend, b_grecv; HostBuf h_gather, h_gather_out; unsigned long long gather_cap = 0;     // h_gather: layout words, header table, rank_n_cand; h_gather_out: the merged arrays
     // timings
     cudaEvent_t ev[MAX_TIMINGS + 1]; const char* ev_name[MAX_TIMINGS + 1]; uint64_t ev_bytes[MAX_TIMINGS + 1]; int n_ev = 0; int n_ev_load = 0; uint64_t launches = 0; uint64_t reruns = 0;
 };
@@ -268,17 +268,10 @@ void snfb_ctx_destroy(snfb_ctx* ctx) {
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->st); cudaStreamSynchronize(ctx->st_copy); cudaStreamSynchronize(ctx->st_side);
     if (ctx->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(ctx->comm);
-    DevBuf* bufs[] = { &ctx->b_rec, &ctx->b_cigar, &ctx->b_var, &ctx->b_seq, &ctx->b_task, &ctx->b_contig, &ctx->b_tr, &ctx->b_trp, &ctx->b_mask, &ctx->b_mask_off, &ctx->b_mask_task,
-                       &ctx->b_ctr, &ctx->arena_r, &ctx->arena_l, &ctx->arena_c, &ctx->b_gsend, &ctx->b_grecv, &ctx->b_comp, &ctx->b_raw, &ctx->b_ing,
-                       &ctx->b_zin, &ctx->b_zslot, &ctx->b_zout, &ctx->b_zwork };
-    for (DevBuf* b : bufs) b->release();
-    HostBuf* hb[] = { &ctx->h_c16, &ctx->h_rec16, &ctx->h_seq_req, &ctx->h_seq_arena, &ctx->h_ctr_buf, &ctx->h_leads, &ctx->h_task_reads, &ctx->h_task_nm, &ctx->h_rec_nm, &ctx->h_cand, &ctx->h_cand_leads,
-                      &ctx->h_rnames, &ctx->h_rn_off, &ctx->h_task_cov, &ctx->h_task_cov_raw, &ctx->h_alt, &ctx->h_cov_bins, &ctx->h_gather, &ctx->h_ing };
-    for (HostBuf* b : hb) b->release();
     for (int i = 0; i <= MAX_TIMINGS; ++i) cudaEventDestroy(ctx->ev[i]);
     cudaEventDestroy(ctx->ev_b); cudaEventDestroy(ctx->ev_mid); cudaEventDestroy(ctx->ev_fork); cudaEventDestroy(ctx->ev_join);
     cudaStreamDestroy(ctx->st_side); cudaStreamDestroy(ctx->st_copy); cudaStreamDestroy(ctx->st);
-    delete ctx;
+    delete ctx;      // frees every buffer
 }
 
 const char* snfb_last_error(snfb_ctx* ctx) { return ctx ? ctx->err.c_str() : "null context"; }
@@ -475,8 +468,8 @@ int snfb_inflate_bgzf(snfb_ctx* ctx, const uint8_t* bgzf, uint64_t n_bytes, uint
     if (inflate_to_device(ctx, bgzf, n_bytes, cstart, blocks, &raw_len)) return 1;
     *out_len = raw_len;
     const size_t nb = blocks.size();
-    if (ctx->b_ing.ensure(256 + sizeof(ingest::BgzfBlock) * (nb + 1))) return fail(ctx, "out of device memory (ingest tables)");
-    ingest::IngestCounters* d_ctr = ctx->b_ing.as<ingest::IngestCounters>(); ingest::BgzfBlock* d_blk = reinterpret_cast<ingest::BgzfBlock*>(ctx->b_ing.as<uint8_t>() + 256);
+    ingest::IngestCounters* d_ctr = nullptr; ingest::BgzfBlock* d_blk = nullptr;
+    if (carve(ctx->b_ing, [&](Carver& c) { d_ctr = c.take<ingest::IngestCounters>(1); d_blk = c.take<ingest::BgzfBlock>(nb + 1); })) return fail(ctx, "out of device memory (ingest tables)");
     CUDA_TRY(cudaMemsetAsync(d_ctr, 0, sizeof(ingest::IngestCounters), ctx->st));
     CUDA_TRY(cudaMemcpyAsync(d_blk, blocks.data(), sizeof(ingest::BgzfBlock) * nb, cudaMemcpyHostToDevice, ctx->st));
     mark(ctx, "inflate", n_bytes + raw_len);
@@ -503,13 +496,11 @@ int snfb_deflate_bgzf(snfb_ctx* ctx, const uint8_t* in, uint64_t n_in, uint8_t* 
     *out_len = 0;
     if (nb == 0) return 0;
     const unsigned grid = (unsigned)std::min<uint64_t>(nb, (uint64_t)NUM_SMS);
-    Carver m; uint32_t* sizes = m.take<uint32_t>(nb + 1); uint32_t* offs = m.take<uint32_t>(nb + 1); uint32_t* tmp = m.take<uint32_t>(prims::scan_tmp_elems(nb));
-    unsigned long long* total = m.take<unsigned long long>(1); uint16_t* scratch = m.take<uint16_t>(2ull * deflate::BLOCK_IN * grid);
-    if (ctx->b_zin.ensure(n_in + 64) || ctx->b_zslot.ensure(nb * deflate::MEMBER_MAX) || ctx->b_zout.ensure(nb * deflate::MEMBER_MAX) || ctx->b_zwork.ensure(m.off + 256))
+    uint32_t *sizes = nullptr, *offs = nullptr, *tmp = nullptr; unsigned long long* total = nullptr; uint16_t* scratch = nullptr;
+    auto lay = [&](Carver& c) { sizes = c.take<uint32_t>(nb + 1); offs = c.take<uint32_t>(nb + 1); tmp = c.take<uint32_t>(prims::scan_tmp_elems(nb));
+                                total = c.take<unsigned long long>(1); scratch = c.take<uint16_t>(2ull * deflate::BLOCK_IN * grid); };
+    if (ctx->b_zin.ensure(n_in + 64) || ctx->b_zslot.ensure(nb * deflate::MEMBER_MAX) || ctx->b_zout.ensure(nb * deflate::MEMBER_MAX) || carve(ctx->b_zwork, lay))
         return fail(ctx, "out of device memory (BGZF compression)");
-    m.base = ctx->b_zwork.as<uint8_t>(); m.off = 0;
-    sizes = m.take<uint32_t>(nb + 1); offs = m.take<uint32_t>(nb + 1); tmp = m.take<uint32_t>(prims::scan_tmp_elems(nb));
-    total = m.take<unsigned long long>(1); scratch = m.take<uint16_t>(2ull * deflate::BLOCK_IN * grid);
     cudaStream_t st = ctx->st;
     mark(ctx, "h2d_deflate", n_in);
     CUDA_TRY(cudaMemcpyAsync(ctx->b_zin.p, in, n_in, cudaMemcpyHostToDevice, st));
@@ -566,12 +557,11 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
         spans[i].ubeg = ub; spans[i].uend = ue; spans[i].task = sp.task; spans[i]._pad = 0;
     }
     if (upload_tables(ctx, &T)) return 1;
-    // fixed part of the work area
-    Carver m0; ingest::IngestCounters* d_ctr = nullptr; ingest::BgzfBlock* d_blk = nullptr; ingest::Span* d_span = nullptr; uint32_t* span_cnt = nullptr; uint32_t* span_base = nullptr; uint32_t* scan_tmp0 = nullptr;
-    auto carve0 = [&](Carver& c) { d_ctr = c.take<ingest::IngestCounters>(1); d_blk = c.take<ingest::BgzfBlock>(nb + 1); d_span = c.take<ingest::Span>(ns + 1); span_cnt = c.take<uint32_t>(ns + 1); span_base = c.take<uint32_t>(ns + 1); scan_tmp0 = c.take<uint32_t>(prims::scan_tmp_elems(ns + 1) + 16); };
-    carve0(m0);
-    if (ctx->b_ing.ensure(m0.off + 256)) return fail(ctx, "out of device memory (ingest tables)");
-    { Carver a; a.base = ctx->b_ing.as<uint8_t>(); carve0(a); }
+    // counters, block and span tables
+    ingest::IngestCounters* d_ctr = nullptr; ingest::BgzfBlock* d_blk = nullptr; ingest::Span* d_span = nullptr; uint32_t* span_cnt = nullptr; uint32_t* span_base = nullptr; uint32_t* scan_tmp0 = nullptr;
+    if (carve(ctx->b_ing, [&](Carver& c) { d_ctr = c.take<ingest::IngestCounters>(1); d_blk = c.take<ingest::BgzfBlock>(nb + 1); d_span = c.take<ingest::Span>(ns + 1); span_cnt = c.take<uint32_t>(ns + 1);
+                                           span_base = c.take<uint32_t>(ns + 1); scan_tmp0 = c.take<uint32_t>(prims::scan_tmp_elems(ns + 1) + 16); }))
+        return fail(ctx, "out of device memory (ingest tables)");
     cudaStream_t st = ctx->st; const uint8_t* raw = ctx->b_raw.as<uint8_t>();
     CUDA_TRY(cudaMemsetAsync(d_ctr, 0, sizeof(ingest::IngestCounters), st));
     CUDA_TRY(cudaMemcpyAsync(d_blk, blocks.data(), sizeof(ingest::BgzfBlock) * nb, cudaMemcpyHostToDevice, st));
@@ -591,19 +581,11 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
     if (hc->bad_chain) return fail(ctx, "BAM record chain broken in " + std::to_string(hc->bad_chain) + " span(s): a span does not start or end on a record boundary, or the data is truncated");
     const uint64_t n_raw = hc->n_raw;
     if (n_raw >= (1ull << 28)) return fail(ctx, "too many records in one block (2^28)");
-    // per-raw-record work arrays live behind the fixed part
+    // per-raw-record work arrays
     ingest::RawRec* recs = nullptr; uint32_t *keep = nullptr, *idx = nullptr, *groups = nullptr, *grp_off = nullptr, *var16 = nullptr, *var_off = nullptr, *seq16 = nullptr, *seq_off = nullptr, *scan_tmp = nullptr;
-    auto carve1 = [&](Carver& c) { carve0(c); recs = c.take<ingest::RawRec>(n_raw + 1); keep = c.take<uint32_t>(n_raw + 1); idx = c.take<uint32_t>(n_raw + 1); groups = c.take<uint32_t>(n_raw + 1); grp_off = c.take<uint32_t>(n_raw + 1);
-                                   var16 = c.take<uint32_t>(n_raw + 1); var_off = c.take<uint32_t>(n_raw + 1); seq16 = c.take<uint32_t>(n_raw + 1); seq_off = c.take<uint32_t>(n_raw + 1); scan_tmp = c.take<uint32_t>(prims::scan_tmp_elems(n_raw + 1) + 16); };
-    Carver m1; carve1(m1);
-    if (m1.off + 256 > ctx->b_ing.cap) {
-        // grow without losing the fixed part: a new buffer, the fixed part copied over
-        DevBuf nbuf; if (nbuf.ensure(m1.off + 256)) return fail(ctx, "out of device memory (ingest work arrays)");
-        CUDA_TRY(cudaMemcpyAsync(nbuf.p, ctx->b_ing.p, m0.off, cudaMemcpyDeviceToDevice, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        ctx->b_ing.release(); ctx->b_ing = nbuf;
-    }
-    { Carver a; a.base = ctx->b_ing.as<uint8_t>(); carve1(a); }
+    if (carve(ctx->b_ing_work, [&](Carver& c) { recs = c.take<ingest::RawRec>(n_raw + 1); keep = c.take<uint32_t>(n_raw + 1); idx = c.take<uint32_t>(n_raw + 1); groups = c.take<uint32_t>(n_raw + 1); grp_off = c.take<uint32_t>(n_raw + 1);
+                                                var16 = c.take<uint32_t>(n_raw + 1); var_off = c.take<uint32_t>(n_raw + 1); seq16 = c.take<uint32_t>(n_raw + 1); seq_off = c.take<uint32_t>(n_raw + 1); scan_tmp = c.take<uint32_t>(prims::scan_tmp_elems(n_raw + 1) + 16); }))
+        return fail(ctx, "out of device memory (ingest work arrays)");
     const uint32_t evt = evt_need(ctx);
     uint64_t n_rec = 0, n_groups = 0, n_var16 = 0, n_seq16 = 0;
     if (n_raw) {
@@ -695,26 +677,11 @@ static void carve_c(snfb_ctx* ctx, Carver& c) {
     cc.alt = c.take<uint8_t>(k.alt + 64); cc.scr = c.take<uint8_t>(k.scr16 * 16 + 64);
     ctx->seq_req = c.take<consensus::SeqReq>(k.req + 1); ctx->seq_arena = c.take<uint8_t>(k.req16 * 16 + 64);
 }
+// carved on every attempt: an arena is reallocated only when it must grow, so unchanged capacities give the same pointers
 static int ensure_arenas(snfb_ctx* ctx) {
-    if (ctx->arena_r_for != ctx->n_rec + 1 || ctx->arena_r_tasks != ctx->n_task || ctx->arena_r_cigar != ctx->n_cigar || !ctx->arena_r.p) {
-        Carver m; carve_r(ctx, m);
-        if (ctx->arena_r.ensure(m.off + 256)) return fail(ctx, "out of device memory (per-record arrays)");
-        Carver a; a.base = ctx->arena_r.as<uint8_t>(); carve_r(ctx, a);
-        ctx->arena_r_for = ctx->n_rec + 1; ctx->arena_r_tasks = ctx->n_task; ctx->arena_r_cigar = ctx->n_cigar;
-    }
-    if (ctx->arena_l_for.lead != ctx->cap.lead || !ctx->arena_l.p) {
-        Carver m; carve_l(ctx, m);
-        if (ctx->arena_l.ensure(m.off + 256)) return fail(ctx, "out of device memory (per-lead arrays)");
-        Carver a; a.base = ctx->arena_l.as<uint8_t>(); carve_l(ctx, a);
-        ctx->arena_l_for = ctx->cap;
-    }
-    const Caps& k = ctx->cap; const Caps& f = ctx->arena_c_for;
-    if (!ctx->arena_c.p || f.cand != k.cand || f.cand_lead != k.cand_lead || f.rn != k.rn || f.alt != k.alt || f.scr16 != k.scr16 || f.item != k.item || f.tile != k.tile || f.req != k.req || f.req16 != k.req16) {
-        Carver m; carve_c(ctx, m);
-        if (ctx->arena_c.ensure(m.off + 256)) return fail(ctx, "out of device memory (candidate / consensus arrays)");
-        Carver a; a.base = ctx->arena_c.as<uint8_t>(); carve_c(ctx, a);
-        ctx->arena_c_for = ctx->cap;
-    }
+    if (carve(ctx->arena_r, [&](Carver& c) { carve_r(ctx, c); })) return fail(ctx, "out of device memory (per-record arrays)");
+    if (carve(ctx->arena_l, [&](Carver& c) { carve_l(ctx, c); })) return fail(ctx, "out of device memory (per-lead arrays)");
+    if (carve(ctx->arena_c, [&](Carver& c) { carve_c(ctx, c); })) return fail(ctx, "out of device memory (candidate / consensus arrays)");
     return 0;
 }
 
@@ -974,6 +941,13 @@ static void finish_cand_view(snfb_ctx* ctx, const DevCounters& c, snfb_cand_view
 }
 
 // ------------------------------------------------------------------------------------------------ the run loop
+// the message of the first counter that fails the run whatever the capacities, or nullptr
+static const char* fatal_counter(const DevCounters& c) {
+    if (c.bad_records) return "the record block is malformed: a record points outside its task table or arenas";
+    if (c.unsorted) return "records are not coordinate sorted inside a task";
+    if (c.ordinal_overflow) return "a read carries more than 65535 SV signatures (16-bit lead ordinal)";
+    return nullptr;
+}
 // upto: 1 = stage A (+ sort and bins), 2 = + stage B and the consensus plan, 3 = + consensus.
 static int run_pipeline(snfb_ctx* ctx, int upto, snfb_lead_view* leads, snfb_cand_view* cands, snfb_seq_view* seqs) {
     if (!ctx->loaded) return fail(ctx, "no records loaded");
@@ -1002,9 +976,7 @@ static int run_pipeline(snfb_ctx* ctx, int upto, snfb_lead_view* leads, snfb_can
         if (upto >= 3 && !ctx->seq_on_demand) { if (enqueue_stage_c(ctx)) return 1; }
         if (mid) {
             CUDA_TRY(cudaEventSynchronize(ctx->ev_mid));
-            if (ctx->h_mid->bad_records) { cudaStreamSynchronize(st); return fail(ctx, "the record block is malformed: a record points outside its task table or arenas"); }
-            if (ctx->h_mid->unsorted) { cudaStreamSynchronize(st); return fail(ctx, "records are not coordinate sorted inside a task"); }
-            if (ctx->h_mid->ordinal_overflow) { cudaStreamSynchronize(st); return fail(ctx, "a read carries more than 65535 SV signatures (16-bit lead ordinal)"); }
+            if (const char* m = fatal_counter(*ctx->h_mid)) { cudaStreamSynchronize(st); return fail(ctx, m); }
             if (!caps_fit(ctx, *ctx->h_mid, ctx->h_work, 2)) { CUDA_TRY(cudaStreamSynchronize(st)); ++ctx->reruns; continue; }
             if (ctx->h_mid->unverified_breaks && !ctx->force_no_cuts) { CUDA_TRY(cudaStreamSynchronize(st)); ctx->force_no_cuts = true; ++ctx->reruns; continue; }   // a chain cut was wrong: redo with whole chains
             if (cands) { if (enqueue_cand_copies(ctx, *ctx->h_mid, ctx->st_copy)) return 1; copies = true; }
@@ -1020,9 +992,7 @@ static int run_pipeline(snfb_ctx* ctx, int upto, snfb_lead_view* leads, snfb_can
         CUDA_TRY(cudaStreamSynchronize(st));
         if (copies) CUDA_TRY(cudaStreamSynchronize(ctx->st_copy));
         CUDA_TRY(cudaGetLastError());
-        if (ctx->h_fin->bad_records) return fail(ctx, "the record block is malformed: a record points outside its task table or arenas");
-        if (ctx->h_fin->unsorted) return fail(ctx, "records are not coordinate sorted inside a task");
-        if (ctx->h_fin->ordinal_overflow) return fail(ctx, "a read carries more than 65535 SV signatures (16-bit lead ordinal)");
+        if (const char* m = fatal_counter(*ctx->h_fin)) return fail(ctx, m);
         if (!caps_fit(ctx, *ctx->h_fin, upto >= 2 ? ctx->h_work + 16 : ctx->h_work, upto)) { ++ctx->reruns; continue; }
         break;
     }
@@ -1108,9 +1078,8 @@ int snfb_allgather_candidates(snfb_ctx* ctx, uint32_t flags, snfb_gather_view* o
     cudaSetDevice(ctx->device);
     const int nr = ctx->nranks, with_leads = (flags & SNFB_GATHER_LEADS) ? 1 : 0; cudaStream_t st = ctx->st; cluster::B& b = ctx->B;
     memset(out, 0, sizeof *out);
-    if (ctx->h_gather.ensure(64 * 8 + (size_t)nr * (sizeof(GatherHdr) + 8) + 256)) return fail(ctx, "out of pinned memory (gather)");
-    unsigned long long* h_layout = ctx->h_gather.as<unsigned long long>();                   // [8] layout, then the header table
-    GatherHdr* h_hdr = reinterpret_cast<GatherHdr*>(h_layout + 8);
+    unsigned long long* h_layout = nullptr; GatherHdr* h_hdr = nullptr; uint64_t* rank_n = nullptr;      // k_gather_merge's [8] layout words, the header table, rank_n_cand
+    if (carve(ctx->h_gather, [&](Carver& c) { h_layout = c.take<unsigned long long>(8); h_hdr = c.take<GatherHdr>(nr); rank_n = c.take<uint64_t>(nr); })) return fail(ctx, "out of pinned memory (gather)");
     for (int attempt = 0; attempt < 4; ++attempt) {
         if (ctx->gather_cap == 0) {
             // first call: the slot size every rank uses is agreed through a small all-gather of what each rank needs
@@ -1128,8 +1097,9 @@ int snfb_allgather_candidates(snfb_ctx* ctx, uint32_t flags, snfb_gather_view* o
             ctx->gather_cap = (grown(mx) + 255ull) & ~255ull;
         }
         const unsigned long long cap = ctx->gather_cap, out_cap = (unsigned long long)nr * cap + 4096ull * 8;
-        if (ctx->b_gsend.ensure(cap + 256) || ctx->b_grecv.ensure((size_t)nr * cap + out_cap + 1024)) return fail(ctx, "out of device memory (gather)");
-        uint8_t* recv = ctx->b_grecv.as<uint8_t>(); uint8_t* merged = recv + (((size_t)nr * cap + 255) & ~(size_t)255); unsigned long long* d_layout = reinterpret_cast<unsigned long long*>(merged + out_cap);     // layout words live behind the merged arrays
+        uint8_t* recv = nullptr; uint8_t* merged = nullptr; unsigned long long* d_layout = nullptr;
+        if (ctx->b_gsend.ensure(cap + 256) || carve(ctx->b_grecv, [&](Carver& c) { recv = c.take<uint8_t>((size_t)nr * cap); merged = c.take<uint8_t>(out_cap); d_layout = c.take<unsigned long long>(8); }))
+            return fail(ctx, "out of device memory (gather)");
         mark(ctx, "allgather");
         launch(ctx->launches, k_gather_pack, NUM_SMS * 4, 256, 0, st, b.ctr, b.cand, ctx->Cc.alt, b.rnames, b.rn_off_out, b.cand_leads, with_leads, nr > 1 ? ctx->b_gsend.as<uint8_t>() : recv, cap);
         if (nr > 1 && g_nccl.AllGather(ctx->b_gsend.p, recv, cap, 0 /* ncclChar */, ctx->comm, st) != 0) return fail(ctx, "ncclAllGather failed");
@@ -1144,19 +1114,13 @@ int snfb_allgather_candidates(snfb_ctx* ctx, uint32_t flags, snfb_gather_view* o
         // next call: a slot size every rank derives from the same table
         if (grown(mx) > cap) ctx->gather_cap = (grown(mx) + 255ull) & ~255ull;
         GatherHdr tot{}; for (int r = 0; r < nr; ++r) { tot.n_cand += h_hdr[r].n_cand; tot.n_alt += h_hdr[r].n_alt; tot.n_rn += h_hdr[r].n_rn; tot.n_leads += h_hdr[r].n_leads; }
-        uint64_t* rank_n = reinterpret_cast<uint64_t*>(h_hdr + nr); for (int r = 0; r < nr; ++r) rank_n[r] = h_hdr[r].n_cand;
+        for (int r = 0; r < nr; ++r) rank_n[r] = h_hdr[r].n_cand;
         out->n_cand = tot.n_cand; out->n_alt_bytes = tot.n_alt; out->n_rnames = tot.n_rn; out->n_cand_leads = tot.n_leads; out->rank_n_cand = rank_n;
         out->dev_buffer = merged; out->dev_bytes_per_rank = cap;
         if (!(flags & SNFB_GATHER_DEVICE_ONLY)) {
             const unsigned long long total = h_layout[5];
-            if (ctx->h_gather.cap < 64 * 8 + (size_t)nr * (sizeof(GatherHdr) + 8) + 256 + total + 512) {
-                // grow while keeping the table: copy it aside
-                std::vector<uint8_t> keep((size_t)64 * 8 + (size_t)nr * (sizeof(GatherHdr) + 8)); memcpy(keep.data(), ctx->h_gather.p, keep.size());
-                if (ctx->h_gather.ensure(64 * 8 + (size_t)nr * (sizeof(GatherHdr) + 8) + 256 + total + 512)) return fail(ctx, "out of pinned memory (gather result)");
-                memcpy(ctx->h_gather.p, keep.data(), keep.size());
-                h_layout = ctx->h_gather.as<unsigned long long>(); h_hdr = reinterpret_cast<GatherHdr*>(h_layout + 8); rank_n = reinterpret_cast<uint64_t*>(h_hdr + nr); out->rank_n_cand = rank_n;
-            }
-            uint8_t* hm = ctx->h_gather.as<uint8_t>() + (((size_t)64 * 8 + (size_t)nr * (sizeof(GatherHdr) + 8) + 255) & ~(size_t)255);
+            if (ctx->h_gather_out.ensure(total)) return fail(ctx, "out of pinned memory (gather result)");
+            uint8_t* hm = ctx->h_gather_out.as<uint8_t>();
             CUDA_TRY(cudaMemcpyAsync(hm, merged, total, cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
             out->cand = reinterpret_cast<const snfb_cand*>(hm + h_layout[0]); out->alt = hm + h_layout[1]; out->rnames = reinterpret_cast<const uint64_t*>(hm + h_layout[2]);
             out->rnames_off = reinterpret_cast<const uint32_t*>(hm + h_layout[3]); out->cand_leads = with_leads ? reinterpret_cast<const snfb_lead*>(hm + h_layout[4]) : nullptr;
@@ -1189,21 +1153,20 @@ int snfb_poa(snfb_ctx* ctx, const snfb_poa_job* jobs, uint32_t n_jobs, const uin
     while (nblk > 1 && nblk * smax > free_b / 3) --nblk;
     if (smax > free_b / 2) return fail(ctx, "snfb_poa: a job needs more scratch than the device has free");
     DevBuf d_jobs, d_seqs, d_offs, d_out, d_len, d_scr, d_ctr;
-    int rc = d_jobs.ensure(sizeof(snfb_poa_job) * n_jobs) | d_seqs.ensure(n_seq_bytes + 16) | d_offs.ensure(4 * n_offs + 16) | d_out.ensure(out_bytes + 16) | d_len.ensure(4 * (size_t)n_jobs) | d_scr.ensure(nblk * smax) | d_ctr.ensure(64);
-    auto done = [&](int r) { d_jobs.release(); d_seqs.release(); d_offs.release(); d_out.release(); d_len.release(); d_scr.release(); d_ctr.release(); return r; };
-    if (rc) return done(fail(ctx, "snfb_poa: out of device memory"));
+    if (d_jobs.ensure(sizeof(snfb_poa_job) * n_jobs) || d_seqs.ensure(n_seq_bytes + 16) || d_offs.ensure(4 * n_offs + 16) || d_out.ensure(out_bytes + 16) || d_len.ensure(4 * (size_t)n_jobs) || d_scr.ensure(nblk * smax) || d_ctr.ensure(64))
+        return fail(ctx, "snfb_poa: out of device memory");
     cudaStream_t st = ctx->st;
-    cudaMemcpyAsync(d_jobs.p, jobs, sizeof(snfb_poa_job) * n_jobs, cudaMemcpyHostToDevice, st); cudaMemcpyAsync(d_seqs.p, seqs, n_seq_bytes, cudaMemcpyHostToDevice, st);
-    cudaMemcpyAsync(d_offs.p, offs, 4 * n_offs, cudaMemcpyHostToDevice, st); cudaMemsetAsync(d_ctr.p, 0, 64, st); cudaMemsetAsync(d_out.p, 0, out_bytes, st);
+    CUDA_TRY(cudaMemcpyAsync(d_jobs.p, jobs, sizeof(snfb_poa_job) * n_jobs, cudaMemcpyHostToDevice, st)); CUDA_TRY(cudaMemcpyAsync(d_seqs.p, seqs, n_seq_bytes, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_offs.p, offs, 4 * n_offs, cudaMemcpyHostToDevice, st)); CUDA_TRY(cudaMemsetAsync(d_ctr.p, 0, 64, st)); CUDA_TRY(cudaMemsetAsync(d_out.p, 0, out_bytes, st));
     poa::Params P{}; P.jobs = d_jobs.as<poa::Job>(); P.n_jobs = n_jobs; P.seqs = d_seqs.as<uint8_t>(); P.offs = d_offs.as<int>(); P.out = d_out.as<uint8_t>(); P.out_len = d_len.as<int>();
     P.scratch = d_scr.as<uint8_t>(); P.scratch_per_block = smax; P.next_job = d_ctr.as<unsigned>();
     mark(ctx, "poa");
     launch(ctx->launches, poa::k_poa, (unsigned)nblk, poa::THREADS, 0, st, P);
     mark(ctx, nullptr);
-    cudaMemcpyAsync(out, d_out.p, out_bytes, cudaMemcpyDeviceToHost, st); cudaMemcpyAsync(out_len, d_len.p, 4 * (size_t)n_jobs, cudaMemcpyDeviceToHost, st);
+    CUDA_TRY(cudaMemcpyAsync(out, d_out.p, out_bytes, cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaMemcpyAsync(out_len, d_len.p, 4 * (size_t)n_jobs, cudaMemcpyDeviceToHost, st));
     const cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return done(fail(ctx, std::string("snfb_poa: ") + cudaGetErrorString(e)));
-    return done(0);
+    if (e != cudaSuccess) return fail(ctx, std::string("snfb_poa: ") + cudaGetErrorString(e));
+    return 0;
 }
 
 // multi-sample combine: every (task, svtype) chain of the plan by one warp (combine.cuh); host buffers in, host buffers out
@@ -1232,42 +1195,39 @@ int snfb_combine_groups(snfb_ctx* ctx, const snfb_combine_in* in, snfb_combine_o
     if (use_alt) for (uint32_t i = 0; i < in->n_cand; ++i) { if (in->alt_off[i] + in->alt_len[i] > in->n_alt_bytes) return fail(ctx, "snfb_combine_groups: ALT outside alt[]"); max_alt = std::max(max_alt, in->alt_len[i]); }
     max_alt = (max_alt + 15u) & ~15u;
     const unsigned blocks = (unsigned)std::min<size_t>((in->n_chain + 3) / 4, NUM_SMS * 4);
-    DevBuf b_in, b_state, b_out;
     // inputs in one buffer, group state in one, outputs in one
-    Carver ci, cs, co;
-    auto lay = [&](Carver& c, combine::P& P, bool in_, bool st_, bool out_) {
-        if (in_) { P.chains = c.take<snfb_combine_chain>(in->n_chain); P.chunks = c.take<snfb_combine_chunk>(in->n_chunk); P.pos = c.take<int32_t>(n); P.svlen = c.take<int32_t>(n); P.sample = c.take<uint32_t>(n);
-                   P.mate_contig = c.take<int32_t>(n); P.mate_pos = c.take<int32_t>(n); P.block_start = c.take<long long>(in->n_cov_block + 1); P.cov = c.take<int32_t>(ncov + 1);
-                   if (use_alt) { P.alt = c.take<uint8_t>(in->n_alt_bytes + 16); P.alt_off = c.take<unsigned long long>(n); P.alt_len = c.take<uint32_t>(n); } }
-        if (st_) { P.g_pos = c.take<double>(n); P.g_len = c.take<double>(n); P.g_mate = c.take<double>(n); P.g_n = c.take<uint32_t>(n); P.g_mc = c.take<int32_t>(n); P.g_incl = c.take<uint32_t>(n * W); P.act = c.take<uint32_t>(n);
-                   P.next_chain = c.take<unsigned int>(4); P.g_first = c.take<uint32_t>(n); P.ex_stamp = c.take<uint32_t>(n); if (use_alt) P.hs = c.take<int8_t>((size_t)blocks * 4 * max_alt + 16); }
-        if (out_) { P.cand_group = c.take<uint32_t>(n); P.emit_chunk = c.take<int32_t>(n); P.emit_ord = c.take<uint32_t>(n); P.cov_non = c.take<int32_t>(n * S); }
-    };
+    DevBuf b_in, b_state, b_out;
     combine::P P{};
-    lay(ci, P, true, false, false); lay(cs, P, false, true, false); lay(co, P, false, false, true);
-    auto done = [&](int r) { b_in.release(); b_state.release(); b_out.release(); return r; };
-    if (b_in.ensure(ci.off + 256) | b_state.ensure(cs.off + 256) | b_out.ensure(co.off + 256)) return done(fail(ctx, "snfb_combine_groups: out of device memory"));
-    ci = Carver{ b_in.as<uint8_t>(), 0 }; cs = Carver{ b_state.as<uint8_t>(), 0 }; co = Carver{ b_out.as<uint8_t>(), 0 };
-    lay(ci, P, true, false, false); lay(cs, P, false, true, false); lay(co, P, false, false, true);
+    auto lay_in = [&](Carver& c) {
+        P.chains = c.take<snfb_combine_chain>(in->n_chain); P.chunks = c.take<snfb_combine_chunk>(in->n_chunk); P.pos = c.take<int32_t>(n); P.svlen = c.take<int32_t>(n); P.sample = c.take<uint32_t>(n);
+        P.mate_contig = c.take<int32_t>(n); P.mate_pos = c.take<int32_t>(n); P.block_start = c.take<long long>(in->n_cov_block + 1); P.cov = c.take<int32_t>(ncov + 1);
+        if (use_alt) { P.alt = c.take<uint8_t>(in->n_alt_bytes + 16); P.alt_off = c.take<unsigned long long>(n); P.alt_len = c.take<uint32_t>(n); }
+    };
+    auto lay_state = [&](Carver& c) {
+        P.g_pos = c.take<double>(n); P.g_len = c.take<double>(n); P.g_mate = c.take<double>(n); P.g_n = c.take<uint32_t>(n); P.g_mc = c.take<int32_t>(n); P.g_incl = c.take<uint32_t>(n * W); P.act = c.take<uint32_t>(n);
+        P.next_chain = c.take<unsigned int>(4); P.g_first = c.take<uint32_t>(n); P.ex_stamp = c.take<uint32_t>(n); if (use_alt) P.hs = c.take<int8_t>((size_t)blocks * 4 * max_alt + 16);
+    };
+    auto lay_out = [&](Carver& c) { P.cand_group = c.take<uint32_t>(n); P.emit_chunk = c.take<int32_t>(n); P.emit_ord = c.take<uint32_t>(n); P.cov_non = c.take<int32_t>(n * S); };
+    if (carve(b_in, lay_in) || carve(b_state, lay_state) || carve(b_out, lay_out)) return fail(ctx, "snfb_combine_groups: out of device memory");
     P.n_chain = in->n_chain; P.n_chunk = in->n_chunk; P.n_cand = in->n_cand; P.n_samples = in->n_samples; P.words = (uint32_t)W;
     P.bins_per_block = in->bins_per_block; P.cov_binsize = in->cov_binsize;
     P.combine_match = in->combine_match; P.combine_match_max = in->combine_match_max; P.cluster_merge_bnd = in->cluster_merge_bnd; P.separate_intra = in->combine_separate_intra; P.overlap_abs = in->combine_overlap_abs;
     cudaStream_t st = ctx->st;
-    auto up = [&](const void* dst, const void* src, size_t bytes) { if (bytes && src) cudaMemcpyAsync(const_cast<void*>(dst), src, bytes, cudaMemcpyHostToDevice, st); };
-    up(P.chains, in->chains, sizeof(snfb_combine_chain) * in->n_chain); up(P.chunks, in->chunks, sizeof(snfb_combine_chunk) * in->n_chunk);
-    up(P.pos, in->pos, 4 * n); up(P.svlen, in->svlen, 4 * n); up(P.sample, in->sample, 4 * n); up(P.mate_contig, in->mate_contig, 4 * n); up(P.mate_pos, in->mate_pos, 4 * n);
-    up(P.block_start, in->block_start, 8 * (size_t)in->n_cov_block); up(P.cov, in->cov, 4 * ncov);
+    auto up = [&](const void* dst, const void* src, size_t bytes) { if (bytes && src) CUDA_TRY(cudaMemcpyAsync(const_cast<void*>(dst), src, bytes, cudaMemcpyHostToDevice, st)); return 0; };
+    if (up(P.chains, in->chains, sizeof(snfb_combine_chain) * in->n_chain) || up(P.chunks, in->chunks, sizeof(snfb_combine_chunk) * in->n_chunk)
+        || up(P.pos, in->pos, 4 * n) || up(P.svlen, in->svlen, 4 * n) || up(P.sample, in->sample, 4 * n) || up(P.mate_contig, in->mate_contig, 4 * n) || up(P.mate_pos, in->mate_pos, 4 * n)
+        || up(P.block_start, in->block_start, 8 * (size_t)in->n_cov_block) || up(P.cov, in->cov, 4 * ncov)) return 1;
     P.pctseq = use_alt ? in->combine_pctseq : 0.0; P.max_alt = max_alt;
-    if (use_alt) { up(P.alt, in->alt, in->n_alt_bytes); up(P.alt_off, in->alt_off, 8 * n); up(P.alt_len, in->alt_len, 4 * n); }
-    cudaMemsetAsync(P.next_chain, 0, 16, st);
+    if (use_alt && (up(P.alt, in->alt, in->n_alt_bytes) || up(P.alt_off, in->alt_off, 8 * n) || up(P.alt_len, in->alt_len, 4 * n))) return 1;
+    CUDA_TRY(cudaMemsetAsync(P.next_chain, 0, 16, st));
     mark(ctx, "combine_groups");
     launch(ctx->launches, combine::k_combine, blocks, 128, 0, st, P);
     mark(ctx, nullptr);
-    cudaMemcpyAsync(out->cand_group, P.cand_group, 4 * n, cudaMemcpyDeviceToHost, st); cudaMemcpyAsync(out->emit_chunk, P.emit_chunk, 4 * n, cudaMemcpyDeviceToHost, st);
-    cudaMemcpyAsync(out->emit_ord, P.emit_ord, 4 * n, cudaMemcpyDeviceToHost, st); cudaMemcpyAsync(out->cov_non, P.cov_non, 4 * n * S, cudaMemcpyDeviceToHost, st);
+    CUDA_TRY(cudaMemcpyAsync(out->cand_group, P.cand_group, 4 * n, cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaMemcpyAsync(out->emit_chunk, P.emit_chunk, 4 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->emit_ord, P.emit_ord, 4 * n, cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaMemcpyAsync(out->cov_non, P.cov_non, 4 * n * S, cudaMemcpyDeviceToHost, st));
     const cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return done(fail(ctx, std::string("snfb_combine_groups: ") + cudaGetErrorString(e)));
-    return done(0);
+    if (e != cudaSuccess) return fail(ctx, std::string("snfb_combine_groups: ") + cudaGetErrorString(e));
+    return 0;
 }
 
 int snfb_selftest_edit_distance(snfb_ctx* ctx, const uint8_t* bytes, uint64_t n_bytes, const uint64_t* a_off, const uint32_t* a_len, const uint64_t* b_off, const uint32_t* b_len, uint32_t n_pairs, int32_t* out) {
@@ -1279,17 +1239,16 @@ int snfb_selftest_edit_distance(snfb_ctx* ctx, const uint8_t* bytes, uint64_t n_
     cudaSetDevice(ctx->device);
     const unsigned blocks = (unsigned)std::min<uint32_t>((n_pairs + 3) / 4, NUM_SMS * 4);
     DevBuf d_b, d_o, d_hs, d_out;
-    auto done = [&](int r) { d_b.release(); d_o.release(); d_hs.release(); d_out.release(); return r; };
-    if (d_b.ensure(n_bytes + 16) | d_o.ensure((size_t)n_pairs * 24 + 64) | d_hs.ensure((size_t)blocks * 4 * max_len + 16) | d_out.ensure((size_t)n_pairs * 4)) return done(fail(ctx, "snfb_selftest_edit_distance: out of device memory"));
+    if (d_b.ensure(n_bytes + 16) || d_o.ensure((size_t)n_pairs * 24 + 64) || d_hs.ensure((size_t)blocks * 4 * max_len + 16) || d_out.ensure((size_t)n_pairs * 4)) return fail(ctx, "snfb_selftest_edit_distance: out of device memory");
     unsigned long long* ao = d_o.as<unsigned long long>(); unsigned long long* bo = ao + n_pairs; uint32_t* al = reinterpret_cast<uint32_t*>(bo + n_pairs); uint32_t* bl = al + n_pairs;
     cudaStream_t st = ctx->st;
-    cudaMemcpyAsync(d_b.p, bytes, n_bytes, cudaMemcpyHostToDevice, st); cudaMemcpyAsync(ao, a_off, 8 * (size_t)n_pairs, cudaMemcpyHostToDevice, st); cudaMemcpyAsync(bo, b_off, 8 * (size_t)n_pairs, cudaMemcpyHostToDevice, st);
-    cudaMemcpyAsync(al, a_len, 4 * (size_t)n_pairs, cudaMemcpyHostToDevice, st); cudaMemcpyAsync(bl, b_len, 4 * (size_t)n_pairs, cudaMemcpyHostToDevice, st);
+    CUDA_TRY(cudaMemcpyAsync(d_b.p, bytes, n_bytes, cudaMemcpyHostToDevice, st)); CUDA_TRY(cudaMemcpyAsync(ao, a_off, 8 * (size_t)n_pairs, cudaMemcpyHostToDevice, st)); CUDA_TRY(cudaMemcpyAsync(bo, b_off, 8 * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(al, a_len, 4 * (size_t)n_pairs, cudaMemcpyHostToDevice, st)); CUDA_TRY(cudaMemcpyAsync(bl, b_len, 4 * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
     launch(ctx->launches, combine::k_edit_selftest, blocks, 128, 0, st, d_b.as<uint8_t>(), ao, al, bo, bl, n_pairs, d_hs.as<int8_t>(), max_len, d_out.as<int>());
-    cudaMemcpyAsync(out, d_out.p, 4 * (size_t)n_pairs, cudaMemcpyDeviceToHost, st);
+    CUDA_TRY(cudaMemcpyAsync(out, d_out.p, 4 * (size_t)n_pairs, cudaMemcpyDeviceToHost, st));
     const cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return done(fail(ctx, std::string("snfb_selftest_edit_distance: ") + cudaGetErrorString(e)));
-    return done(0);
+    if (e != cudaSuccess) return fail(ctx, std::string("snfb_selftest_edit_distance: ") + cudaGetErrorString(e));
+    return 0;
 }
 
 // mean coverage of `binsize`-base bins over one task's region (snf.py:248-267: the 500-bp means the SNF writer stores)
@@ -1310,7 +1269,6 @@ int snfb_coverage_bins(snfb_ctx* ctx, uint32_t task, int binsize, const double**
     unsigned long long* raw = reinterpret_cast<unsigned long long*>(ctx->h_cov_bins.as<uint8_t>() + 8 * (size_t)(nb + 1));
     CUDA_TRY(cudaMemcpyAsync(raw, acc.p, 8 * (size_t)nb, cudaMemcpyDeviceToHost, ctx->st));
     CUDA_TRY(cudaStreamSynchronize(ctx->st));
-    acc.release();
     double* o = ctx->h_cov_bins.as<double>();
     for (long long i = 0; i < nb; ++i) o[i] = (double)raw[i] / (double)binsize;
     *out = o; *n_bins = (uint64_t)nb; return 0;
