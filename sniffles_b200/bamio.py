@@ -4,6 +4,8 @@ index, SAM spec §5.2), so a task only inflates the BGZF blocks its region touch
 record block) exists for the tests and the benchmark inputs; it is not part of the product path.
 
 Base qualities are never decoded; of the aux tags only NM, HP, PS, SA and the CG:B,I long-CIGAR escape are read."""
+import bisect
+import os
 import struct
 import zlib
 
@@ -18,6 +20,31 @@ _BGZF_EOF = bytes.fromhex("1f8b08040000000000ff0600424302001b0003000000000000000
 
 
 # ------------------------------------------------------------------------------------------------ BGZF
+def bgzf_header(buf, o=0):
+    """The BGZF member header at offset o of a bytes-like buffer (SAM spec §4.1: the gzip magic with FEXTRA, then the BC subfield)
+    -> (bsize, payload offset, payload length): the member's total size and where in `buf` its raw DEFLATE data lies."""
+    if buf[o:o + 4] != b"\x1f\x8b\x08\x04":
+        raise ValueError("not a BGZF block")
+    xlen = struct.unpack_from("<H", buf, o + 10)[0]
+    e = o + 12
+    while e + 4 <= o + 12 + xlen:
+        slen = struct.unpack_from("<H", buf, e + 2)[0]
+        if buf[e] == 66 and buf[e + 1] == 67:
+            bsize = struct.unpack_from("<H", buf, e + 4)[0] + 1
+            return bsize, o + 12 + xlen, bsize - 12 - xlen - 8
+        e += 4 + slen
+    raise ValueError("BGZF block without a BC field")
+
+
+def bgzf_members(z):
+    """(start, payload offset, payload length, ISIZE) of every member of a buffer of whole BGZF members"""
+    o = 0
+    while o < len(z):
+        bsize, po, pl = bgzf_header(z, o)
+        yield o, po, pl, struct.unpack_from("<I", z, o + bsize - 4)[0]
+        o += bsize
+
+
 class BgzfReader:
     """random access by BGZF virtual offset (coffset << 16 | uoffset)"""
 
@@ -28,26 +55,22 @@ class BgzfReader:
     def close(self):
         self.f.close()
 
-    def _block(self, coffset):
-        if self._cache[0] == coffset:
-            return self._cache[1], self._cache[2]
+    def member(self, coffset):
+        """bgzf_header of the member at a file offset, with the payload offset relative to it; (0, 0, 0) at the end of the file"""
         self.f.seek(coffset)
         head = self.f.read(18)
         if len(head) < 18:
+            return 0, 0, 0
+        return bgzf_header(head + self.f.read(max(struct.unpack_from("<H", head, 10)[0] - 6, 0)))
+
+    def _block(self, coffset):
+        if self._cache[0] == coffset:
+            return self._cache[1], self._cache[2]
+        bsize, po, pl = self.member(coffset)
+        if bsize == 0:
             return b"", 0
-        if head[:4] != b"\x1f\x8b\x08\x04":
-            raise ValueError("not a BGZF block")
-        xlen = struct.unpack("<H", head[10:12])[0]
-        extra = head[12:] + self.f.read(xlen - 6)
-        bsize, i = None, 0
-        while i + 4 <= len(extra):
-            si1, si2, slen = extra[i], extra[i + 1], struct.unpack("<H", extra[i + 2:i + 4])[0]
-            if si1 == 66 and si2 == 67:
-                bsize = struct.unpack("<H", extra[i + 4:i + 6])[0] + 1
-            i += 4 + slen
-        if bsize is None:
-            raise ValueError("BGZF block without a BC field")
-        cdata = self.f.read(bsize - 12 - xlen - 8)
+        self.f.seek(coffset + po)
+        cdata = self.f.read(pl)
         trailer = self.f.read(8)
         data = zlib.decompress(cdata, -15)
         # the gzip trailer, checked as htslib checks it: a damaged block can still inflate to ISIZE bytes, but not to the same CRC-32
@@ -126,12 +149,26 @@ def ref_span(cigar):
 
 
 # ------------------------------------------------------------------------------------------------ BAI
-def reg2bins(beg, end):
+def reg2bins(beg, end, min_shift=14, depth=5):
+    """bins overlapping [beg, end) in the binning scheme of SAM spec §5.3; the defaults are the BAI / TBI geometry"""
     end -= 1
-    bins = [0]
-    for shift, off in ((26, 1), (23, 9), (20, 73), (17, 585), (14, 4681)):
-        bins.extend(range(off + (beg >> shift), off + (end >> shift) + 1))
+    bins, t, s = [], 0, min_shift + 3 * depth
+    for lvl in range(depth + 1):
+        bins.extend(range(t + (beg >> s), t + (end >> s) + 1))
+        t += 1 << (3 * lvl)
+        s -= 3
     return bins
+
+
+def _merge_ranges(ranges):
+    """ascending (beg, end) ranges -> [beg, end] lists with every overlapping or touching run merged into one"""
+    merged = []
+    for a, b in ranges:
+        if merged and a <= merged[-1][1]:
+            merged[-1][1] = max(merged[-1][1], b)
+        else:
+            merged.append([a, b])
+    return merged
 
 
 def reg2bin(beg, end):
@@ -152,7 +189,6 @@ class BamFile:
         if head[:4] != b"BAM\1":
             raise ValueError("not a BAM file")
         l_text = struct.unpack("<i", head[4:8])[0]
-        _, v = self.bgzf.read_from(8 << 0, 0)
         data, v = self.bgzf.read_from(0, 12 + l_text)
         n_ref = struct.unpack("<i", data[8 + l_text:12 + l_text])[0]
         self.contigs = []
@@ -163,7 +199,6 @@ class BamFile:
             self.contigs.append((d[:l_name - 1].decode(), struct.unpack("<i", d[l_name:l_name + 4])[0]))
         self.first_record = v
         self.name_to_id = {n: i for i, (n, _) in enumerate(self.contigs)}
-        import os
         if index_path is None:
             index_path = next((p for p in (path + ".bai", path + ".csi", path[:-4] + ".bai" if path.endswith(".bam") else path + ".bai") if os.path.exists(p)), path + ".bai")
         self.min_shift, self.depth = 14, 5
@@ -228,15 +263,6 @@ class BamFile:
         return refs
 
     # ---- index queries shared by fetch and device_input
-    def _reg2bins(self, beg, end):
-        end -= 1
-        bins, t, s = [], 0, self.min_shift + 3 * self.depth
-        for lvl in range(self.depth + 1):
-            bins.extend(range(t + (beg >> s), t + (end >> s) + 1))
-            t += 1 << (3 * lvl)
-            s -= 3
-        return bins
-
     def _min_offset(self, rid, start):
         """smallest virtual offset a record overlapping `start` can have: BAI's linear index, or CSI's per-bin loffset found the way
         htslib looks it up (the leaf bin of start, else the nearest earlier sibling / ancestor that exists)"""
@@ -267,65 +293,40 @@ class BamFile:
         ch = bins.get(self.meta_bin)
         return int(ch[1][0]) if ch and len(ch) > 1 else None
 
+    def records(self, v, stop=1 << 64):
+        """the raw records (without their block_size prefix) that start at virtual offsets from v up to `stop`, in file order"""
+        while v < stop:
+            d, v = self.bgzf.read_from(v, 4)
+            if len(d) < 4:
+                return
+            bs = struct.unpack("<i", d)[0]
+            b, v = self.bgzf.read_from(v, bs)
+            if len(b) < bs:
+                return
+            yield b
+
     def fetch(self, contig, start, end):
         rid = self.name_to_id[contig]
-        bins = self.index[rid][0]
-        min_off = self._min_offset(rid, max(start, 0))
-        chunks = sorted(c for b in self._reg2bins(max(start, 0), max(end, start + 1)) if b in bins and b != self.meta_bin for c in bins[b] if c[1] > min_off)
-        seen_to = 0
-        for beg, stop in chunks:
-            v = max(beg, seen_to, min_off)
-            while v < stop:
-                d, v2 = self.bgzf.read_from(v, 4)
-                if len(d) < 4:
-                    break
-                bs = struct.unpack("<i", d)[0]
-                b, v = self.bgzf.read_from(v2, bs)
-                if len(b) < bs:
-                    break
+        for vb, ve in self.merged_chunks(contig, start, end):
+            for b in self.records(vb, ve):
                 ref_id, pos = struct.unpack("<ii", b[:8])
-                if ref_id != rid or pos >= end:
-                    if ref_id > rid or pos >= end:
-                        seen_to = stop
-                        break
-                    continue
-                r = decode_record(b)
-                if pos + max(ref_span(r["cigar"]), 1) > start:
-                    yield r
-            seen_to = max(seen_to, v)
+                if ref_id > rid or pos >= end:
+                    break
+                if ref_id == rid:
+                    r = decode_record(b)
+                    if pos + max(ref_span(r["cigar"]), 1) > start:
+                        yield r
 
     # ---- device ingest (snfb_load_bam): the index work stays on the host, the bytes stay compressed
     def merged_chunks(self, contig, start, end):
-        """disjoint, ascending virtual-offset ranges holding every record `fetch(contig, start, end)` would look at (the BAI chunks of
-        the region's bins behind the linear-index minimum, merged the way htslib merges them)"""
+        """disjoint, ascending virtual-offset ranges holding every record `fetch(contig, start, end)` looks at (the BAI chunks of the
+        region's bins behind the linear-index minimum, merged the way htslib merges them)"""
         rid = self.name_to_id[contig]
         bins = self.index[rid][0]
         min_off = self._min_offset(rid, max(start, 0))
-        chunks = sorted(c for b in self._reg2bins(max(start, 0), max(end, start + 1)) if b in bins and b != self.meta_bin for c in bins[b] if c[1] > min_off)
-        merged = []
-        for beg, stop in chunks:
-            beg = max(beg, min_off)
-            if merged and beg <= merged[-1][1]:
-                merged[-1][1] = max(merged[-1][1], stop)
-            else:
-                merged.append([beg, stop])
-        return [(a, b) for a, b in merged if b > a]
-
-    def _bsize_at(self, coffset):
-        """total size of the BGZF block that starts at a file offset (0 at end of file)"""
-        self.bgzf.f.seek(coffset)
-        head = self.bgzf.f.read(18)
-        if len(head) < 18:
-            return 0
-        xlen = struct.unpack("<H", head[10:12])[0]
-        extra = head[12:] + self.bgzf.f.read(max(xlen - 6, 0))
-        i = 0
-        while i + 4 <= len(extra):
-            slen = struct.unpack("<H", extra[i + 2:i + 4])[0]
-            if extra[i] == 66 and extra[i + 1] == 67:
-                return struct.unpack("<H", extra[i + 4:i + 6])[0] + 1
-            i += 4 + slen
-        raise ValueError("BGZF block without a BC field")
+        chunks = sorted(c for b in reg2bins(max(start, 0), max(end, start + 1), self.min_shift, self.depth) if b in bins and b != self.meta_bin
+                        for c in bins[b] if c[1] > min_off)
+        return [(a, b) for a, b in _merge_ranges((max(beg, min_off), stop) for beg, stop in chunks) if b > a]
 
     def device_input(self, regions, split=True):
         """regions: [(contig, start, end)] = the tasks, in task order.  Returns (bgzf, spans): the compressed bytes of every BGZF block the
@@ -343,16 +344,10 @@ class BamFile:
             cb, ce = vb >> 16, ve >> 16
             if ve & 0xffff:
                 if ce not in bs_cache:
-                    bs_cache[ce] = self._bsize_at(ce)
+                    bs_cache[ce] = self.bgzf.member(ce)[0]
                 ce += bs_cache[ce]
             iv.append((cb, ce))
-        iv.sort()
-        merged = []
-        for a, b in iv:
-            if merged and a <= merged[-1][1]:
-                merged[-1][1] = max(merged[-1][1], b)
-            else:
-                merged.append([a, b])
+        merged = _merge_ranges(sorted(iv))
         starts, base, parts = [], [], []
         off = 0
         for a, b in merged:
@@ -365,7 +360,6 @@ class BamFile:
             parts.append(d)
             off += len(d)
         bgzf = np.frombuffer(b"".join(parts), "u1") if parts else np.zeros(0, "u1")
-        import bisect
 
         def to_buf(c):                                   # file offset of a block start (or of an interval's end) -> offset in bgzf
             k = bisect.bisect_right(starts, c) - 1
@@ -528,12 +522,14 @@ def tabix_index(text: bytes, coffsets) -> bytes:
 
 
 # ------------------------------------------------------------------------------------------------ writer (tests / benchmark inputs)
-def _bgzf_block(data: bytes, level: int = 6) -> bytes:
-    c = zlib.compressobj(level, zlib.DEFLATED, -15)
+def _bgzf_block(data: bytes, level: int = 6, strategy: int = zlib.Z_DEFAULT_STRATEGY) -> bytes:
+    """one BGZF member: the header with its BC subfield, the raw DEFLATE stream of `data` from zlib, the CRC-32 / ISIZE trailer"""
+    c = zlib.compressobj(level, zlib.DEFLATED, -15, 8, strategy)
     comp = c.compress(data) + c.flush()
-    bsize = len(comp) + 25
-    return (b"\x1f\x8b\x08\x04\x00\x00\x00\x00\x00\xff\x06\x00BC\x02\x00" + struct.pack("<H", bsize) + comp
-            + struct.pack("<II", zlib.crc32(data) & 0xffffffff, len(data)))
+    if len(comp) + 26 > 65536:
+        raise ValueError(f"a BGZF member holds at most 65536 bytes; this one would take {len(comp) + 26}")
+    return (b"\x1f\x8b\x08\x04\x00\x00\x00\x00\x00\xff\x06\x00BC\x02\x00" + struct.pack("<H", len(comp) + 25) + comp
+            + struct.pack("<II", zlib.crc32(data), len(data)))
 
 
 def write_bam(path, blk: RecordBlock, block_bytes=0xff00, level=6, qual_seed=None, index="bai"):
@@ -559,16 +555,19 @@ def write_bam(path, blk: RecordBlock, block_bytes=0xff00, level=6, qual_seed=Non
             buf = bytearray()
 
     def put(data):
+        """append to the BGZF stream -> virtual offsets of the first byte and of the byte after the end"""
         nonlocal buf
         if len(buf) + len(data) > block_bytes:
             flush()
         v0 = (coff << 16) | len(buf)
-        while len(data) > block_bytes:                 # a record larger than one block spans several
-            buf += data[:block_bytes - len(buf)]
-            data = data[block_bytes - len(buf):] if False else data[len(buf):]
-            flush()
-        buf += data
-        return v0
+        if len(data) > block_bytes:                    # larger than one block: cut into block_bytes pieces, flushed as each fills
+            for k in range(0, len(data), block_bytes):
+                buf += data[k:k + block_bytes]
+                if len(buf) >= block_bytes:
+                    flush()
+        else:
+            buf += data
+        return v0, (coff << 16) | len(buf)
     put(head)
     flush()
     for r in blk.rec:
@@ -599,19 +598,7 @@ def write_bam(path, blk: RecordBlock, block_bytes=0xff00, level=6, qual_seed=Non
             n_cig = 2
         body = struct.pack("<iiBBHHHiiii", rid, pos, len(qname), int(r["mapq"]), reg2bin(pos, end), n_cig, int(r["flag"]), l_seq, -1, -1, 0) \
             + qname + cig_b + seq + (b"\xff" * l_seq if qrng is None else np.clip(qrng.normal(22.0, 9.0, l_seq), 2, 50).astype("u1").tobytes()) + aux
-        data = struct.pack("<i", len(body)) + body
-        if len(buf) + len(data) > block_bytes:
-            flush()
-        v0 = (coff << 16) | len(buf)
-        if len(data) > block_bytes:
-            for k in range(0, len(data), block_bytes):
-                buf += data[k:k + block_bytes]
-                if len(buf) >= block_bytes:
-                    flush()
-        else:
-            buf += data
-        v1 = (coff << 16) | len(buf)
-        placed.append((rid, pos, end, v0, v1))
+        placed.append((rid, pos, end, *put(struct.pack("<i", len(body)) + body)))
     flush()
     out.write(_BGZF_EOF)
     out.close()

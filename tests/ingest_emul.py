@@ -4,12 +4,11 @@ lanes.  Lets the index / span logic of bamio.device_input and the decoders be ch
 library with the host reader."""
 import ctypes as C
 import os
-import struct
 import subprocess
 
 import numpy as np
 
-from sniffles_b200 import abi
+from sniffles_b200 import abi, bamio
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, "native", "ingest_host.cpp")
@@ -48,28 +47,10 @@ def inflate(comp: bytes, n_out: int, lead: int = 0):
     return rc, out[:ol.value].tobytes()
 
 
-def walk_bgzf(z: bytes):
-    """[(block start, payload offset, payload length, isize)] of a buffer of whole BGZF blocks"""
-    o, out = 0, []
-    while o < len(z):
-        assert z[o:o + 4] == b"\x1f\x8b\x08\x04"
-        xlen = struct.unpack("<H", z[o + 10:o + 12])[0]
-        e, bsize = o + 12, None
-        while e + 4 <= o + 12 + xlen:
-            slen = struct.unpack("<H", z[e + 2:e + 4])[0]
-            if z[e] == 66 and z[e + 1] == 67:
-                bsize = struct.unpack("<H", z[e + 4:e + 6])[0] + 1
-            e += 4 + slen
-        isize = struct.unpack("<I", z[o + bsize - 4:o + bsize])[0]
-        out.append((o, o + 12 + xlen, bsize - 12 - xlen - 8, isize))
-        o += bsize
-    return out
-
-
 def load_bam(bgzf: np.ndarray, spans: np.ndarray, task_table: np.ndarray, evt_min: int = 11):
     """-> list of per-record dicts in output order (what snfb_load_bam packs), fields as bamio.decode_record + task + cigar16"""
     z = bgzf.tobytes()
-    blocks = walk_bgzf(z)
+    blocks = list(bamio.bgzf_members(z))
     starts = [b[0] for b in blocks]
     uoff, raw = [], bytearray()
     for k, (_, po, pl, isz) in enumerate(blocks):

@@ -61,16 +61,22 @@ def test_region_fetch_equals_overlap_filter(bam):
     f.close()
 
 
-def test_long_cigar_escape(tmp_path):
-    """more than 65535 CIGAR ops: the CG:B,I tag carries the real CIGAR behind an <l_seq>S<reflen>N placeholder"""
-    n = 70000
+def long_cigar_block(n=70000):
+    """one record of n CIGAR ops (3M 1D ...), larger than one BGZF block"""
     cig = np.empty(n, "<u4"); cig[0::2] = (3 << 4) | 0; cig[1::2] = (1 << 4) | 2          # 3M 1D ...
     l_seq = 3 * (n // 2)
     rec = np.zeros(1, abi.REC_DTYPE)
     rec[0] = (0, 100, 0, 60, abi.AUX_NM, 0, 2, 0, 5, 0, n, l_seq, 0, 0, 0, 0, 0)
     contig = np.zeros(1, abi.CONTIG_DTYPE); contig[0] = (abi.fnv1a64(b"c"), 1_000_000, 0)
     task = np.zeros(1, abi.TASK_DTYPE); task[0] = (0, 0, 999_999, 1_000_000, 0, 0, 0, 0)
-    blk = synth.RecordBlock(rec=rec, cigar=cig, var=np.frombuffer(b"rd", "u1"), seq=np.full((l_seq + 1) // 2, 0x12, "u1"), task=task, contig=contig, tr=np.zeros(0, "<i4"), contig_names=["c"])
+    return synth.RecordBlock(rec=rec, cigar=cig, var=np.frombuffer(b"rd", "u1"), seq=np.full((l_seq + 1) // 2, 0x12, "u1"), task=task, contig=contig, tr=np.zeros(0, "<i4"), contig_names=["c"])
+
+
+def test_long_cigar_escape(tmp_path):
+    """more than 65535 CIGAR ops: the CG:B,I tag carries the real CIGAR behind an <l_seq>S<reflen>N placeholder"""
+    n = 70000
+    blk = long_cigar_block(n)
+    cig = blk.cigar
     path = str(tmp_path / "long.bam")
     bamio.write_bam(path, blk)
     f = bamio.BamFile(path)
@@ -99,6 +105,25 @@ def test_csi_index_equals_bai(bam, tmp_path):
     fa.close(); fb.close()
 
 
+def test_device_input_checks_the_header_of_a_block_it_sizes(bam, tmp_path):
+    """a span that ends inside a block needs that whole block, sized from its header: a header without the gzip magic is refused"""
+    blk, path = bam
+    name = blk.contig_names[0]
+    f = bamio.BamFile(path)
+    ve = f.merged_chunks(name, 0, f.get_reference_length(name))[-1][1]
+    f.close()
+    assert ve & 0xffff                                   # the contig's last record ends inside a block: device_input has to size it
+    z = bytearray(open(path, "rb").read())
+    z[ve >> 16] ^= 0x01
+    bad = str(tmp_path / "bad_magic.bam")
+    open(bad, "wb").write(bytes(z))
+    open(bad + ".bai", "wb").write(open(path + ".bai", "rb").read())
+    f = bamio.BamFile(bad)
+    with pytest.raises(ValueError, match="not a BGZF block"):
+        f.device_input([(name, 0, f.get_reference_length(name))], split=False)
+    f.close()
+
+
 # hg002.bam and its .csi: the reference's own htslib-written test data (src/tests/data), stored as a fixture
 REF_DATA = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "bams")
 
@@ -107,22 +132,13 @@ REF_DATA = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "b
 def test_reference_bams_through_csi_and_device_spans(name):
     """htslib-written files: region fetch through their .csi equals a linear scan, the one-lane host build of the device DEFLATE decoder
     inflates every block like zlib, and the spans of device_input cover exactly the records of every contig"""
-    import struct
     import zlib
     import ingest_emul
     f = bamio.BamFile(os.path.join(REF_DATA, name))
-    v, allr = f.first_record, []
-    while True:
-        d, v2 = f.bgzf.read_from(v, 4)
-        if len(d) < 4:
-            break
-        b, v = f.bgzf.read_from(v2, struct.unpack("<i", d)[0])
-        r = bamio.decode_record(b)
-        if r["ref_id"] >= 0:
-            allr.append(r)
+    allr = [r for r in map(bamio.decode_record, f.records(f.first_record)) if r["ref_id"] >= 0]
     assert allr
     z = open(os.path.join(REF_DATA, name), "rb").read()
-    for k, (_, po, pl, isz) in enumerate(ingest_emul.walk_bgzf(z)):
+    for k, (_, po, pl, isz) in enumerate(bamio.bgzf_members(z)):
         rc, got = ingest_emul.inflate(z[po:po + pl], isz, lead=k % 4)
         assert rc == 0 and got == zlib.decompress(z[po:po + pl], -15)
     key = lambda r: (r["pos"], bytes(r["qname"]), r["flag"])

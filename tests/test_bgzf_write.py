@@ -73,15 +73,29 @@ def test_ratio_not_above_zlib_level_1(compress, inputs):
 
 # ------------------------------------------------------------------------------------------------ write_bam after the index refactor
 def test_write_bam_bytes_unchanged(tmp_path):
-    """BAM / BAI / CSI bytes of a seeded block, as the writer produced them before the BAI tables moved into bamio.bin_index"""
-    blk = synth.generate(31, [200_000, 120_000], 10.0, len_mean=8000.0, len_sd=2000.0, sv_spacing=6000.0)
+    """BAM / BAI / CSI bytes as the writer produced them before the BAI tables moved into bamio.bin_index and before the header and
+    the records shared one placement step: a seeded block, the same in 100-byte blocks (the header spans two), a record larger than
+    a BGZF block, and the benchmark's config-6 block (at a twentieth of its contig length) at levels 6 and 0"""
+    from test_bamio import long_cigar_block
+    seeded = synth.generate(31, [200_000, 120_000], 10.0, len_mean=8000.0, len_sd=2000.0, sv_spacing=6000.0)
+    c6 = synth.generate(606, [75_000] * 4, 30.0, len_mean=15000.0, len_sd=6000.0, sv_spacing=8000.0, phased_frac=0.3, tr_frac=0.2)
     sha = lambda p: hashlib.sha256(open(p, "rb").read()).hexdigest()
-    want_bam = "3e7667e27b50add1657dad351344613556fd6ef6bd5a95cd3f0e04792c6173ab"
-    for index, want in (("bai", "dc7c958d85f87e9d2115da854ae640be1750b600f8a76b7b67f96b7f65fd0005"),
-                        ("csi", "df6a8826d2d1e2ea338dd24b0ddca739d59bc2c443f0abfb96ac8198c4cfeb88")):
-        path = str(tmp_path / f"s_{index}.bam")
-        bamio.write_bam(path, blk, index=index)
-        assert sha(path) == want_bam and sha(path + "." + index) == want
+    cases = [                                              # (block, write_bam arguments, BAM, BAI, CSI)
+        (seeded, {}, "3e7667e27b50add1657dad351344613556fd6ef6bd5a95cd3f0e04792c6173ab",
+         "dc7c958d85f87e9d2115da854ae640be1750b600f8a76b7b67f96b7f65fd0005", "df6a8826d2d1e2ea338dd24b0ddca739d59bc2c443f0abfb96ac8198c4cfeb88"),
+        (seeded, dict(block_bytes=100), "20e822ae86af4dbd9658e9e78b5de32ff456d09fd11e823b3a97ad0a02b0340c",
+         "205faa87aa0f85c62a36aaa2e6d5041475cf1e60dba0fec6312711b665d1bad3", "7f902495365c46893ed9c1d5f9db5c7c5a84cb9d0b0a505645b4bfd703ca93fa"),
+        (long_cigar_block(), {}, "76231e29f22c1030016ac9cb3c663a36571f7c11cf86cbfb85919fd00b880c7f",
+         "89faea55223bdd931bc7a919d92521ff344da72aaa4c57f8c507f8cddfcc7055", "84a5f6e7675cf0dea1a9fd78f197270efa7188120ecd3c73b4803615f65c8d77"),
+        (c6, dict(level=6, qual_seed=7), "8534220ed4568b93d2ca4e188e6e12a6ab81d2a22300b8e4db3c1f72b0390d74",
+         "695e250a26062270b6e52461c97ac5c27781d35c7b3913627f3403f7853da2d6", "b5370d7aaca84225502555f618ab0c3a2c89d00b9ff0afee699c5ced306b6b07"),
+        (c6, dict(level=0, qual_seed=7), "0b5e09ce9ab52f822839a8def7a5e7ebd41075ab059e1c5ba43d392edc51fe6e",
+         "3e2ab91e8481f93ae4899afbb7998fb2ccffe2a84ea6a54c853f12b110517392", "90203aa79feab924f39b4434427c7e0bb16758802bc856359f3713955a4390fe")]
+    for k, (blk, kw, want_bam, want_bai, want_csi) in enumerate(cases):
+        for index, want in (("bai", want_bai), ("csi", want_csi)):
+            path = str(tmp_path / f"s{k}_{index}.bam")
+            bamio.write_bam(path, blk, index=index, **kw)
+            assert sha(path) == want_bam and sha(path + "." + index) == want, (k, index)
 
 
 # ------------------------------------------------------------------------------------------------ tabix
@@ -136,14 +150,11 @@ def parse_tbi(body: bytes):
     return [n.decode() for n in names], refs
 
 
-def _file_blocks(z: bytes):
-    """coffset -> start of its data in the text, from the BGZF headers of the written file"""
-    starts, o, u = {}, 0, 0
-    while o < len(z):
-        bsize = struct.unpack_from("<H", z, o + 16)[0] + 1
-        isize = struct.unpack_from("<I", z, o + bsize - 4)[0]
-        starts[o] = u
-        o, u = o + bsize, u + isize
+def _text_starts(z: bytes):
+    """coffset -> start of its data in the text, from the members of the written file"""
+    starts, u = {}, 0
+    for o, _, _, isize in bamio.bgzf_members(z):
+        starts[o], u = u, u + isize
     return starts
 
 
@@ -187,7 +198,7 @@ def test_tabix_queries_match_a_linear_scan(compress, tmp_path):
     out.close()
     z = open(tmp_path / "q.vcf.gz", "rb").read()
     assert gzip.decompress(z) == text
-    starts = _file_blocks(z)
+    starts = _text_starts(z)
     assert len(starts) > 40
     names, refs = parse_tbi(gzip.decompress(open(tmp_path / "q.vcf.gz.tbi", "rb").read()))
     rows = [l.split(b"\t") for l in text.split(b"\n")[:-1] if not l.startswith(b"#")]

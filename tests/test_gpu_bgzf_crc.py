@@ -8,7 +8,6 @@ import zlib
 import numpy as np
 import pytest
 
-import ingest_emul
 from sniffles_b200 import abi, bamio, binding, synth, tasks
 from sniffles_b200 import config as sconfig
 from test_gpu_ingest import _compare, _device_records
@@ -29,12 +28,10 @@ def ctx():
 
 def _member(data: bytes, level: int):
     """one BGZF member with a correct trailer, or None when it would exceed BGZF's 64 KiB block size"""
-    c = zlib.compressobj(level, zlib.DEFLATED, -15)
-    comp = c.compress(data) + c.flush()
-    if len(comp) + 26 > 65536:
+    try:
+        return bamio._bgzf_block(data, level)
+    except ValueError:                                   # larger than 65536 bytes
         return None
-    return (b"\x1f\x8b\x08\x04\x00\x00\x00\x00\x00\xff\x06\x00BC\x02\x00" + struct.pack("<H", len(comp) + 25) + comp
-            + struct.pack("<II", zlib.crc32(data), len(data)))
 
 
 @pytest.fixture(scope="module")
@@ -83,7 +80,7 @@ def test_each_bad_member_is_named(ctx, members):
 
 def _equal_zlib_and_host_reader(ctx, path):
     z = open(path, "rb").read()
-    want = b"".join(zlib.decompress(z[po:po + pl], -15) for _, po, pl, _ in ingest_emul.walk_bgzf(z))
+    want = b"".join(zlib.decompress(z[po:po + pl], -15) for _, po, pl, _ in bamio.bgzf_members(z))
     assert ctx.inflate_bgzf(np.frombuffer(z, "u1")) == want
     f = bamio.BamFile(path)
     regions = [(n, 0, L) for n, L in f.contigs]
@@ -112,7 +109,7 @@ def _corrupt_one_base(path: str, out: str):
     """Re-emit, at level 0, one block of a level-0 BAM that holds read bases, with one byte of a record's 4-bit sequence changed and
     the block's original CRC trailer kept: the DEFLATE stream, ISIZE and the record chain stay valid.  Returns (block index, contig)."""
     z = open(path, "rb").read()
-    blocks = ingest_emul.walk_bgzf(z)
+    blocks = list(bamio.bgzf_members(z))
     raw = [zlib.decompress(z[po:po + pl], -15) for _, po, pl, _ in blocks]
     ubase = np.cumsum([0] + [len(d) for d in raw])
     stream = b"".join(raw)

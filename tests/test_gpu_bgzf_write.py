@@ -11,7 +11,7 @@ import pytest
 import bgzf_host
 from sniffles_b200 import bamio, binding, synth, tasks, vcf
 from sniffles_b200 import config as sconfig
-from test_bgzf_write import _linear, _query, _file_blocks, parse_tbi
+from test_bgzf_write import _linear, _query, _text_starts, parse_tbi
 
 pytestmark = pytest.mark.gpu
 
@@ -29,7 +29,7 @@ def host(tmp_path_factory):
 
 
 def _starts(z: bytes):
-    return list(_file_blocks(z).keys())
+    return [o for o, *_ in bamio.bgzf_members(z)]
 
 
 def _check(ctx, host, data):
@@ -87,7 +87,7 @@ def test_call_task_to_indexed_vcf(tmp_path):
     assert gzip.decompress(out["calls.vcf.gz"]) == text
     names, refs = parse_tbi(gzip.decompress(open(tmp_path / "calls.vcf.gz.tbi", "rb").read()))
     assert names == blk.contig_names
-    starts = _file_blocks(out["calls.vcf.gz"][:-len(bamio._BGZF_EOF)])
+    starts = _text_starts(out["calls.vcf.gz"][:-len(bamio._BGZF_EOF)])
     for name, L in contigs:
         for beg in range(0, L, L // 50):
             assert _query(text, starts, names, refs, name, beg, beg + 20_000) == _linear(text, name, beg, beg + 20_000)

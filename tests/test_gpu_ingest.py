@@ -7,7 +7,6 @@ import numpy as np
 import pytest
 
 import devcheck
-import ingest_emul
 from sniffles_b200 import abi, bamio, binding, synth
 from sniffles_b200 import config as sconfig
 
@@ -30,18 +29,10 @@ def ctx():
     c.close()
 
 
-def _bgzf_member(data: bytes, level=6, strategy=zlib.Z_DEFAULT_STRATEGY) -> bytes:
-    import struct
-    c = zlib.compressobj(level, zlib.DEFLATED, -15, 8, strategy)
-    comp = c.compress(data) + c.flush()
-    return (b"\x1f\x8b\x08\x04\x00\x00\x00\x00\x00\xff\x06\x00BC\x02\x00" + struct.pack("<H", len(comp) + 25) + comp
-            + struct.pack("<II", zlib.crc32(data) & 0xffffffff, len(data)))
-
-
 def test_inflate_equals_zlib(bam, ctx):
     _, path = bam
     z = open(path, "rb").read()
-    want = b"".join(zlib.decompress(z[po:po + pl], -15) for _, po, pl, _ in ingest_emul.walk_bgzf(z))
+    want = b"".join(zlib.decompress(z[po:po + pl], -15) for _, po, pl, _ in bamio.bgzf_members(z))
     got = ctx.inflate_bgzf(np.frombuffer(z, "u1"))
     assert got == want and len(got) > 5_000_000
 
@@ -56,7 +47,7 @@ def test_inflate_block_kinds(ctx):
     for d in datas:
         for level in (0, 1, 6, 9):
             for strat in (zlib.Z_DEFAULT_STRATEGY, zlib.Z_FIXED, zlib.Z_HUFFMAN_ONLY, zlib.Z_RLE):
-                m = _bgzf_member(d, level, strat)
+                m = bamio._bgzf_block(d, level, strat)
                 if len(m) <= 65536:
                     members.append(m)
                     want.append(d)
@@ -67,7 +58,7 @@ def test_inflate_block_kinds(ctx):
 def test_corrupt_block_fails_cleanly(bam, ctx):
     _, path = bam
     z = bytearray(open(path, "rb").read())
-    blocks = ingest_emul.walk_bgzf(bytes(z))
+    blocks = list(bamio.bgzf_members(z))
     _, po, pl, _ = blocks[len(blocks) // 2]
     for k in range(po + 20, po + 60):
         z[k] ^= 0x5a
