@@ -326,15 +326,6 @@ uint64_t snfb_pack_cigar16(const snfb_rec* rec_in, uint64_t n_rec, const uint32_
     return total;
 }
 
-// thread per record: every offset of the block must stay inside its arena / table (ADVICE r1: a malformed block fails instead of reading out of bounds)
-__global__ void k_validate(const snfb_rec* __restrict__ rec, uint32_t n_rec, uint32_t n_task, uint64_t n_cigar, uint64_t n_var, uint64_t n_seq, int check_seq, DevCounters* ctr) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; if (i >= n_rec) return;
-    const snfb_rec r = rec[i];
-    bool bad = r.task < 0 || (uint32_t)r.task >= n_task || (r.cigar_off & 7) || r.cigar_off + (uint64_t)r.n_cigar > n_cigar || r.var_off + (uint64_t)r.l_qname + r.sa_len > n_var || r.l_seq < 0;
-    if (check_seq && r.l_seq >= 0 && r.seq_off + (uint64_t)((r.l_seq + 1) / 2) > n_seq) bad = true;
-    if (bad) atomicAdd(&ctr->bad_records, 1ULL);
-}
-
 // host-side checks of the small tables of a block
 static int check_tables(snfb_ctx* ctx, const snfb_records* R) {
     for (uint32_t t = 0; t < R->n_task; ++t) {
@@ -721,11 +712,11 @@ static int enqueue_stage_a(snfb_ctx* ctx) {
     }
     mark(ctx, "k_rec_index");
     if (nrec) {
-        launch(ctx->launches, k_validate, (unsigned)((nrec + 255) / 256), 256, 0, st, ctx->d_rec, (uint32_t)nrec, nt, ctx->n_cigar, ctx->n_var, ctx->n_seq, ctx->seq_on_demand ? 0 : 1, ctr);
         extract::IndexParams I{};
         I.rec = ctx->d_rec; I.cigar = ctx->d_cigar; I.task = b.task; I.n_rec = (uint32_t)nrec; I.n_task = nt; I.rec_pos = ctx->rec_pos; I.task_first = ctx->task_first; I.task_last = ctx->task_last;
         I.scan = ctx->scanrec; I.clip = ctx->clip; I.rec_end = ctx->rec_end; I.rec_flags = ctx->rec_flags; I.rec_nm = ctx->rec_nm; I.rec_nlead = ctx->rec_nlead; I.ctr = ctr;
-        I.mapq_min = cf.mapq; I.alen_min = cf.min_alignment_length; I.excl = cf.exclude_flags; I.want_nm = (cf.qc_nm_measure || cf.phase) ? 1 : 0; I.n_cigar = ctx->n_cigar;
+        I.mapq_min = cf.mapq; I.alen_min = cf.min_alignment_length; I.excl = cf.exclude_flags; I.want_nm = (cf.qc_nm_measure || cf.phase) ? 1 : 0;
+        I.n_cigar = ctx->n_cigar; I.n_var = ctx->n_var; I.n_seq = ctx->n_seq; I.check_seq = ctx->seq_on_demand ? 0 : 1;
         I.sa_list = ctx->sa_list; I.n_sa = &ctr->n_sa;
         launch(ctx->launches, extract::k_rec_index, (unsigned)((nrec + 255) / 256), 256, 0, st, I);
         // the CIGAR walk: bytes = the CIGAR16 arena (bench.py counts the passing records' groups)

@@ -238,7 +238,7 @@ __device__ __noinline__ unsigned process_sa(const snfb_config* __restrict__ cfgp
 
 // ================================================================================================
 // Stage A kernels:
-//   k_rec_index (thread per record): task boundaries, sortedness, and everything that only needs the record core and the
+//   k_rec_index (thread per record): the record's offset checks, task boundaries, sortedness, and everything that only needs the record core and the
 //           clip ops at the two ends of its CIGAR: query_alignment_start/end, the read filters of iter_region, the
 //           16-byte scan descriptor and the clip facts k_emit / k_sa use, the SA work list.
 //   k_cigar_walk (hot, HBM-bound): the CIGAR walk, see "stage A streaming: the CIGAR walk" below: reference end, the NM correction,
@@ -277,20 +277,66 @@ struct RecClip { int32_t alen, qas, clip_left, clip_right; };                   
 constexpr uint32_t RM_PASS = 1u << 24, RM_HAS_NM = 1u << 25, RM_HAS_SA = 1u << 26;   // RecScan.meta: task (0..15) | mapq (16..23) | flags | hp (27..28)
 
 struct IndexParams {
-    const snfb_rec* rec; const uint16_t* cigar; const snfb_task* task; uint32_t n_rec; uint32_t n_task; unsigned long long n_cigar;
+    const snfb_rec* rec; const uint16_t* cigar; const snfb_task* task; uint32_t n_rec; uint32_t n_task; unsigned long long n_cigar, n_var, n_seq;
+    int check_seq;                                    // the seq arena is resident: seq offsets are checked too
     int32_t* rec_pos; uint32_t* task_first; uint32_t* task_last;
     RecScan* scan; RecClip* clip; int32_t* rec_end; uint8_t* rec_flags; double* rec_nm; uint32_t* rec_nlead;
     uint32_t* sa_list; unsigned long long* n_sa;     // passing records with an SA tag (k_sa's work list)
     DevCounters* ctr; int mapq_min, alen_min, excl, want_nm;
 };
-// leadprov.py:488-516 (filters), pysam query_alignment_start / query_alignment_end; returns whether record i goes on the SA list
+
+// the clip ops at the two ends of a CIGAR16 record of n words, word(k) = word k: query_alignment_start / end (qas, qae, starting from
+// 0 and l_seq) and the first / last op's length when it is a clip.  Pad words (0) are skipped; an op's extension words follow its base word.
+template <class Word>
+__device__ __forceinline__ void clip_walk(uint32_t n, Word&& word, int& qas, int& qae, int& clip_left, int& clip_right) {
+    uint32_t fe = 0;
+    { bool first = true; uint32_t k = 0;
+      while (k < n) {
+          const unsigned w = word(k); if (w == 0) { ++k; continue; }
+          unsigned len = w & C16_LEN_MASK; const unsigned cls = c16_word_class(w); uint32_t k2 = k + 1;
+          while (k2 < n) { const unsigned e = word(k2); if (!(e & C16_EXT)) break; len += c16_ext_add(e); ++k2; }
+          if (first) { if (cls == C16_S || cls == C16_H) clip_left = (int)len; first = false; fe = k2; }
+          if (cls == C16_S) qas += (int)len; else if (cls != C16_H) break;
+          k = k2;
+      } }
+    { bool last = true; long k = (long)n - 1;
+      while (k >= (long)fe) {
+          long b = k; while (b > (long)fe && (word((uint32_t)b) & C16_EXT)) --b;
+          const unsigned w = word((uint32_t)b); if (w == 0) { k = b - 1; continue; }
+          unsigned len = w & C16_LEN_MASK; const unsigned cls = c16_word_class(w);
+          for (long e2 = b + 1; e2 <= k; ++e2) len += c16_ext_add(word((uint32_t)e2));
+          if (last) { if (cls == C16_S || cls == C16_H) clip_right = (int)len; last = false; }
+          if (cls == C16_S) qae -= (int)len; else if (cls != C16_H) break;
+          k = b - 1;
+      }
+      if (last) clip_right = clip_left; }            // a single op is both the first and the last one
+}
+// word k of a record when it lies in its first group (f: words 0..7) or its last group (l: words l0..l0+7).  Otherwise `miss` is set and
+// the word is a zero-length M, which ends either walk at once.  An op never straddles a group, so the clip walk stays inside these two
+// groups unless the clips at an end take more than one group.
+__device__ __forceinline__ unsigned end_word(const uint4& f, const uint4& l, uint32_t l0, uint32_t k, bool& miss) {
+    const bool in_f = k < 8u, in_l = k >= l0;
+    if (!in_f && !in_l) miss = true;
+    const uint4 v = in_f ? f : l; const uint32_t h = (k & 7u) >> 1;
+    const uint32_t x = h < 2u ? (h ? v.y : v.x) : (h == 2u ? v.z : v.w);
+    return (in_f || in_l) ? (x >> (16u * (k & 1u))) & 0xffffu : C16_M << C16_CLASS_SHIFT;
+}
+
+// leadprov.py:488-516 (filters), pysam query_alignment_start / query_alignment_end; returns whether record i goes on the SA list.
+// Also checks that every offset of the record stays inside its arena or table; a record that does not is counted in bad_records (the run fails).
 __device__ __forceinline__ bool index_record(const IndexParams& P, uint32_t i) {
     const uint4* core = reinterpret_cast<const uint4*>(P.rec + i);
-    const uint4 c0 = __ldg(core), c1 = __ldg(core + 1), c2 = __ldg(core + 2);
+    const uint4 c0 = __ldg(core), c1 = __ldg(core + 1), c2 = __ldg(core + 2), c3 = __ldg(core + 3);
     const int task = (int)c0.x, pos = (int)c0.y; const unsigned flag = c0.z & 0xffffu, mapq = (c0.z >> 16) & 255u, aux = c0.z >> 24; unsigned hp = c0.w & 255u;
-    const int nm = (int)c1.x; const uint32_t n = c1.z; const int l_seq = (int)c1.w;
+    const uint32_t l_qname = (c0.w >> 8) & 255u;
+    const int nm = (int)c1.x; const uint32_t n = c1.z; const int l_seq = (int)c1.w; const uint32_t sa_len = c2.x;
     const unsigned long long cigar_off = (unsigned long long)c2.z | ((unsigned long long)c2.w << 32);
-    if ((uint32_t)task >= P.n_task || (cigar_off & 7) || cigar_off + n > P.n_cigar) {      // malformed record (counted by k_validate: the run fails); touch nothing through its offsets
+    const unsigned long long seq_off = (unsigned long long)c3.x | ((unsigned long long)c3.y << 32), var_off = (unsigned long long)c3.z | ((unsigned long long)c3.w << 32);
+    const bool bad_core = (uint32_t)task >= P.n_task || (cigar_off & 7) || cigar_off + n > P.n_cigar;
+    const bool bad = bad_core || var_off + l_qname + sa_len > P.n_var || l_seq < 0
+                     || (P.check_seq && seq_off + (unsigned long long)((l_seq + 1) / 2) > P.n_seq);
+    if (bad) atomicAdd(&P.ctr->bad_records, 1ULL);
+    if (bad_core) {                                  // touch nothing through its offsets
         RecScan s; s.cig8 = 0; s.n_words = 0; s.pos = pos; s.meta = 0; store16(P.scan + i, s);
         RecClip c; c.alen = 0; c.qas = 0; c.clip_left = 0; c.clip_right = 0; store16(P.clip + i, c);
         P.rec_pos[i] = pos; P.rec_flags[i] = 0; P.rec_nm[i] = -1.0; P.rec_end[i] = -1; P.rec_nlead[i] = 0; return false;
@@ -299,29 +345,17 @@ __device__ __forceinline__ bool index_record(const IndexParams& P, uint32_t i) {
     if (i == 0) P.task_first[task] = 0;
     else { const int2 pv = __ldg(reinterpret_cast<const int2*>(P.rec + i - 1)); if (pv.x != task) { P.task_first[task] = i; if ((uint32_t)pv.x < P.n_task) P.task_last[pv.x] = i; } else if (pv.y > pos) atomicAdd(&P.ctr->unsorted, 1ULL); }
     if (i + 1 == P.n_rec) P.task_last[task] = P.n_rec;
-    // clips at the two ends
+    // clips at the two ends: from the first and the last group (two independent loads), word by word only when the clips leave them
     const uint16_t* cg = P.cigar + cigar_off;
-    int qas = 0, qae = l_seq, clip_left = 0, clip_right = 0; uint32_t fe = 0;
-    { bool first = true; uint32_t k = 0;
-      while (k < n) {
-          const unsigned w = __ldg(cg + k); if (w == 0) { ++k; continue; }
-          unsigned len = w & C16_LEN_MASK; const unsigned cls = c16_word_class(w); uint32_t k2 = k + 1;
-          while (k2 < n) { const unsigned e = __ldg(cg + k2); if (!(e & C16_EXT)) break; len += c16_ext_add(e); ++k2; }
-          if (first) { if (cls == C16_S || cls == C16_H) clip_left = (int)len; first = false; fe = k2; }
-          if (cls == C16_S) qas += (int)len; else if (cls != C16_H) break;
-          k = k2;
-      } }
-    { bool last = true; long k = (long)n - 1;
-      while (k >= (long)fe) {
-          long b = k; while (b > (long)fe && (__ldg(cg + b) & C16_EXT)) --b;
-          const unsigned w = __ldg(cg + b); if (w == 0) { k = b - 1; continue; }
-          unsigned len = w & C16_LEN_MASK; const unsigned cls = c16_word_class(w);
-          for (long e2 = b + 1; e2 <= k; ++e2) { const unsigned e = __ldg(cg + e2); len += c16_ext_add(e); }
-          if (last) { if (cls == C16_S || cls == C16_H) clip_right = (int)len; last = false; }
-          if (cls == C16_S) qae -= (int)len; else if (cls != C16_H) break;
-          k = b - 1;
-      }
-      if (last) clip_right = clip_left; }            // a single op is both the first and the last one
+    int qas = 0, qae = l_seq, clip_left = 0, clip_right = 0;
+    const uint32_t G = (n + 7u) >> 3;
+    bool miss = G == 0 || cigar_off + 8ull * G > P.n_cigar;          // the last group would end behind the arena: word by word
+    if (!miss) {
+        const uint4* g4 = reinterpret_cast<const uint4*>(cg);
+        const uint4 f = __ldg(g4), l = __ldg(g4 + (G - 1u)); const uint32_t l0 = 8u * (G - 1u);
+        clip_walk(n, [&](uint32_t k) { return end_word(f, l, l0, k, miss); }, qas, qae, clip_left, clip_right);
+    }
+    if (miss) { qas = 0; qae = l_seq; clip_left = 0; clip_right = 0; clip_walk(n, [&](uint32_t k) { return (unsigned)__ldg(cg + k); }, qas, qae, clip_left, clip_right); }
     const int alen = qae - qas;
     const snfb_task tk = P.task[task];
     const bool pass = !((int)mapq < P.mapq_min || (flag & 256u) || alen < P.alen_min) && !(P.excl && (flag & (unsigned)P.excl)) && pos >= tk.start && pos < tk.end && n > 0;
@@ -470,6 +504,12 @@ __device__ __forceinline__ void group_events(const uint4 v, uint32_t q0, int r0,
     }
 }
 
+// a read-only 16-byte load whose L2 miss fetches the whole 256-byte block around it: a lane's chunk is up to 256 contiguous bytes, so its first
+// load brings the rest of the chunk into L2 at once instead of one 32-byte sector per later load
+__device__ __forceinline__ uint4 ldg_l2_256(const uint4* p) {
+    uint4 v; asm("ld.global.nc.L2::256B.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p)); return v;
+}
+
 template <int TILE>
 __global__ void __launch_bounds__(WALK_THREADS, 4) k_cigar_walk(const __grid_constant__ WalkParams P) {
     // per warp, in shared memory to keep them out of the registers of the load loop: the tile's RecScans (cig8, n_words, pos, meta), and the
@@ -508,7 +548,7 @@ __global__ void __launch_bounds__(WALK_THREADS, 4) k_cigar_walk(const __grid_con
                 for (int gb = 0; gb < ng; gb += 8) {
                     uint4 v[8];
                     #pragma unroll
-                    for (int g = 0; g < 8; ++g) v[g] = gb + g < ng ? __ldg(src + gb + g) : make_uint4(0u, 0u, 0u, 0u);
+                    for (int g = 0; g < 8; ++g) v[g] = gb + g < ng ? ldg_l2_256(src + gb + g) : make_uint4(0u, 0u, 0u, 0u);
                     uint32_t aq = 0, ar = 0, ext = 0;
                     #pragma unroll
                     for (int g = 0; g < 8; ++g) {
