@@ -301,7 +301,8 @@ typedef struct snfb_seq_view {
 typedef struct snfb_ctx snfb_ctx;
 
 int         snfb_version(void);
-/* sizeof of the ABI structs, for binding self-checks: 0 rec, 1 task, 2 contig, 3 records, 4 config, 5 lead, 6 cand, 7 gather_view */
+/* sizeof of the ABI structs, for binding self-checks: 0 rec, 1 task, 2 contig, 3 records, 4 config, 5 lead, 6 cand, 7 gather_view,
+ * 8 gt_in, 9 gt_out */
 size_t      snfb_sizeof(int which);
 uint64_t    snfb_hash_name(const char* s, size_t n);
 int         snfb_ctx_create(int device, snfb_ctx** out);
@@ -376,6 +377,27 @@ uint64_t    snfb_rerun_count(snfb_ctx* ctx);
  * *out is a library-owned buffer of *n_bins doubles, valid until the next call on the ctx.  Needs snfb_extract_leads
  * (or snfb_run) first. */
 int         snfb_coverage_bins(snfb_ctx* ctx, uint32_t task, int binsize, const double** out, uint64_t* n_bins);
+/* ---- force calling (--genotype-vcf; GenotypeTask.execute, parallel.py:300-369) ----
+ * Runs after snfb_run (or snfb_cluster_call) on the same context and changes nothing that call produced.  Targets are SoA host arrays,
+ * ordered by task and then by input order (a BND target takes the `end` of the previous non-BND target of its task, as
+ * postprocessing.coverage does).  svtype is SNFB_INS .. SNFB_BND, or -1 for a type the reference does not bin (not matched, still
+ * probed).  mate_contig is a contig-table index, -1 for a name the BAM header lacks (never matches).  A target is matched against the
+ * candidates of its task, svtype and 5000-bp bin (plus the neighbouring bin within 500 bp of an edge), SINGLE_* excluded:
+ * non-BND: dist = |dpos| + ||svlen_t| - |svlen_c|| with min(|svlen_t|, |svlen_c|) > 0, dist <= combine_match * sqrt(minlen) and
+ * dist <= combine_match_max; BND: dist = |dpos| <= cluster_merge_bnd (snfb_config) and equal mate contigs.  The smallest distance wins,
+ * ties go to the earlier candidate.  Outputs per target (host arrays): the candidate's index in the run's emission order (-1 none), the
+ * start / center / end coverage probes, and bnd_no_prev = 1 for a BND with no earlier non-BND target in its task (the reference's
+ * UnboundLocalError: that task fails).  Records a "genotype" timing mark. */
+typedef struct snfb_gt_in {
+    uint64_t n;
+    const int32_t* task; const int32_t* svtype; const int32_t* pos; const int32_t* svlen; const int32_t* bnd_is_first; const int32_t* mate_contig;
+    int32_t combine_match, combine_match_max;
+} snfb_gt_in;
+typedef struct snfb_gt_out {
+    int64_t* match;
+    int32_t* cov_start; int32_t* cov_center; int32_t* cov_end; int32_t* bnd_no_prev;
+} snfb_gt_out;
+int         snfb_genotype_targets(snfb_ctx* ctx, const snfb_gt_in* in, snfb_gt_out* out);
 
 /* ---- multi-GPU: one process per GPU, contigs sharded over the ranks, ONE all-gather of the per-rank candidate buffers ----
  * snfb_nccl_unique_id fills the 128 bytes of an ncclUniqueId on one rank; the host hands them to every rank (any transport),

@@ -161,6 +161,15 @@ class GatherView(C.Structure):
                 ("dev_buffer", C.c_void_p), ("dev_bytes_per_rank", C.c_uint64)]
 
 
+class GtIn(C.Structure):                                        # snfb_gt_in
+    _fields_ = [("n", C.c_uint64), ("task", C.c_void_p), ("svtype", C.c_void_p), ("pos", C.c_void_p), ("svlen", C.c_void_p),
+                ("bnd_is_first", C.c_void_p), ("mate_contig", C.c_void_p), ("combine_match", C.c_int32), ("combine_match_max", C.c_int32)]
+
+
+class GtOut(C.Structure):                                       # snfb_gt_out
+    _fields_ = [("match", C.c_void_p), ("cov_start", C.c_void_p), ("cov_center", C.c_void_p), ("cov_end", C.c_void_p), ("bnd_no_prev", C.c_void_p)]
+
+
 def view(ptr, dtype, n):
     """numpy array over library-owned memory (no copy); empty array for n == 0 / NULL."""
     dtype = np.dtype(dtype)

@@ -17,7 +17,8 @@ EXPORTS = ["snfb_version", "snfb_sizeof", "snfb_hash_name", "snfb_ctx_create", "
            "snfb_last_timings", "snfb_device_candidates", "snfb_device_alt", "snfb_launch_count",
            "snfb_pin_host", "snfb_unpin_host", "snfb_pack_cigar16", "snfb_rerun_count", "snfb_coverage_bins",
            "snfb_nccl_unique_id", "snfb_comm_init", "snfb_allgather_candidates", "snfb_selftest_sqrt_frac", "snfb_poa", "snfb_combine_groups", "snfb_selftest_edit_distance",
-           "snfb_load_bam", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf", "snfb_deflate_bgzf"]
+           "snfb_load_bam", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf", "snfb_deflate_bgzf",
+           "snfb_genotype_targets"]
 
 
 def lib():
@@ -61,6 +62,7 @@ def lib():
         L.snfb_comm_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
         L.snfb_allgather_candidates.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(abi.GatherView)]
         L.snfb_poa.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
+        L.snfb_genotype_targets.argtypes = [C.c_void_p, C.POINTER(abi.GtIn), C.POINTER(abi.GtOut)]
         L.snfb_combine_groups.argtypes = [C.c_void_p, C.POINTER(abi.CombineIn), C.POINTER(abi.CombineOut)]
         L.snfb_selftest_edit_distance.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
         L.snfb_selftest_sqrt_frac.restype = C.c_double
@@ -288,6 +290,23 @@ class Context:
         n = C.c_uint64()
         self._check(self._lib.snfb_coverage_bins(self._h, int(task), int(binsize), C.byref(p), C.byref(n)), "snfb_coverage_bins")
         return abi.view(p.value, "<f8", n.value).copy()
+
+    def genotype_targets(self, task, svtype, pos, svlen, bnd_is_first, mate_contig, combine_match, combine_match_max):
+        """Force calling on the device (snfb_genotype_targets) after `run` / `cluster_call` on this context.  Targets as int32 arrays,
+        ordered by task then input order.  Returns (match, cov_start, cov_center, cov_end, bnd_no_prev): match = the candidate's index
+        in the run's emission order (int64, -1 none); bnd_no_prev = 1 for a BND with no earlier non-BND target in its task."""
+        cols = [np.ascontiguousarray(a, dtype="<i4") for a in (task, svtype, pos, svlen, bnd_is_first, mate_contig)]
+        n = len(cols[0])
+        if any(len(a) != n for a in cols):
+            raise ValueError("genotype_targets: the target arrays differ in length")
+        out = (np.full(n, -1, "<i8"),) + tuple(np.zeros(n, "<i4") for _ in range(4))
+        I, O = abi.GtIn(), abi.GtOut()
+        I.n = n
+        I.task, I.svtype, I.pos, I.svlen, I.bnd_is_first, I.mate_contig = (a.ctypes.data for a in cols)
+        I.combine_match, I.combine_match_max = int(combine_match), int(combine_match_max)
+        O.match, O.cov_start, O.cov_center, O.cov_end, O.bnd_no_prev = (a.ctypes.data for a in out)
+        self._check(self._lib.snfb_genotype_targets(self._h, C.byref(I), C.byref(O)), "snfb_genotype_targets")
+        return out
 
     def comm_init(self, unique_id: bytes, rank: int, nranks: int):
         """Join the NCCL communicator of the per-GPU processes (the 128-byte id comes from `nccl_unique_id()` on one rank)."""

@@ -209,7 +209,9 @@ class SnifflesConfig(argparse.Namespace):
                 self.cluster_merge_len = self.default_cluster_merge_len_mosaic
         if self.dev_min_leads_cluster == -1:
             self.dev_min_leads_cluster = 1 if self.no_qc else 2
-        self.mode = "call_sample"
+        self.mode = "call_sample" if self.genotype_vcf is None else "genotype_vcf"
+        if self.mode != "call_sample" and self.snf is not None:
+            raise SystemExit(f"--snf cannot be used with run mode {self.mode}")
         self.qc_nm_threshold = 0.0
         self.average_regional_nm = 0.0
         self.dev_trace_read = False

@@ -26,6 +26,7 @@
 #include "combine.cuh"
 #include "ingest.cuh"
 #include "bgzf_write.cuh"
+#include "genotype.cuh"
 
 // one owning allocation of device memory, or of pinned host memory when Pinned; freed by the destructor
 template <bool Pinned> struct Buf {
@@ -100,6 +101,7 @@ struct snfb_ctx {
     HostBuf h_c16, h_rec16;        // BAM32 host input converted to CIGAR16 before the upload
     DevBuf b_comp, b_raw, b_ing, b_ing_work; HostBuf h_ing; uint64_t ing_sizes[8] = {0, 0, 0, 0, 0, 0, 0, 0}; bool from_bam = false;      // device BAM ingest: BGZF bytes, inflated stream, block / span tables, per-raw-record work arrays
     DevBuf b_zin, b_zslot, b_zout, b_zwork;          // BGZF compression: input bytes, 64 KiB member slots, packed members, sizes / offsets / candidate scratch
+    DevBuf b_gt;                                     // force calling: candidate bin keys, sort scratch, targets and their results
     std::vector<snfb_task> tasks;
     // capacities and the three arenas carved by them
     Caps cap; bool force_no_cuts = false;
@@ -233,7 +235,8 @@ extern "C" {
 int snfb_version(void) { return SNFB_ABI_VERSION; }
 size_t snfb_sizeof(int which) {
     switch (which) { case 0: return sizeof(snfb_rec); case 1: return sizeof(snfb_task); case 2: return sizeof(snfb_contig); case 3: return sizeof(snfb_records);
-                     case 4: return sizeof(snfb_config); case 5: return sizeof(snfb_lead); case 6: return sizeof(snfb_cand); case 7: return sizeof(snfb_gather_view); default: return 0; }
+                     case 4: return sizeof(snfb_config); case 5: return sizeof(snfb_lead); case 6: return sizeof(snfb_cand); case 7: return sizeof(snfb_gather_view);
+                     case 8: return sizeof(snfb_gt_in); case 9: return sizeof(snfb_gt_out); default: return 0; }
 }
 
 uint64_t snfb_hash_name(const char* s, size_t n) {
@@ -1263,6 +1266,61 @@ int snfb_coverage_bins(snfb_ctx* ctx, uint32_t task, int binsize, const double**
     double* o = ctx->h_cov_bins.as<double>();
     for (long long i = 0; i < nb; ++i) o[i] = (double)raw[i] / (double)binsize;
     *out = o; *n_bins = (uint64_t)nb; return 0;
+}
+
+// force calling (GenotypeTask.execute, parallel.py:300-369): targets matched against the resident candidates, plus their coverage probes
+int snfb_genotype_targets(snfb_ctx* ctx, const snfb_gt_in* in, snfb_gt_out* out) {
+    if (!ctx || !in || !out) return ctx ? fail(ctx, "snfb_genotype_targets: null argument") : 1;
+    if (!ctx->stage_b_done) return fail(ctx, "snfb_genotype_targets: snfb_run or snfb_cluster_call must run first");
+    const uint64_t n = in->n;
+    if (n == 0) return 0;
+    if (!in->task || !in->svtype || !in->pos || !in->svlen || !in->bnd_is_first || !in->mate_contig || !out->match || !out->cov_start || !out->cov_center || !out->cov_end || !out->bnd_no_prev)
+        return fail(ctx, "snfb_genotype_targets: null array");
+    // the leaked `end` of a BND comes from the last non-BND target of its task before it: found here in one pass, so a long run of BNDs
+    // costs no walk on the device
+    std::vector<int64_t> prev(n);
+    int64_t last = -1;
+    for (uint64_t i = 0; i < n; ++i) {
+        if (in->task[i] < 0 || (uint32_t)in->task[i] >= ctx->n_task) return fail(ctx, "snfb_genotype_targets: target task out of range");
+        if (i && in->task[i] < in->task[i - 1]) return fail(ctx, "snfb_genotype_targets: targets are not ordered by task");
+        if (in->svtype[i] < -1 || in->svtype[i] > SNFB_BND) return fail(ctx, "snfb_genotype_targets: target svtype must be SNFB_INS .. SNFB_BND or -1");
+        if (i && in->task[i] != in->task[i - 1]) last = -1;
+        prev[i] = last;
+        if (in->svtype[i] != SNFB_BND) last = (int64_t)i;
+    }
+    cudaSetDevice(ctx->device);
+    const unsigned long long nc = ctx->h_fin->n_cand;
+    genotype::P G{}; uint64_t* k1 = nullptr; uint32_t* v1 = nullptr; prims::RadixTemp rt{};
+    int32_t* t_in = nullptr; uint64_t* k0 = nullptr; uint32_t* v0 = nullptr;
+    auto lay = [&](Carver& c) {
+        k0 = c.take<uint64_t>(nc + 1); v0 = c.take<uint32_t>(nc + 1); k1 = c.take<uint64_t>(nc + 1); v1 = c.take<uint32_t>(nc + 1);
+        rt.hist = c.take<uint32_t>(prims::radix_hist_elems(nc)); rt.scan_tmp = c.take<uint32_t>(prims::scan_tmp_elems(prims::radix_hist_elems(nc)) + 16);
+        t_in = c.take<int32_t>(6 * n); G.prev = c.take<int64_t>(n); G.match = c.take<long long>(n); G.cov_start = c.take<int32_t>(4 * n);
+    };
+    if (carve(ctx->b_gt, lay)) return fail(ctx, "snfb_genotype_targets: out of device memory");
+    G.task = t_in; G.svtype = t_in + n; G.pos = t_in + 2 * n; G.svlen = t_in + 3 * n; G.bnd_is_first = t_in + 4 * n; G.mate_contig = t_in + 5 * n;
+    G.cov_center = G.cov_start + n; G.cov_end = G.cov_start + 2 * n; G.bnd_no_prev = G.cov_start + 3 * n;
+    cudaStream_t st = ctx->st;
+    const int32_t* src[6] = { in->task, in->svtype, in->pos, in->svlen, in->bnd_is_first, in->mate_contig };
+    for (int k = 0; k < 6; ++k) CUDA_TRY(cudaMemcpyAsync(t_in + (size_t)k * n, src[k], 4 * n, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(const_cast<int64_t*>(G.prev), prev.data(), 8 * n, cudaMemcpyHostToDevice, st));
+    ctx->n_ev = 0;
+    mark(ctx, "genotype");
+    bool first = true;
+    if (nc) {
+        launch(ctx->launches, genotype::k_cand_keys, grid_for(nc, 256), 256, 0, st, ctx->B.cand, nc, k0, v0);
+        prims::radix_sort(ctx->launches, k0, v0, k1, v1, rt, &ctx->B.ctr->n_cand, nc, genotype::KEY_BITS + bits_for(ctx->n_task), &first, st);
+    }
+    G.b = ctx->B; G.key = first ? k0 : k1; G.val = first ? v0 : v1; G.n_cand = nc; G.n = n;
+    G.combine_match = in->combine_match; G.combine_match_max = in->combine_match_max; G.cluster_merge_bnd = ctx->cfg.cluster_merge_bnd;
+    launch(ctx->launches, genotype::k_genotype, grid_for(n * 32, 128), 128, 0, st, G);
+    mark(ctx, nullptr);
+    CUDA_TRY(cudaMemcpyAsync(out->match, G.match, 8 * n, cudaMemcpyDeviceToHost, st));
+    int32_t* dst[4] = { out->cov_start, out->cov_center, out->cov_end, out->bnd_no_prev };
+    for (int k = 0; k < 4; ++k) CUDA_TRY(cudaMemcpyAsync(dst[k], G.cov_start + (size_t)k * n, 4 * n, cudaMemcpyDeviceToHost, st));
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, std::string("snfb_genotype_targets: ") + cudaGetErrorString(e));
+    return 0;
 }
 
 }  // extern "C"

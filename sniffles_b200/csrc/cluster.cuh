@@ -888,25 +888,43 @@ __device__ inline void cov_at_warp(const B& b, int t, long long idx, int* out) {
     uint32_t c[3]; cover_count_warp(b, t, idx, c); *out = (int)((c[0] + c[1] + c[2]) & 0xffffu);
 }
 
+// what postprocessing.coverage reads of one call
+struct CovSv { int task, svtype; long long pos, svlen; int bnd_is_first; };
+// postprocessing.coverage's probe positions (postprocessing.py:69-130) of call i of a list ordered by task: p = upstream, start, center,
+// end, downstream.  `at(j)` returns call j; `prev(i)` the index of the last non-BND call of i's task before i, or -1.  A BND takes the
+// `end` left over from that call; with none the reference raises UnboundLocalError, and this returns false with end = start.  Any
+// svtype other than INS / BND (also an unsupported one, < 0) takes the interval branch.
+template <class At, class Prev> __device__ inline bool cov_probes(long long i, At at, Prev prev, long long bs, long long ud, long long p[5]) {
+    const CovSv c = at(i); long long start = c.pos, end; bool ok = true;
+    if (c.svtype == SNFB_INS) end = start + 1;
+    else if (c.svtype == SNFB_BND) {
+        if (c.bnd_is_first) start -= 1;
+        const long long j = prev(i);
+        if (j >= 0) { const CovSv q = at(j); end = q.svtype == SNFB_INS ? q.pos + 1 : q.pos + (q.svlen < 0 ? -q.svlen : q.svlen); }
+        else { end = start; ok = false; }
+    } else end = c.pos + (c.svlen < 0 ? -c.svlen : c.svlen);
+    if (c.svtype == SNFB_INS || c.svtype == SNFB_BND) { p[1] = start - bs; p[2] = start; p[3] = end + bs; }
+    else { p[1] = start; p[2] = (long long)__ddiv_rn((double)(start + end), 2.0); p[3] = end - bs; }
+    p[0] = start - ud; p[4] = end + ud;
+    return ok;
+}
+
 // postprocessing.coverage (postprocessing.py:69-130) including the `end` that leaks from the previous call,
 // plus the hap-REF counts of the cluster's first bin (cluster.py:255-260).  One warp per candidate.
 __global__ void k_coverage(B b) {
     const unsigned long long nc = b.ctr->n_cand < b.cand_cap ? b.ctr->n_cand : b.cand_cap;
     const long long bs = b.cfg.coverage_binsize, ud = (long long)b.cfg.coverage_binsize * b.cfg.coverage_updown_bins;
     const unsigned long long nw = ((unsigned long long)gridDim.x * blockDim.x) >> 5;
+    const auto at = [&](long long j) { const snfb_cand& q = b.cand[j]; return CovSv{ q.task, q.svtype, q.pos, q.svlen, q.bnd_is_first }; };
+    const auto prev = [&](long long i) {          // candidates of a task hold few BNDs in a row: walk back
+        const int t = b.cand[i].task; long long j = i - 1; while (j >= 0 && b.cand[j].task == t && b.cand[j].svtype == SNFB_BND) --j;
+        return j >= 0 && b.cand[j].task == t ? j : -1ll; };
     for (unsigned long long i = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < nc; i += nw) {
-        snfb_cand* c = &b.cand[i]; long long start = c->pos, end; const int t = c->task; const int svtype = c->svtype;
-        if (svtype == SNFB_INS) end = start + 1;
-        else if (svtype == SNFB_BND) {
-            if (c->bnd_is_first) start -= 1;
-            long long j = (long long)i - 1; while (j >= 0 && b.cand[j].task == t && b.cand[j].svtype == SNFB_BND) --j;
-            if (j >= 0 && b.cand[j].task == t) { const snfb_cand* p = &b.cand[j]; end = p->svtype == SNFB_INS ? (long long)p->pos + 1 : (long long)p->pos + (p->svlen < 0 ? -(long long)p->svlen : p->svlen); }
-            else { end = start; if (lane_id() == 0) atomicAdd(&b.ctr->soft_errors, 1ULL); }
-        } else end = (long long)c->pos + (c->svlen < 0 ? -(long long)c->svlen : c->svlen);
+        snfb_cand* c = &b.cand[i]; const int t = c->task;
+        long long p[5];
+        if (!cov_probes((long long)i, at, prev, bs, ud, p) && lane_id() == 0) atomicAdd(&b.ctr->soft_errors, 1ULL);
         int v[5] = { 0, 0, 0, 0, 0 };          // upstream, start, center, end, downstream
-        if (svtype == SNFB_INS || svtype == SNFB_BND) { cov_at_warp(b, t, start - bs, &v[1]); cov_at_warp(b, t, start, &v[2]); cov_at_warp(b, t, end + bs, &v[3]); }
-        else { cov_at_warp(b, t, start, &v[1]); cov_at_warp(b, t, (long long)__ddiv_rn((double)(start + end), 2.0), &v[2]); cov_at_warp(b, t, end - bs, &v[3]); }
-        cov_at_warp(b, t, start - ud, &v[0]); cov_at_warp(b, t, end + ud, &v[4]);
+        for (int k = 0; k < 5; ++k) cov_at_warp(b, t, p[k], &v[k]);
         uint32_t hr[3]; const int cb = b.cfg.cluster_binsize; cover_count_warp(b, t, (long long)(c->cluster_seed / cb) * cb + cb - 1, hr);
         if (lane_id() == 0) {
             c->cov_upstream = v[0]; c->cov_start = v[1]; c->cov_center = v[2]; c->cov_end = v[3]; c->cov_downstream = v[4];

@@ -74,6 +74,7 @@ class SVCall:                              # field surface of sv.SVCall (sv.py:8
     coverage_end: int = 0
     sample_internal_id: int = None
     bnd_info: SVCallBNDInfo = None
+    cand_index: int = None                 # index of the device candidate in the run's emission order (force calling maps matches by it)
 
     def set_info(self, k, v):
         self.info[k] = v
@@ -132,7 +133,7 @@ def calls_from_result(res, task_index, lo, hi, contig_names, task_contig, task_i
                       info=info, svtype=svtype, svlen=int(c["svlen"]), end=int(c["end"]), genotypes={}, precise=bool(c["precise"]),
                       support=int(c["support"]), rnames=None, qc=True, nm=float(c["nm_mean"]), postprocess=cv, fwd=int(c["fwd"]), rev=int(c["rev"]),
                       coverage_upstream=int(c["cov_upstream"]), coverage_downstream=int(c["cov_downstream"]), coverage_start=int(c["cov_start"]),
-                      coverage_center=int(c["cov_center"]), coverage_end=int(c["cov_end"]), bnd_info=bnd)
+                      coverage_center=int(c["cov_center"]), coverage_end=int(c["cov_end"]), bnd_info=bnd, cand_index=lo + k)
         if svtype == "INS" and int(c["alt_off"]) >= 0 and not config.symbolic:
             call.alt = res.alt[int(c["alt_off"]):int(c["alt_off"]) + int(c["alt_len"])].tobytes().decode()      # annotate_sv, done on the device
         out.append(call)

@@ -179,3 +179,21 @@ def config_block(index: int, scale: float = 1.0, threads: int = 0, with_seq: boo
                         len_min=5000, len_max=60000, tech="ont", sv_spacing=1000.0, ins_only=True, tr_frac=0.0,
                         clip_prob=0.0, sv_min=50, sv_max=5000, threads=threads, with_seq=with_seq)
     raise ValueError(f"no synthetic shape for BASELINE config {index}")
+
+
+def genotype_targets(cand, n_task, contig_len, rng, n):
+    """seeded force-calling targets as the int32 columns of snfb_gt_in (task, svtype, pos, svlen, bnd_is_first, mate_contig), ordered by
+    task: half are candidates jittered inside and beyond the matching limits (exact copies included), half random decoys and edge cases
+    (POS 0, the contig's last positions, bin edges, svlen 0, unsupported types, unknown mate contigs)"""
+    rows = []
+    for c in cand[rng.integers(0, len(cand), n // 2)]:
+        j = int(rng.choice([0, 0, 5, 50, 300, 1200]))
+        rows.append((int(c["task"]), int(c["svtype"]) if int(c["svtype"]) <= abi.BND else -1, int(c["pos"]) + int(rng.integers(-j, j + 1)),
+                     int(c["svlen"]) + int(rng.integers(-j, j + 1)), int(c["bnd_is_first"]), int(c["bnd_mate_contig"]) if rng.random() < 0.9 else -1))
+    for _ in range(n - len(rows)):
+        t = int(rng.integers(0, n_task))
+        L = int(contig_len[t])
+        pos = int(rng.choice([rng.integers(0, L), -1, 0, L - 2, int(rng.integers(0, L // 5000)) * 5000 + int(rng.choice([0, 499, 500, 4500, 4501, 4999]))]))
+        rows.append((t, int(rng.integers(-1, 5)), pos, int(rng.choice([0, rng.integers(-20000, 20000), 60])), int(rng.integers(0, 2)), int(rng.integers(-1, 3))))
+    rows.sort(key=lambda r: r[0])          # stable: input order inside a task
+    return np.array(rows, dtype=np.int64).T.astype(np.int32)

@@ -27,6 +27,7 @@ class BlockRun:
     result: object
     cand_range: list          # per task (lo, hi) into result.cand
     rec_nm: Optional[np.ndarray] = None
+    genotype: Optional[dict] = None   # per task index: snfb_genotype_targets results of the task's targets (genotype.device_targets)
 
 
 def run_block(block, config, device: int = 0, ctx=None) -> BlockRun:
@@ -207,3 +208,46 @@ class CallTask(Task):
             calls = sorted(calls, key=lambda c: c.pos)
         self.result = calls
         return calls, read_count
+
+
+class GenotypeTaskError(RuntimeError):
+    """the task fails as the reference's worker fails it: its targets are not written"""
+
+
+class GenotypeTask(Task):
+    def label(self):
+        return f"GenotypeTask(id={self.id}, contig={self.contig}, start={self.start}, end={self.end})"
+
+    def execute(self, worker=None):
+        """parallel.py:300-369: candidates finalized with QC fails kept, each target matched to the nearest candidate of its bins and
+        probed for coverage on the device (snfb_genotype_targets), then genotyped.  Returns (targets, read_count)."""
+        from . import genotype
+        config = self.config
+        self.bind(worker)
+        _, read_count = self.build_leadtab()
+        cands = self.call_candidates(False, config)
+        calls = self.finalize_candidates(cands, True, config)
+        targets = list(self.genotype_svs or [])
+        seen = False
+        for c in calls:          # postprocessing.coverage over the candidates raises UnboundLocalError before any target is looked at
+            if c.svtype == "BND" and not seen:
+                raise GenotypeTaskError(f"candidate {c.id} is a BND with no earlier non-BND candidate in its task")
+            seen = seen or c.svtype != "BND"
+        for t in targets:
+            if t.svtype not in genotype.SVTYPE_CODE:
+                genotype.log.warning(f"Unsupported SVTYPE: {t.svtype}")
+        br = self.block_run
+        if br.genotype is not None and self.task_index in br.genotype:
+            res = br.genotype[self.task_index]
+        else:
+            res = genotype.device_targets(self._ctx(), [(self.task_index, targets)], {n: i for i, n in enumerate(br.block.contig_names)}, config)[self.task_index]
+        match, cov_start, cov_center, cov_end, bnd_no_prev = res
+        if bnd_no_prev.any():
+            # postprocessing.coverage raises UnboundLocalError for a BND with no earlier non-BND target in the task (postprocessing.py:81-90)
+            raise GenotypeTaskError(f"BND target at line {targets[int(np.argmax(bnd_no_prev))].raw_vcf_line_index} has no earlier non-BND target in its task")
+        by_index = {c.cand_index: c for c in calls}
+        for t, m, s, c, e in zip(targets, match.tolist(), cov_start.tolist(), cov_center.tolist(), cov_end.tolist()):
+            t.genotype_match_sv = by_index[m] if m >= 0 else None
+            t.coverage_start, t.coverage_center, t.coverage_end = s, c, e
+        self.result = targets
+        return targets, read_count
