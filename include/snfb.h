@@ -23,6 +23,9 @@
  *   snfb_poa               <- spoa.poa as LocalAsm.assembly calls it (local_asm.py:287-291); call site parallel.py:186-196
  *   snfb_coverage_bins     <- SNFile.annotate_block_coverages' reshape-mean of lead_provider.coverage
  *                             (snf.py:248-267)
+ *   snfb_load_reference / snfb_reference_runs / snfb_fetch_reference
+ *                          <- pysam.FastaFile behind LeadProvider._mask_N_coverage (leadprov.py:420-443) and
+ *                             VCF.open_reference / write_call (vcf.py:108-119, 299-342)
  *   snfb_allgather_candidates <- the parent collecting every worker's finished task results before VCF
  *                             emission (sniffles:544-547, parallel.py:270-271), as one NCCL all-gather
  *
@@ -302,7 +305,7 @@ typedef struct snfb_ctx snfb_ctx;
 
 int         snfb_version(void);
 /* sizeof of the ABI structs, for binding self-checks: 0 rec, 1 task, 2 contig, 3 records, 4 config, 5 lead, 6 cand, 7 gather_view,
- * 8 gt_in, 9 gt_out */
+ * 8 gt_in, 9 gt_out, 10 ref_contig, 11 ref_input, 12 ref_query */
 size_t      snfb_sizeof(int which);
 uint64_t    snfb_hash_name(const char* s, size_t n);
 int         snfb_ctx_create(int device, snfb_ctx** out);
@@ -477,6 +480,44 @@ int         snfb_combine_groups(snfb_ctx* ctx, const snfb_combine_in* in, snfb_c
 double      snfb_selftest_sqrt_frac(uint64_t p_hi, uint64_t p_lo, uint64_t q, int slow);
 /* self-check of the device edit distance behind group.align_call: n_pairs pairs (a_off/a_len, b_off/b_len into bytes[]), distances to out[] */
 int         snfb_selftest_edit_distance(snfb_ctx* ctx, const uint8_t* bytes, uint64_t n_bytes, const uint64_t* a_off, const uint32_t* a_len, const uint64_t* b_off, const uint32_t* b_len, uint32_t n_pairs, int32_t* out);
+/* ---- the reference FASTA (--reference) on the device ----
+ * snfb_load_reference  <- pysam.FastaFile(config.reference) as LeadProvider._mask_N_coverage and VCF.open_reference open it
+ *                         (leadprov.py:420-443, vcf.py:108-119): the bytes of the file (plain text, or whole BGZF members back to back with
+ *                         is_bgzf = 1, inflated and CRC-checked on the device as snfb_load_bam does) and per contig its .fai geometry with
+ *                         the raw offset rebased to those bytes (their inflated stream for BGZF).  Contig c becomes the newline-free bases
+ *                         raw[offset + (p / linebases) * linewidth + p % linebases], p < length, kept byte for byte (case, IUPAC codes).
+ *                         Every line that more sequence follows must end in "\n" (linewidth = linebases + 1) or "\r\n" (+ 2) and no base
+ *                         may be a line break; otherwise the call fails naming the contig index and the line of the first violation (a
+ *                         stale .fai, which htslib would read as wrong bases).  The maximal runs of 'N' (upper case only: leadprov.py:439
+ *                         compares with 78) are computed on the device.  The genome stays resident on the context, replacing any earlier
+ *                         one, until the next call or snfb_ctx_destroy; the raw stream is not kept.  Timing marks: h2d_ref, inflate
+ *                         (BGZF), ref_unwrap, ref_nruns.
+ * snfb_reference_runs  <- the `mask == 78` of _mask_N_coverage (leadprov.py:439): the runs as int32 (start, end) pairs, sorted per contig,
+ *                         contig c owning runs[contig_off[c] .. contig_off[c + 1]); library-owned host arrays valid until the next call on
+ *                         the context.  They enter a block through the N-mask tables of snfb_records / snfb_bam_input.
+ * snfb_fetch_reference <- FastaFile.fetch(contig, start, end) of VCF.write_call (vcf.py:304-338): n resolved queries, one gather on the device
+ *                         and one device -> host copy into out (query k fills out[out_off .. + length)).  The caller applies pysam's rules
+ *                         (clipping, empty and invalid intervals) first: a query outside its contig fails the call. */
+typedef struct snfb_ref_contig {
+    uint64_t offset;          /* raw byte offset of the first base (the .fai OFFSET, rebased to the bytes given)   */
+    uint64_t length;          /* bases (.fai LENGTH, < 2^31)                                                       */
+    uint32_t linebases;       /* bases per line (.fai LINEBASES; may be 0 only when length is 0)                   */
+    uint32_t linewidth;       /* bytes per line with its terminator (.fai LINEWIDTH)                               */
+} snfb_ref_contig;
+typedef struct snfb_ref_input {
+    const uint8_t* bytes; uint64_t n_bytes;
+    uint32_t is_bgzf;         /* 0 plain text, 1 whole BGZF members                                                */
+    uint32_t n_contig;
+    const snfb_ref_contig* contig;
+} snfb_ref_input;
+typedef struct snfb_ref_query {
+    uint32_t contig; uint32_t _pad;
+    uint64_t start, length;   /* 0 <= start, start + length <= the contig's length                                 */
+    uint64_t out_off;
+} snfb_ref_query;
+int         snfb_load_reference(snfb_ctx* ctx, const snfb_ref_input* in);
+int         snfb_reference_runs(snfb_ctx* ctx, const int32_t** runs, const uint64_t** contig_off, uint64_t* n_runs);
+int         snfb_fetch_reference(snfb_ctx* ctx, const snfb_ref_query* q, uint64_t n, uint8_t* out, uint64_t out_cap);
 /* BAM CIGAR words -> CIGAR16 (host code, OpenMP; no GPU needed).  rec_out receives copies of rec_in with cigar_off / n_cigar
  * rewritten for the 16-bit arena.  Call with out16 == NULL to get the number of 16-bit words the arena needs (a multiple
  * of 8); returns that number, or UINT64_MAX when a record holds an op the path does not know (B) or out_cap is too small.

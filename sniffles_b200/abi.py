@@ -170,6 +170,14 @@ class GtOut(C.Structure):                                       # snfb_gt_out
     _fields_ = [("match", C.c_void_p), ("cov_start", C.c_void_p), ("cov_center", C.c_void_p), ("cov_end", C.c_void_p), ("bnd_no_prev", C.c_void_p)]
 
 
+REF_CONTIG_DTYPE = np.dtype([("offset", "<u8"), ("length", "<u8"), ("linebases", "<u4"), ("linewidth", "<u4")])       # snfb_ref_contig
+REF_QUERY_DTYPE = np.dtype([("contig", "<u4"), ("_pad", "<u4"), ("start", "<u8"), ("length", "<u8"), ("out_off", "<u8")])  # snfb_ref_query
+
+
+class RefInput(C.Structure):                                    # snfb_ref_input
+    _fields_ = [("bytes", C.c_void_p), ("n_bytes", C.c_uint64), ("is_bgzf", C.c_uint32), ("n_contig", C.c_uint32), ("contig", C.c_void_p)]
+
+
 def view(ptr, dtype, n):
     """numpy array over library-owned memory (no copy); empty array for n == 0 / NULL."""
     dtype = np.dtype(dtype)

@@ -18,7 +18,7 @@ EXPORTS = ["snfb_version", "snfb_sizeof", "snfb_hash_name", "snfb_ctx_create", "
            "snfb_pin_host", "snfb_unpin_host", "snfb_pack_cigar16", "snfb_rerun_count", "snfb_coverage_bins",
            "snfb_nccl_unique_id", "snfb_comm_init", "snfb_allgather_candidates", "snfb_selftest_sqrt_frac", "snfb_poa", "snfb_combine_groups", "snfb_selftest_edit_distance",
            "snfb_load_bam", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf", "snfb_deflate_bgzf",
-           "snfb_genotype_targets"]
+           "snfb_genotype_targets", "snfb_load_reference", "snfb_reference_runs", "snfb_fetch_reference"]
 
 
 def lib():
@@ -63,6 +63,9 @@ def lib():
         L.snfb_allgather_candidates.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(abi.GatherView)]
         L.snfb_poa.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
         L.snfb_genotype_targets.argtypes = [C.c_void_p, C.POINTER(abi.GtIn), C.POINTER(abi.GtOut)]
+        L.snfb_load_reference.argtypes = [C.c_void_p, C.POINTER(abi.RefInput)]
+        L.snfb_reference_runs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
+        L.snfb_fetch_reference.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
         L.snfb_combine_groups.argtypes = [C.c_void_p, C.POINTER(abi.CombineIn), C.POINTER(abi.CombineOut)]
         L.snfb_selftest_edit_distance.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
         L.snfb_selftest_sqrt_frac.restype = C.c_double
@@ -307,6 +310,32 @@ class Context:
         O.match, O.cov_start, O.cov_center, O.cov_end, O.bnd_no_prev = (a.ctypes.data for a in out)
         self._check(self._lib.snfb_genotype_targets(self._h, C.byref(I), C.byref(O)), "snfb_genotype_targets")
         return out
+
+    def load_reference(self, data, contigs, is_bgzf=False):
+        """Reference FASTA -> the unwrapped genome resident on this context, and its 'N' runs (snfb_load_reference).  data: the file's bytes
+        (whole BGZF members when is_bgzf); contigs: abi.REF_CONTIG_DTYPE rows (raw offset rebased to `data`'s inflated stream, length,
+        linebases, linewidth).  Returns (runs int32 [n, 2], contig_off uint64 [n_contig + 1]) as snfb_reference_runs gives them."""
+        data = np.frombuffer(data, "u1") if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, dtype="u1")
+        contigs = np.ascontiguousarray(contigs, dtype=abi.REF_CONTIG_DTYPE)
+        I = abi.RefInput()
+        I.bytes, I.n_bytes, I.is_bgzf, I.n_contig, I.contig = data.ctypes.data, len(data), int(bool(is_bgzf)), len(contigs), contigs.ctypes.data
+        self._ref_n_contig = len(contigs)
+        self._check(self._lib.snfb_load_reference(self._h, C.byref(I)), "snfb_load_reference")
+        return self.reference_runs()
+
+    def reference_runs(self):
+        """(runs int32 [n, 2], contig_off uint64 [n_contig + 1]) of the loaded reference (snfb_reference_runs), copied"""
+        r, o, n = C.c_void_p(), C.c_void_p(), C.c_uint64()
+        self._check(self._lib.snfb_reference_runs(self._h, C.byref(r), C.byref(o), C.byref(n)), "snfb_reference_runs")
+        return abi.view(r.value, "<i4", 2 * n.value).reshape(-1, 2).copy(), abi.view(o.value, "<u8", 0 if not o.value else self._ref_n_contig + 1).copy()
+
+    def fetch_reference(self, queries) -> np.ndarray:
+        """resolved gathers from the loaded reference (snfb_fetch_reference): abi.REF_QUERY_DTYPE rows -> the output bytes (uint8)"""
+        queries = np.ascontiguousarray(queries, dtype=abi.REF_QUERY_DTYPE)
+        cap = int((queries["out_off"] + queries["length"]).max()) if len(queries) else 0
+        out = np.zeros(max(cap, 1), "u1")
+        self._check(self._lib.snfb_fetch_reference(self._h, queries.ctypes.data, len(queries), out.ctypes.data, cap), "snfb_fetch_reference")
+        return out[:cap]
 
     def comm_init(self, unique_id: bytes, rank: int, nranks: int):
         """Join the NCCL communicator of the per-GPU processes (the 128-byte id comes from `nccl_unique_id()` on one rank)."""

@@ -27,6 +27,7 @@
 #include "ingest.cuh"
 #include "bgzf_write.cuh"
 #include "genotype.cuh"
+#include "reference.cuh"
 
 // one owning allocation of device memory, or of pinned host memory when Pinned; freed by the destructor
 template <bool Pinned> struct Buf {
@@ -43,6 +44,7 @@ template <bool Pinned> struct Buf {
         cap = want; return 0;
     }
     template <class T> T* as() { return reinterpret_cast<T*>(p); }
+    void reset() { release(); }      // gives the memory back (a transient buffer)
 private:
     void release() { if (p) { if (Pinned) cudaFreeHost(p); else cudaFree(p); } p = nullptr; cap = 0; }
 };
@@ -102,6 +104,8 @@ struct snfb_ctx {
     DevBuf b_comp, b_raw, b_ing, b_ing_work; HostBuf h_ing; uint64_t ing_sizes[8] = {0, 0, 0, 0, 0, 0, 0, 0}; bool from_bam = false;      // device BAM ingest: BGZF bytes, inflated stream, block / span tables, per-raw-record work arrays
     DevBuf b_zin, b_zslot, b_zout, b_zwork;          // BGZF compression: input bytes, 64 KiB member slots, packed members, sizes / offsets / candidate scratch
     DevBuf b_gt;                                     // force calling: candidate bin keys, sort scratch, targets and their results
+    DevBuf b_ref, b_ref_work; std::vector<refseq::Contig> ref_ctg; bool have_ref = false;     // the unwrapped reference genome; tables / counters / N-run scratch
+    HostBuf h_ref_runs, h_ref_coff, h_ref_out; uint64_t ref_n_runs = 0;                       // N runs and per-contig offsets; gather staging
     std::vector<snfb_task> tasks;
     // capacities and the three arenas carved by them
     Caps cap; bool force_no_cuts = false;
@@ -236,7 +240,8 @@ int snfb_version(void) { return SNFB_ABI_VERSION; }
 size_t snfb_sizeof(int which) {
     switch (which) { case 0: return sizeof(snfb_rec); case 1: return sizeof(snfb_task); case 2: return sizeof(snfb_contig); case 3: return sizeof(snfb_records);
                      case 4: return sizeof(snfb_config); case 5: return sizeof(snfb_lead); case 6: return sizeof(snfb_cand); case 7: return sizeof(snfb_gather_view);
-                     case 8: return sizeof(snfb_gt_in); case 9: return sizeof(snfb_gt_out); default: return 0; }
+                     case 8: return sizeof(snfb_gt_in); case 9: return sizeof(snfb_gt_out);
+                     case 10: return sizeof(snfb_ref_contig); case 11: return sizeof(snfb_ref_input); case 12: return sizeof(snfb_ref_query); default: return 0; }
 }
 
 uint64_t snfb_hash_name(const char* s, size_t n) {
@@ -436,11 +441,11 @@ static int walk_bgzf(snfb_ctx* ctx, const uint8_t* z, uint64_t n, std::vector<in
     }
     *raw_len = uo; return 0;
 }
-static int inflate_to_device(snfb_ctx* ctx, const uint8_t* z, uint64_t n, std::vector<uint64_t>& cstart, std::vector<ingest::BgzfBlock>& blocks, uint64_t* raw_len) {
+static int inflate_to_device(snfb_ctx* ctx, const uint8_t* z, uint64_t n, std::vector<uint64_t>& cstart, std::vector<ingest::BgzfBlock>& blocks, uint64_t* raw_len, const char* h2d_mark = "h2d_bgzf") {
     if (walk_bgzf(ctx, z, n, blocks, cstart, raw_len)) return 1;
     if (*raw_len >= (1ull << 36)) return fail(ctx, "more than 64 GiB of inflated BAM in one ingest call: split the task list");
     if (ctx->b_comp.ensure(n + 64) || ctx->b_raw.ensure(*raw_len + 64)) return fail(ctx, "out of device memory for the BGZF bytes / the inflated stream");
-    mark(ctx, "h2d_bgzf", n);
+    mark(ctx, h2d_mark, n);
     CUDA_TRY(cudaMemcpyAsync(ctx->b_comp.p, z, n, cudaMemcpyHostToDevice, ctx->st));
     CUDA_TRY(cudaMemsetAsync(ctx->b_comp.as<uint8_t>() + n, 0, 64, ctx->st));
     CUDA_TRY(cudaMemsetAsync(ctx->b_raw.as<uint8_t>() + *raw_len, 0, 64, ctx->st));
@@ -1320,6 +1325,142 @@ int snfb_genotype_targets(snfb_ctx* ctx, const snfb_gt_in* in, snfb_gt_out* out)
     for (int k = 0; k < 4; ++k) CUDA_TRY(cudaMemcpyAsync(dst[k], G.cov_start + (size_t)k * n, 4 * n, cudaMemcpyDeviceToHost, st));
     const cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, std::string("snfb_genotype_targets: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+// ---- the reference FASTA (--reference): raw bytes -> unwrapped genome, its 'N' runs, REF / anchor gathers ----
+int snfb_load_reference(snfb_ctx* ctx, const snfb_ref_input* in) {
+    if (!ctx || !in) return ctx ? fail(ctx, "snfb_load_reference: null argument") : 1;
+    if ((in->n_bytes && !in->bytes) || (in->n_contig && !in->contig)) return fail(ctx, "snfb_load_reference: null table");
+    cudaSetDevice(ctx->device);
+    ctx->have_ref = false; ctx->ref_n_runs = 0; ctx->n_ev = 0;
+    cudaStream_t st = ctx->st;
+    uint64_t raw_len = 0;
+    if (in->is_bgzf) {      // the ingest's inflate, CRC-checked; the raw stream lives in b_raw until the genome is built
+        std::vector<ingest::BgzfBlock> blocks; std::vector<uint64_t> cstart;
+        if (inflate_to_device(ctx, in->bytes, in->n_bytes, cstart, blocks, &raw_len, "h2d_ref")) return 1;
+        const size_t nb = blocks.size();
+        ingest::IngestCounters* d_ctr = nullptr; ingest::BgzfBlock* d_blk = nullptr;
+        if (carve(ctx->b_ref_work, [&](Carver& c) { d_ctr = c.take<ingest::IngestCounters>(1); d_blk = c.take<ingest::BgzfBlock>(nb + 1); })) return fail(ctx, "out of device memory (reference inflate tables)");
+        CUDA_TRY(cudaMemsetAsync(d_ctr, 0, sizeof(ingest::IngestCounters), st));
+        CUDA_TRY(cudaMemcpyAsync(d_blk, blocks.data(), sizeof(ingest::BgzfBlock) * nb, cudaMemcpyHostToDevice, st));
+        mark(ctx, "inflate", in->n_bytes + raw_len);
+        if (nb) launch_inflate(ctx, d_blk, (unsigned)nb, d_ctr);
+        mark(ctx, nullptr);
+        ingest::IngestCounters hc;
+        CUDA_TRY(cudaMemcpyAsync(&hc, d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if (hc.bad_blocks) { ctx->b_raw.reset(); ctx->b_comp.reset(); inflate_failed(ctx, hc, cstart); ctx->err = "reference " + ctx->err; return 1; }
+        ctx->b_comp.reset();
+    } else {
+        raw_len = in->n_bytes;
+        if (ctx->b_raw.ensure(raw_len + 64)) return fail(ctx, "out of device memory for the reference FASTA bytes");
+        mark(ctx, "h2d_ref", raw_len);
+        CUDA_TRY(cudaMemcpyAsync(ctx->b_raw.p, in->bytes, raw_len, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemsetAsync(ctx->b_raw.as<uint8_t>() + raw_len, 0, 64, st));
+    }
+    // the .fai geometry: checked on the host, laid out as 16-byte aligned contigs of the genome and cut into tiles
+    const uint32_t nc = in->n_contig;
+    std::vector<refseq::Contig> ctg(nc); std::vector<refseq::Tile> ut, nt; std::vector<int64_t> first_nt(nc, -1);
+    uint64_t total = 0;
+    for (uint32_t c = 0; c < nc; ++c) {
+        const snfb_ref_contig& k = in->contig[c];
+        const std::string who = "snfb_load_reference: contig " + std::to_string(c);
+        if (k.length >= (1ull << 31)) { ctx->b_raw.reset(); return fail(ctx, who + " is 2^31 bases or longer"); }
+        if (k.length) {
+            if (k.linebases == 0) { ctx->b_raw.reset(); return fail(ctx, who + ": LINEBASES is 0"); }
+            const bool multi = k.length > k.linebases;
+            if (k.linewidth != k.linebases + 1 && k.linewidth != k.linebases + 2 && (multi || k.linewidth != k.linebases)) { ctx->b_raw.reset(); return fail(ctx, who + ": LINEWIDTH must be LINEBASES + 1 or + 2"); }
+            const uint64_t last = k.length - 1, end = k.offset + (last / k.linebases) * k.linewidth + last % k.linebases + 1;
+            if (end > raw_len || end < k.offset) { ctx->b_raw.reset(); return fail(ctx, who + ": the .fai geometry reaches byte " + std::to_string(end) + " of a " + std::to_string(raw_len) + "-byte file"); }
+        }
+        total = (total + 15) & ~15ull;
+        ctg[c] = refseq::Contig{ k.offset, k.length, total, k.linebases, k.linewidth };
+        for (uint64_t p = 0; p < k.length; p += refseq::UNW_TILE) ut.push_back(refseq::Tile{ c, 0, p });
+        if (k.length) first_nt[c] = (int64_t)nt.size();
+        for (uint64_t p = 0; p < k.length; p += refseq::NR_TILE) nt.push_back(refseq::Tile{ c, 0, p });
+        total += k.length;
+    }
+    if (nt.size() >= (1ull << 31)) { ctx->b_raw.reset(); return fail(ctx, "snfb_load_reference: genome too large"); }
+    if (ctx->b_ref.ensure(total + 256)) { ctx->b_raw.reset(); return fail(ctx, "out of device memory for the reference genome"); }
+    const size_t nu = ut.size(), nn = nt.size();
+    refseq::Contig* d_ctg = nullptr; refseq::Tile* d_ut = nullptr; refseq::Tile* d_nt = nullptr; refseq::Bad* d_bad = nullptr;
+    uint32_t *n_s = nullptr, *n_e = nullptr, *o_s = nullptr, *o_e = nullptr, *tmp = nullptr; unsigned long long* tot = nullptr;
+    if (carve(ctx->b_ref_work, [&](Carver& c) { d_ctg = c.take<refseq::Contig>(nc + 1); d_ut = c.take<refseq::Tile>(nu + 1); d_nt = c.take<refseq::Tile>(nn + 1); d_bad = c.take<refseq::Bad>(1);
+                                                n_s = c.take<uint32_t>(nn + 1); n_e = c.take<uint32_t>(nn + 1); o_s = c.take<uint32_t>(nn + 1); o_e = c.take<uint32_t>(nn + 1);
+                                                tmp = c.take<uint32_t>(prims::scan_tmp_elems(nn + 1) + 16); tot = c.take<unsigned long long>(2); }))
+        { ctx->b_raw.reset(); return fail(ctx, "out of device memory (reference tables)"); }
+    if (nc) CUDA_TRY(cudaMemcpyAsync(d_ctg, ctg.data(), sizeof(refseq::Contig) * nc, cudaMemcpyHostToDevice, st));
+    if (nu) CUDA_TRY(cudaMemcpyAsync(d_ut, ut.data(), sizeof(refseq::Tile) * nu, cudaMemcpyHostToDevice, st));
+    if (nn) CUDA_TRY(cudaMemcpyAsync(d_nt, nt.data(), sizeof(refseq::Tile) * nn, cudaMemcpyHostToDevice, st));
+    const refseq::Bad bad0{ 0ull, ~0ull };
+    CUDA_TRY(cudaMemcpyAsync(d_bad, &bad0, sizeof(bad0), cudaMemcpyHostToDevice, st));
+    mark(ctx, "ref_unwrap", raw_len + total);
+    if (nu) launch(ctx->launches, refseq::k_ref_unwrap, (unsigned)std::min<size_t>(nu, (size_t)NUM_SMS * 8), refseq::UNW_THREADS, 0, st, ctx->b_raw.as<const uint8_t>(), d_ctg, d_ut, (unsigned)nu, ctx->b_ref.as<uint8_t>(), d_bad);
+    mark(ctx, "ref_nruns", 2 * total);
+    if (nn) {
+        launch(ctx->launches, refseq::k_ref_nruns_count, (unsigned)nn, refseq::NR_THREADS, 0, st, ctx->b_ref.as<const uint8_t>(), d_ctg, d_nt, n_s, n_e);
+        prims::exclusive_scan(ctx->launches, n_s, o_s, tmp, nullptr, nn, tot, st);
+        prims::exclusive_scan(ctx->launches, n_e, o_e, tmp, nullptr, nn, tot + 1, st);
+    } else CUDA_TRY(cudaMemsetAsync(tot, 0, 16, st));
+    refseq::Bad hb; unsigned long long ht[2];
+    CUDA_TRY(cudaMemcpyAsync(&hb, d_bad, sizeof(hb), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(ht, tot, sizeof(ht), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    ctx->b_raw.reset();                                   // only the unwrapped genome stays resident
+    if (hb.n) return fail(ctx, "snfb_load_reference: " + std::to_string(hb.n) + " line(s) do not match the .fai geometry (first: contig " + std::to_string(hb.first >> 40)
+                               + ", line " + std::to_string(hb.first & ((1ull << 40) - 1)) + "): the index does not describe this file");
+    if (ht[0] != ht[1]) return fail(ctx, "snfb_load_reference: N-run starts and ends do not pair up");
+    const uint64_t nr = ht[0];
+    if (ctx->h_ref_runs.ensure(8 * (nr + 1)) || ctx->h_ref_coff.ensure(8 * ((size_t)nc + 1)) || ctx->h_ref_out.ensure(4 * (nn + 1))) return fail(ctx, "out of pinned memory (reference N runs)");
+    DevBuf d_runs;
+    if (d_runs.ensure(8 * (nr + 1))) return fail(ctx, "out of device memory (reference N runs)");
+    if (nn && nr) launch(ctx->launches, refseq::k_ref_nruns_write, (unsigned)nn, refseq::NR_THREADS, 0, st, ctx->b_ref.as<const uint8_t>(), d_ctg, d_nt, o_s, o_e, d_runs.as<int32_t>());
+    mark(ctx, nullptr);
+    if (nr) CUDA_TRY(cudaMemcpyAsync(ctx->h_ref_runs.p, d_runs.p, 8 * nr, cudaMemcpyDeviceToHost, st));
+    uint32_t* h_os = ctx->h_ref_out.as<uint32_t>();
+    if (nn) CUDA_TRY(cudaMemcpyAsync(h_os, o_s, 4 * nn, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    uint64_t* coff = ctx->h_ref_coff.as<uint64_t>();
+    coff[nc] = nr;
+    for (int64_t c = (int64_t)nc - 1; c >= 0; --c) coff[c] = first_nt[c] >= 0 ? h_os[first_nt[c]] : coff[c + 1];
+    ctx->ref_ctg = std::move(ctg); ctx->ref_n_runs = nr; ctx->have_ref = true;
+    return 0;
+}
+
+int snfb_reference_runs(snfb_ctx* ctx, const int32_t** runs, const uint64_t** contig_off, uint64_t* n_runs) {
+    if (!ctx || !runs || !contig_off || !n_runs) return ctx ? fail(ctx, "snfb_reference_runs: null argument") : 1;
+    if (!ctx->have_ref) return fail(ctx, "snfb_reference_runs: no reference is loaded (snfb_load_reference)");
+    *runs = ctx->h_ref_runs.as<int32_t>(); *contig_off = ctx->h_ref_coff.as<uint64_t>(); *n_runs = ctx->ref_n_runs;
+    return 0;
+}
+
+int snfb_fetch_reference(snfb_ctx* ctx, const snfb_ref_query* q, uint64_t n, uint8_t* out, uint64_t out_cap) {
+    if (!ctx || (n && (!q || !out))) return ctx ? fail(ctx, "snfb_fetch_reference: null argument") : 1;
+    if (!ctx->have_ref) return fail(ctx, "snfb_fetch_reference: no reference is loaded (snfb_load_reference)");
+    std::vector<refseq::Query> hq(n); uint64_t span = 0;
+    for (uint64_t i = 0; i < n; ++i) {
+        const snfb_ref_query& x = q[i];
+        if (x.contig >= ctx->ref_ctg.size()) return fail(ctx, "snfb_fetch_reference: query " + std::to_string(i) + ": contig index out of range");
+        const refseq::Contig& c = ctx->ref_ctg[x.contig];
+        if (x.start > c.len || x.length > c.len - x.start) return fail(ctx, "snfb_fetch_reference: query " + std::to_string(i) + " reaches past the end of contig " + std::to_string(x.contig));
+        if (x.out_off > out_cap || x.length > out_cap - x.out_off) return fail(ctx, "snfb_fetch_reference: query " + std::to_string(i) + " does not fit out_cap");
+        hq[i] = refseq::Query{ c.out_off + x.start, x.length, x.out_off };
+        span = std::max<uint64_t>(span, x.out_off + x.length);
+    }
+    ctx->n_ev = 0;
+    if (n == 0) return 0;
+    cudaSetDevice(ctx->device);
+    refseq::Query* d_q = nullptr; uint8_t* d_out = nullptr;
+    if (carve(ctx->b_ref_work, [&](Carver& c) { d_q = c.take<refseq::Query>(n); d_out = c.take<uint8_t>(span + 16); })) return fail(ctx, "snfb_fetch_reference: out of device memory");
+    cudaStream_t st = ctx->st;
+    CUDA_TRY(cudaMemcpyAsync(d_q, hq.data(), sizeof(refseq::Query) * n, cudaMemcpyHostToDevice, st));
+    mark(ctx, "ref_gather", 2 * span);
+    launch(ctx->launches, refseq::k_ref_gather, grid_for(n * 32, 256), 256, 0, st, ctx->b_ref.as<const uint8_t>(), d_q, (unsigned long long)n, d_out);
+    mark(ctx, nullptr);
+    CUDA_TRY(cudaMemcpyAsync(out, d_out, span, cudaMemcpyDeviceToHost, st));
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, std::string("snfb_fetch_reference: ") + cudaGetErrorString(e));
     return 0;
 }
 

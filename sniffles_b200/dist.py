@@ -29,6 +29,14 @@ def subset_block(block, task_ids):
     return sub
 
 
+def rank_reference(path, ctx, block, task_ids):
+    """the reference FASTA of --reference loaded on a rank's device with only the contigs of its tasks (fasta.Reference); the N mask
+    built from it travels with the block (subset_block)"""
+    from . import fasta
+    names = sorted({block.contig_names[int(block.task[t]["contig"])] for t in task_ids})
+    return fasta.Reference(path, ctx, contigs=names)
+
+
 def allgather_bytes(local, group=None):
     """All-gather of variable-length uint8 tensors: sizes first, then max-padded payloads.  Returns the list of
     per-rank tensors (trimmed).  `local` lives on the device of the backend (cuda for nccl, cpu for gloo)."""

@@ -252,6 +252,7 @@ def genotype_vcf(config, device=0):
             return 0
         tr = {k: [(int(a), int(b)) for a, b in tr_all[name]] for k, (_, name, _, _, _) in enumerate(planned) if name in tr_all}
         block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[name], s, e, tid) for tid, name, s, e, _ in planned], tandem_repeats=tr or None)
+        tasks.mask_block(block, config, ctx)            # target coverage is N-masked as in GenotypeTask's LeadProvider
         ctx.set_config(abi.Config.from_sniffles(config))
         bgzf, spans = bam.device_input([(name, s, e) for _, name, s, e, _ in planned])
         n_rec = ctx.load_bam(bgzf, spans, block)["n_rec"]

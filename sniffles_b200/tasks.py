@@ -4,6 +4,7 @@ execute — with the three hot calls forwarded to libsnfb200 through ctypes.
 
 A `Task` works on one contig (one snfb_task); several tasks can share one record block and one
 device run (`run_block`), which is how the contigs of a genome are processed per GPU."""
+import logging
 from dataclasses import dataclass, field
 from typing import Optional
 
@@ -18,6 +19,34 @@ def device_context(device: int = 0) -> binding.Context:
     if device not in _CTX:
         _CTX[device] = binding.Context(device)
     return _CTX[device]
+
+
+_REF = {}      # per (device context, FASTA path): the fasta.Reference loaded on it, or None when it could not be loaded
+
+
+def reference_for(ctx, path):
+    """the reference FASTA resident on `ctx`, loaded on first use.  A FASTA that cannot be opened or read (a missing or stale index, a
+    damaged BGZF block) is logged once as the reference logs it (vcf.py:116-119) and the run goes on without it."""
+    key = (ctx, str(path))
+    if key not in _REF:
+        from . import fasta
+        try:
+            _REF[key] = fasta.Reference(path, ctx)
+        except (OSError, ValueError, RuntimeError) as e:
+            logging.error(f"Unable to open reference file {path}: {e}")
+            _REF[key] = None
+    return _REF[key]
+
+
+def mask_block(block, config, ctx):
+    """with config.reference: the block's N-mask tables from the reference loaded on `ctx` (LeadProvider._mask_N_coverage,
+    leadprov.py:420-443), before the block is loaded; without it the block is left as it is"""
+    if getattr(config, "reference", None):
+        ref = reference_for(ctx, config.reference)
+        if ref is not None:
+            from . import fasta
+            fasta.mask_block(block, ref)
+    return block
 
 
 @dataclass
@@ -152,11 +181,11 @@ class Task:
                 # the reference's `bam.fetch(contig, start, end)` (parallel.py:95-98, leadprov.py:488) with htslib's work on the GPU: the host
                 # only resolves the BAI index; BGZF inflate, record decode, region filter and CIGAR16 packing are snfb_load_bam
                 bam = self._open()
-                block = self._tables(bam)
+                block = mask_block(self._tables(bam), self.config, ctx)
                 bgzf, spans = bam.device_input([(self.contig, int(self.start), int(self.end))])
                 n_rec = ctx.load_bam(bgzf, spans, block)["n_rec"]
             else:
-                block = self._own_block()
+                block = mask_block(self._own_block(), self.config, ctx)
                 ctx.load(block, cigar16=False)                   # BAM words: the library converts them (snfb_load_records)
                 n_rec = len(block.rec)
             res = ctx.extract_leads()                            # snfb_extract_leads

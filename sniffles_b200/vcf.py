@@ -219,6 +219,19 @@ class VCFWriter:
         return 1
 
 
+def reference_intervals(calls, config):
+    """every (contig, start, end) `VCFWriter.write_call` can fetch from the reference for these calls (vcf.py:304-338): the DEL's anchor
+    base plus deleted bases (pos - 1, pos - svlen), and the anchor base (max(0, pos - 1), + 1) of any call.  A superset: what the writer
+    skips (symbolic output, long DELs, single breaks) is listed anyway, so one Reference.prefetch serves a whole call set."""
+    out = []
+    for call in calls:
+        if call.svtype == "DEL":
+            out.append((call.contig, call.pos - 1, call.pos - call.svlen))
+        a = max(0, call.pos - 1)
+        out.append((call.contig, a, a + 1))
+    return out
+
+
 class BgzfIndexedOutput:
     """Text handle for a `--vcf out.vcf.gz` (sniffles:229-244, :573-584): VCFWriter writes into it unchanged; `close()` compresses the
     text into BGZF members with `compress(bytes) -> (members, coffsets)` (binding.Context.deflate_bgzf on the product path), then writes
