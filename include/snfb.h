@@ -153,7 +153,8 @@ typedef struct snfb_records {
     const snfb_contig* contig;
     const int32_t*     tr;    /* n_tr pairs (start,end), per task sorted (util.py:121-147) */
     /* optional: reference 'N' runs per task for LeadProvider._mask_N_coverage (leadprov.py:420-443, only with --reference):
-     * n_mask half-open pairs (start,end), sorted and disjoint inside a task; task t owns mask[mask_task_off[t] .. mask_task_off[t+1]) */
+     * n_mask half-open pairs (start,end), sorted and disjoint inside a task; task t owns mask[mask_task_off[t] .. mask_task_off[t+1]).
+     * snfb_load_records / snfb_load_bam refuse a task whose runs have start > end or overlap / precede the run before them. */
     uint32_t n_mask;
     uint32_t cigar_fmt;   /* SNFB_CIGAR_*; BAM32 host arenas are converted on the host inside snfb_load_records (device arenas must be CIGAR16) */
     const int32_t*  mask;
@@ -376,7 +377,8 @@ uint64_t    snfb_launch_count(snfb_ctx* ctx);
 /* number of times a run was repeated because a buffer capacity was too small or a chain cut had to be undone */
 uint64_t    snfb_rerun_count(snfb_ctx* ctx);
 /* mean coverage of consecutive `binsize`-base bins over the whole contig of one task, as the SNF writer stores it
- * (snf.py:248-267: the coverage vector zero-padded to a multiple of binsize, row means; the writer rounds them).
+ * (snf.py:248-267: the coverage vector zero-padded to a multiple of binsize, row means; the writer rounds them).  With an N mask
+ * loaded, positions inside the task's runs (clipped to the task region) count 0, as in the masked vector (leadprov.py:470).
  * *out is a library-owned buffer of *n_bins doubles, valid until the next call on the ctx.  Needs snfb_extract_leads
  * (or snfb_run) first. */
 int         snfb_coverage_bins(snfb_ctx* ctx, uint32_t task, int binsize, const double** out, uint64_t* n_bins);

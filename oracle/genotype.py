@@ -75,11 +75,15 @@ def record_spans(blk):
     """reference span of every record of a packed block (BAM CIGAR words: M, D, N, =, X advance the reference)"""
     import numpy as np
     adv = np.isin(blk.cigar & 15, [0, 2, 3, 7, 8])
-    return np.add.reduceat(np.where(adv, blk.cigar >> 4, 0), blk.rec["cigar_off"].astype(np.int64), dtype=np.int64)
+    cs = np.concatenate(([0], np.cumsum(np.where(adv, blk.cigar >> 4, 0), dtype=np.int64)))     # records may share or reorder CIGARs
+    off = blk.rec["cigar_off"].astype(np.int64)
+    return cs[off + blk.rec["n_cigar"].astype(np.int64)] - cs[off]
 
 
-def coverage_vector(blk, ok, span, t):
-    """LeadProvider.coverage of task t as a per-base uint16 vector: reads passing the filters (`ok`) over [pos, pos + span)"""
+def coverage_vector(blk, ok, span, t, runs=None):
+    """LeadProvider.coverage of task t as a per-base uint16 vector: reads passing the filters (`ok`) over [pos, pos + span).  `runs`:
+    reference 'N' runs [(a, b)] of the task; _mask_N_coverage zeroes them inside the task region only (the mask is fetched per region,
+    leadprov.py:436-439), and the slice clips to the vector"""
     import numpy as np
     L = int(blk.task[t]["contig_len"])
     sel = ok & (blk.rec["task"] == t)
@@ -87,7 +91,13 @@ def coverage_vector(blk, ok, span, t):
     cov = np.zeros(L + 1, np.int64)
     np.add.at(cov, s, 1)
     np.add.at(cov, np.minimum(s + span[sel], L), -1)
-    return np.cumsum(cov)[:L].astype(np.uint16)
+    cov = np.cumsum(cov)[:L].astype(np.uint16)
+    start, end = int(blk.task[t]["start"]), int(blk.task[t]["end"])
+    for a, b in runs or ():
+        a, b = max(int(a), start, 0), min(int(b), end, L)
+        if a < b:
+            cov[a:b] = 0
+    return cov
 
 
 class Sv:

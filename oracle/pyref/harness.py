@@ -183,9 +183,10 @@ def run_task(block, t, config, finalize=True):
     return out
 
 
-def write_reference_snf(block, config_args, path):
+def write_reference_snf(block, config_args, path, reference=None):
     """The reference's own --snf output for a block: every task runs CallTask's SNF branch (parallel.py:279-292: store the candidates,
-    annotate_block_coverages, write_and_index) and SNFile.write_results joins the parts (snf.py:193-224)."""
+    annotate_block_coverages, write_and_index) and SNFile.write_results joins the parts (snf.py:193-224).  `reference`: a FASTA path
+    for --reference, read through whatever pysam.FastaFile the caller installed (LeadProvider._mask_N_coverage, leadprov.py:420-443)."""
     import io
     import os
     import types
@@ -193,6 +194,7 @@ def write_reference_snf(block, config_args, path):
     from sniffles import leadprov, parallel, snf as refsnf
     from sniffles.region import Region
     config = make_config("--snf", path, *config_args)
+    config.reference = reference
     if not hasattr(config, "mode"):
         config.mode = "call_sample"
     config.task_read_id_offset_mult = 10 ** 9

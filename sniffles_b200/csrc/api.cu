@@ -345,6 +345,13 @@ static int check_tables(snfb_ctx* ctx, const snfb_records* R) {
     }
     if (R->n_mask && R->mask && R->mask_task_off) {
         for (uint32_t t = 0; t < R->n_task; ++t) if (R->mask_task_off[t] > R->mask_task_off[t + 1] || R->mask_task_off[t + 1] > R->n_mask) return fail(ctx, "mask_task_off must be non-decreasing and end at n_mask");
+        // the probes binary-search a task's runs and the contig mean subtracts each run once: they must be sorted and disjoint
+        for (uint32_t t = 0; t < R->n_task; ++t)
+            for (uint32_t m = R->mask_task_off[t]; m < R->mask_task_off[t + 1]; ++m) {
+                const uint32_t k = m - R->mask_task_off[t];
+                if (R->mask[2 * m] > R->mask[2 * m + 1]) return fail(ctx, "N mask of task " + std::to_string(t) + ": run " + std::to_string(k) + " has start > end");
+                if (k && R->mask[2 * m] < R->mask[2 * m - 1]) return fail(ctx, "N mask of task " + std::to_string(t) + ": run " + std::to_string(k) + " starts before run " + std::to_string(k - 1) + " ends (runs must be sorted and disjoint)");
+            }
     }
     return 0;
 }
@@ -1250,7 +1257,8 @@ int snfb_selftest_edit_distance(snfb_ctx* ctx, const uint8_t* bytes, uint64_t n_
     return 0;
 }
 
-// mean coverage of `binsize`-base bins over one task's region (snf.py:248-267: the 500-bp means the SNF writer stores)
+// mean coverage of `binsize`-base bins over one task's region (snf.py:248-267: the 500-bp means the SNF writer stores), N-masked as the
+// contig mean is
 int snfb_coverage_bins(snfb_ctx* ctx, uint32_t task, int binsize, const double** out, uint64_t* n_bins) {
     if (!ctx || !ctx->stage_a_done) return ctx ? fail(ctx, "snfb_extract_leads must run first") : 1;
     if (task >= ctx->n_task || binsize <= 0 || !out || !n_bins) return fail(ctx, "bad arguments");
@@ -1261,10 +1269,15 @@ int snfb_coverage_bins(snfb_ctx* ctx, uint32_t task, int binsize, const double**
     if (ctx->h_cov_bins.ensure(16 * (size_t)(nb + 1))) return fail(ctx, "out of pinned memory (coverage bins)");
     DevBuf acc; if (acc.ensure(8 * (size_t)(nb + 1))) return fail(ctx, "out of device memory (coverage bins)");
     CUDA_TRY(cudaMemsetAsync(acc.p, 0, 8 * (size_t)(nb + 1), ctx->st));
-    uint32_t lohi[2];
+    uint32_t lohi[2], runs[2] = { 0, 0 };
     CUDA_TRY(cudaMemcpyAsync(&lohi[0], ctx->task_first + task, 4, cudaMemcpyDeviceToHost, ctx->st)); CUDA_TRY(cudaMemcpyAsync(&lohi[1], ctx->task_last + task, 4, cudaMemcpyDeviceToHost, ctx->st));
+    if (ctx->n_mask) CUDA_TRY(cudaMemcpyAsync(runs, ctx->b_mask_off.as<uint32_t>() + task, 8, cudaMemcpyDeviceToHost, ctx->st));
     CUDA_TRY(cudaStreamSynchronize(ctx->st));
-    if (nb && lohi[1] > lohi[0]) launch(ctx->launches, k_cov_bins, grid_for(lohi[1] - lohi[0], 256), 256, 0, ctx->st, ctx->rec_pos, ctx->rec_end, ctx->rec_flags, lohi[0], lohi[1], binsize, L, nb, acc.as<unsigned long long>());
+    if (nb && lohi[1] > lohi[0]) {
+        launch(ctx->launches, k_cov_bins, grid_for(lohi[1] - lohi[0], 256), 256, 0, ctx->st, ctx->rec_pos, ctx->rec_end, ctx->rec_flags, lohi[0], lohi[1], binsize, L, nb, acc.as<unsigned long long>());
+        // the writer averages the N-masked vector (leadprov.py:470, snf.py:258): take the read bases inside the task's runs back out
+        if (runs[1] > runs[0]) launch(ctx->launches, cluster::k_mask_bins, grid_for((unsigned long long)(runs[1] - runs[0]) * 32, 128), 128, 0, ctx->st, ctx->B, (int)task, binsize, acc.as<unsigned long long>());
+    }
     unsigned long long* raw = reinterpret_cast<unsigned long long*>(ctx->h_cov_bins.as<uint8_t>() + 8 * (size_t)(nb + 1));
     CUDA_TRY(cudaMemcpyAsync(raw, acc.p, 8 * (size_t)nb, cudaMemcpyDeviceToHost, ctx->st));
     CUDA_TRY(cudaStreamSynchronize(ctx->st));

@@ -933,29 +933,57 @@ __global__ void k_coverage(B b) {
     }
 }
 
+// run m of task t as the coverage vector sees it: the mask is fetched per region (leadprov.py:436-438) and slices clip to [0, L)
+__device__ inline void mask_run(const B& b, int t, unsigned long long m, long long* a, long long* e) {
+    const long long L = b.task[t].contig_len;
+    *a = b.mask[2 * m]; *e = b.mask[2 * m + 1];
+    if (*a < b.task[t].start) *a = b.task[t].start; if (*e > b.task[t].end) *e = b.task[t].end; if (*a < 0) *a = 0; if (*e > L) *e = L;
+}
+// the passing reads of task t that overlap [a, e): each lane visits its share and calls f(o0, o1) with the overlap, the read's end
+// clipped to the contig as the coverage slice is (leadprov.py:510).  Records are coordinate sorted, so they start in (a - longest span, e).
+template <class F> __device__ inline void pass_overlaps_warp(const B& b, int t, long long a, long long e, F f) {
+    const uint32_t lo = b.task_first[t], hi = b.task_last[t];
+    if (a >= e || lo >= hi) return;
+    const long long L = b.task[t].contig_len;
+    uint32_t x = lo, z = hi;                     // first record with pos >= e
+    while (x < z) { const uint32_t mid = x + ((z - x) >> 1); if ((long long)b.rec_pos[mid] < e) x = mid + 1; else z = mid; }
+    const long long span = b.task_maxspan[t];
+    for (long long i = (long long)x - 1 - lane_id(); i >= (long long)lo; i -= 32) {
+        const long long ps = b.rec_pos[i]; if (ps + span <= a) break;
+        if (!(b.rec_flags[i] & extract::RF_PASS)) continue;
+        long long re = b.rec_end[i]; if (re > L) re = L;
+        const long long o0 = ps > a ? ps : a, o1 = re < e ? re : e;
+        if (o1 > o0) f(o0, o1);
+    }
+}
+
 // _mask_N_coverage for the contig mean: subtract the read bases that fall inside reference 'N' runs.  One warp per run.
 __global__ void k_mask_bp(B b, const uint32_t* __restrict__ mask_task, uint32_t n_mask, unsigned long long* task_cov_bp) {
     const unsigned long long nw = ((unsigned long long)gridDim.x * blockDim.x) >> 5;
     for (unsigned long long m = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; m < n_mask; m += nw) {
-        const int t = (int)mask_task[m]; const long long L = b.task[t].contig_len;
-        long long a = b.mask[2 * m], e = b.mask[2 * m + 1]; if (a < b.task[t].start) a = b.task[t].start; if (e > b.task[t].end) e = b.task[t].end; if (a < 0) a = 0; if (e > L) e = L;
-        const uint32_t lo = b.task_first[t], hi = b.task_last[t];
+        const int t = (int)mask_task[m]; long long a, e; mask_run(b, t, m, &a, &e);
         unsigned long long sum = 0;
-        if (a < e && lo < hi) {
-            uint32_t x = lo, z = hi;                 // first record with pos >= e
-            while (x < z) { const uint32_t mid = x + ((z - x) >> 1); if ((long long)b.rec_pos[mid] < e) x = mid + 1; else z = mid; }
-            const long long span = b.task_maxspan[t];
-            for (long long i = (long long)x - 1 - lane_id(); i >= (long long)lo; i -= 32) {
-                const long long ps = b.rec_pos[i]; if (ps + span <= a) break;
-                if (!(b.rec_flags[i] & extract::RF_PASS)) continue;
-                long long re = b.rec_end[i]; if (re > L) re = L;
-                const long long o0 = ps > a ? ps : a, o1 = re < e ? re : e;
-                if (o1 > o0) sum += (unsigned long long)(o1 - o0);
-            }
-        }
+        pass_overlaps_warp(b, t, a, e, [&](long long o0, long long o1) { sum += (unsigned long long)(o1 - o0); });
         #pragma unroll
         for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(FULL, sum, o);
         if (lane_id() == 0 && sum) atomicAdd(&task_cov_bp[t], 0ull - sum);
+    }
+}
+
+// _mask_N_coverage for the SNF coverage means (snfb_coverage_bins): the same read bases subtracted from the `binsize`-base bin sums of
+// task t that they fall in.  One warp per run.
+__global__ void k_mask_bins(B b, int t, int binsize, unsigned long long* acc) {
+    const unsigned long long nw = ((unsigned long long)gridDim.x * blockDim.x) >> 5;
+    const uint32_t m0 = b.mask_task_off[t], m1 = b.mask_task_off[t + 1];
+    for (unsigned long long m = m0 + (((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5); m < m1; m += nw) {
+        long long a, e; mask_run(b, t, m, &a, &e);
+        pass_overlaps_warp(b, t, a, e, [&](long long o0, long long o1) {
+            for (long long bb = o0 / binsize; bb <= (o1 - 1) / binsize; ++bb) {
+                const long long s0 = bb * binsize, s1 = s0 + binsize;
+                const long long x0 = o0 > s0 ? o0 : s0, x1 = o1 < s1 ? o1 : s1;
+                atomicAdd(&acc[bb], 0ull - (unsigned long long)(x1 - x0));
+            }
+        });
     }
 }
 

@@ -77,6 +77,23 @@ def n_runs(bases):
     return np.stack([np.flatnonzero(d == 1), np.flatnonzero(d == -1)], axis=1).astype("<i4")
 
 
+def task_runs(blk, seqs):
+    """{task: [(a, b)]} N runs a --reference run loads for a block: a task's contig must be in the FASTA and reach the task's end,
+    or the reference's _mask_N_coverage fails its fetch and leaves the task unmasked (leadprov.py:431-441)"""
+    by_name = dict(seqs)
+    out = {}
+    for t, k in enumerate(blk.task):
+        s = by_name.get(blk.contig_names[int(k["contig"])])
+        if s is not None and len(s) >= int(k["end"]):
+            out[t] = [tuple(map(int, r)) for r in n_runs(s)]
+    return out
+
+
+def coverage_bins(cv, binsize):
+    """SNFile.annotate_block_coverages' means (snf.py:257-258): the vector zero-padded to a multiple of binsize, row means"""
+    return np.pad(np.asarray(cv, np.int64), (0, -len(cv) % binsize)).reshape(-1, binsize).mean(axis=1)
+
+
 def golden_fasta(name):
     """(FASTA bytes, [(contig, bases)]) of a golden block"""
     seed, contigs = GOLDEN_FASTA[name]

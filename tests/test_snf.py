@@ -2,22 +2,27 @@
 tests/golden/make_golden.py snf): the reader parses it, the candidates in it equal this package's candidates for the same block,
 the 500-bp coverage entries equal the reshape-mean of the coverage, and the writer produces blocks that unpickle to the same content."""
 import io
+import json
 import os
 
 import numpy as np
 import pytest
 
+from oracle import genotype as ogt
 from sniffles_b200 import abi, postprocess, snf, tasks
 from sniffles_b200 import config as sconfig
 import oracle.oracle as orc
+import ref_fasta
 from test_oracle_golden import GOLDEN, load_fixture
 
 PATH = os.path.join(GOLDEN, "c2_ont_wgs_small.snf")
+REF_SNF_COVERAGE = os.path.join(GOLDEN, "reference", "snf_coverage.json")
 FIELDS = ["svtype", "pos", "end", "svlen", "support", "qual", "filter", "qc", "precise", "alt", "ref", "id", "fwd", "rev", "coverage_upstream", "coverage_start", "coverage_center",
           "coverage_end", "coverage_downstream", "genotypes", "rnames", "nm"]
 
 
-def _numpy_cov_bins(blk, cfg, t, step):
+def _numpy_cov_bins(blk, cfg, t, step, runs=None):
+    """the SNF writer's bin means of task t's coverage vector, N runs `runs` zeroed (leadprov.py:470, snf.py:257-258)"""
     rec = blk.rec
     first = blk.cigar[rec["cigar_off"]]
     last = blk.cigar[rec["cigar_off"] + rec["n_cigar"] - 1]
@@ -25,16 +30,37 @@ def _numpy_cov_bins(blk, cfg, t, step):
     trail = np.where(((last & 15) == 4) & (rec["n_cigar"] > 1), last >> 4, 0).astype(np.int64)
     alen = rec["l_seq"].astype(np.int64) - lead - trail
     tk = blk.task[rec["task"]]
-    ok = (rec["mapq"] >= cfg.mapq) & ((rec["flag"] & 256) == 0) & (alen >= cfg.min_alignment_length) & (rec["pos"] >= tk["start"]) & (rec["pos"] < tk["end"]) & (rec["task"] == t)
-    adv = np.isin(blk.cigar & 15, [0, 2, 3, 7, 8])
-    span = np.add.reduceat(np.where(adv, blk.cigar >> 4, 0).astype(np.int64), rec["cigar_off"].astype(np.int64))
-    L = int(blk.task[t]["contig_len"])
-    cov = np.zeros(L + 1, np.int64)
-    s = rec["pos"][ok].astype(np.int64)
-    np.add.at(cov, s, 1)
-    np.add.at(cov, np.minimum(s + span[ok], L), -1)
-    cov = np.cumsum(cov)[:L]
-    return np.pad(cov, (0, -L % step)).reshape(-1, step).mean(axis=1)
+    ok = (rec["mapq"] >= cfg.mapq) & ((rec["flag"] & 256) == 0) & (alen >= cfg.min_alignment_length) & (rec["pos"] >= tk["start"]) & (rec["pos"] < tk["end"])
+    return ref_fasta.coverage_bins(ogt.coverage_vector(blk, ok, ogt.record_spans(blk), t, runs), step)
+
+
+def snf_coverage_entries(bins, cfg, blocks):
+    """the `_COVERAGE` dict SNFile.annotate_block_coverages stores in each SNF block at `blocks` (snf.py:260-264)"""
+    step, bs = cfg.coverage_binsize_combine, cfg.snf_block_size
+    per = bs // step
+    return {b: {b + i * step: round(float(bins[b // bs * per + i])) for i in range(per) if b // bs * per + i < len(bins)} for b in blocks}
+
+
+@pytest.mark.parametrize("name", sorted(ref_fasta.GOLDEN_FASTA))
+def test_masked_bins_match_the_reference_snf_coverage(name):
+    """The N-masked restatement of the writer's bin means equals the `_COVERAGE` the reference itself stored with --snf --reference
+    (tests/golden/reference/snf_coverage.json, made by tests/golden/make_snf_coverage_golden.py), and the mask moves some of them."""
+    with open(REF_SNF_COVERAGE) as f:
+        gold = json.load(f)["blocks"][name]
+    _, blk = load_fixture(name)
+    text, seqs = ref_fasta.golden_fasta(name)
+    assert ref_fasta.sha256(text) == gold["fasta_sha256"]
+    cfg = sconfig.default_config("--snf", "x.snf", *gold["args"])
+    runs = ref_fasta.task_runs(blk, seqs)
+    moved = 0
+    for t in range(len(blk.task)):
+        contig = blk.contig_names[int(blk.task[t]["contig"])]
+        want = {int(b): {int(p): v for p, v in e.items()} for b, e in gold["coverage"].get(contig, {}).items()}
+        got = snf_coverage_entries(_numpy_cov_bins(blk, cfg, t, cfg.coverage_binsize_combine, runs.get(t)), cfg, want)
+        assert got == want, (name, contig)
+        plain = snf_coverage_entries(_numpy_cov_bins(blk, cfg, t, cfg.coverage_binsize_combine), cfg, want)
+        moved += sum(got[b][p] != plain[b][p] for b in got for p in got[b])
+    assert moved > 0 and sum(len(v) for v in gold["coverage"].values()) >= 5
 
 
 def _our_candidates(fx, blk, cfg, res):
