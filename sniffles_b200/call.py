@@ -1,0 +1,221 @@
+"""Calling a whole sample from its BAM (`sniffles -i sample.bam -v out.vcf [--snf out.snf]`, the call_sample mode of sniffles:131-590).
+
+  * planning is tasks.plan, shared with --genotype-vcf: one task per processed contig, [0, length - 1], task ids counted as the
+    reference counts them; config.task_read_id_offset_mult follows sniffles:304-309 from the index's mapped-read counts;
+  * the genome streams through the device in passes: consecutive tasks, in task-id order, whose inflated BAM bytes (the ISIZE of every
+    BGZF block bamio.BamFile.device_input selects for them) fit a budget.  A pass is one mask_block, one snfb_load_bam and one snfb_run;
+    its tasks then run as tasks.CallTask on the pass's BlockRun, and their VCF records and SNF parts are written before the next pass
+    loads (host memory stays bounded, and snfb_coverage_bins reads the block loaded on the context);
+  * the VCF goes through vcf.open_output (a .vcf.gz gets BGZF compressed on the GPU and a .tbi), the SNF through snf.write_results."""
+import contextlib
+import logging
+import math
+import os
+import time
+
+import numpy as np
+
+from . import abi, bamio, binding, snf, tasks, vcf
+
+log = logging.getLogger("sniffles_b200.call")
+
+# Peak device memory of one snfb_load_bam + snfb_run, as measured with scripts/call_sample_bench.py on an H100 80GB HBM3 (700 W; DESIGN §8):
+# 2.02 GB for 0.396 GB of inflated BAM (config 6) and 4.67 GB for 1.55 GB (config 2 at 1/100), i.e. about 1.1 GB fixed + 2.3 bytes per
+# inflated byte.  The budget of a pass is the free device memory, less the fixed part, over the per-byte factor; both carry a margin.
+DEVICE_BYTES_PER_INFLATED_BYTE = 2.6
+DEVICE_BYTES_FIXED = 1_500_000_000
+# the share of the free device memory a pass may plan on: the rest is left for the coverage bins, the REF gathers and the VCF compression
+FREE_MEMORY_SHARE = 0.9
+
+
+class CallSampleError(RuntimeError):
+    """the run stops as the reference's util.fatal_error_main stops it; the message is the reference's where it has one"""
+
+
+def read_id_offset_mult(total_mapped):
+    """config.task_read_id_offset_mult (sniffles:304-309): 10 ** ceil(ln(total_mapped) + 1), 10 ** 9 when the index counts no mapped
+    reads (the reference's CRAM case)"""
+    if total_mapped == 0:
+        return 10 ** 9
+    return 10 ** math.ceil(math.log(total_mapped) + 1)
+
+
+def total_mapped(bam):
+    """pysam's AlignmentFile.mapped: the mapped-read counts of the index's pseudo-bins, summed over the contigs"""
+    return sum(bam.count_mapped(name) or 0 for name, _ in bam.contigs)
+
+
+def check_outputs(config):
+    """the reference's checks before it opens any output (sniffles:122-127, 238-248, 265-267)"""
+    if config.vcf is None and config.snf is None:
+        raise CallSampleError("Please specify at least one of: --vcf or --snf for output (both may be used at the same time)")
+    for path in (config.vcf, config.snf):
+        if path is not None and os.path.exists(path) and not config.allow_overwrite:
+            raise CallSampleError(f"Output file '{path}' already exists! Use --allow-overwrite to ignore this check and overwrite.")
+    if config.vcf is not None:
+        parent = os.path.dirname(os.path.abspath(config.vcf))
+        if not os.path.exists(parent):
+            raise CallSampleError(f"Directory {parent} does not exists.")
+
+
+def inflated_bytes(bgzf):
+    """the sum of ISIZE over whole BGZF members: what snfb_load_bam inflates them to"""
+    return sum(isize for _, _, _, isize in bamio.bgzf_members(np.ascontiguousarray(bgzf, dtype="u1").tobytes()))
+
+
+def device_budget(device=0):
+    """the inflated BAM bytes one pass may load: the device's free memory, less DEVICE_BYTES_FIXED, over DEVICE_BYTES_PER_INFLATED_BYTE
+    (at least one byte: a task larger than the budget still runs, alone in its pass)"""
+    import torch
+    free, _ = torch.cuda.mem_get_info(device)
+    return max(1, int((free * FREE_MEMORY_SHARE - DEVICE_BYTES_FIXED) / DEVICE_BYTES_PER_INFLATED_BYTE))
+
+
+def group_passes(items, budget, size=lambda item: item[-1]):
+    """consecutive items, in order, grouped so that the sizes of a group sum to at most `budget`; an item larger than the budget forms a
+    group of its own.  Lazy: an item is taken from `items` only when the group before it is complete or still has room."""
+    group, used = [], 0
+    for item in items:
+        n = size(item)
+        if group and used + n > budget:
+            yield group
+            group, used = [], 0
+        group.append(item)
+        used += n
+    if group:
+        yield group
+
+
+def task_inputs(bam, planned, stats=None):
+    """per planned task, in task order: (task id, contig, start, end, BGZF bytes, spans, inflated bytes) of bamio.BamFile.device_input;
+    the time spent reading is added to stats["read_s"]"""
+    for tid, name, s, e in planned:
+        t0 = time.perf_counter()
+        z, spans = bam.device_input([(name, s, e)])
+        n = inflated_bytes(z)
+        if stats is not None:
+            stats["read_s"] += time.perf_counter() - t0
+        yield tid, name, s, e, z, spans, n
+
+
+def join_inputs(inputs):
+    """the device_input of several tasks as one snfb_load_bam input: the BGZF bytes back to back, each task's spans shifted to its bytes
+    and numbered by its place in the pass"""
+    parts, rows, base = [], [], 0
+    for k, (z, spans) in enumerate(inputs):
+        sp = spans.copy()
+        sp["cbeg"] += base
+        sp["cend"] += base
+        sp["task"] = k
+        parts.append(z)
+        rows.append(sp)
+        base += len(z)
+    bgzf = np.concatenate(parts) if parts else np.zeros(0, "u1")
+    return bgzf, np.concatenate(rows) if rows else np.zeros(0, abi.SPAN_DTYPE)
+
+
+def run_pass(ctx, bam, group, config, tr_all, device=0):
+    """one device pass over `group` (items of task_inputs): mask_block, snfb_load_bam, snfb_run, then every task as a CallTask on the
+    pass's BlockRun.  Returns [(CallTask, calls)] in task order and the pass's split {"load_bam_s", "run_s", "finalize_s"}."""
+    tr = {k: [(int(a), int(b)) for a, b in tr_all[g[1]]] for k, g in enumerate(group) if g[1] in tr_all}
+    block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[name], s, e, tid) for tid, name, s, e, *_ in group], tandem_repeats=tr or None)
+    tasks.mask_block(block, config, ctx)
+    ctx.set_config(abi.Config.from_sniffles(config))
+    bgzf, spans = join_inputs([(g[4], g[5]) for g in group])
+    split = {}
+    try:
+        t0 = time.perf_counter()
+        n_rec = ctx.load_bam(bgzf, spans, block)["n_rec"]
+        t1 = time.perf_counter()
+        res = ctx.run(want_leads=True, want_cands=True, want_seqs=True)
+        t2 = time.perf_counter()
+    except binding.SnfbError as e:
+        names = ", ".join(g[1] for g in group)
+        raise CallSampleError(f"the device pass over contig(s) {names} ({sum(g[6] for g in group)} inflated BAM bytes) failed: {e}") from e
+    split["load_bam_s"], split["run_s"] = t1 - t0, t2 - t1
+    rec_nm = abi.view(res._rec_nm_ptr, "<f8", n_rec).copy() if getattr(res, "_rec_nm_ptr", None) else None
+    br = tasks.BlockRun(block, res, tasks.cand_ranges(res.cand, len(block.task)), rec_nm)
+    done = []
+    for k, (tid, name, s, e, *_) in enumerate(group):
+        task = tasks.CallTask(id=tid, sv_id=0, contig=name, start=s, end=e, config=config, block_run=br, task_index=k, device=device)
+        try:
+            calls, _ = task.execute()
+        except tasks.CallTaskError as err:      # logged and left out, as the reference's worker leaves a failed task out
+            log.error(f"Error in worker process while executing CallTask(id={tid}, contig={name}, start={s}, end={e}): {err}")
+            continue
+        done.append((task, calls))
+    split["finalize_s"] = time.perf_counter() - t2
+    return done, split
+
+
+def call_sample(config, device=0, budget=None, stats=None):
+    """the call_sample run mode: config.input (one indexed BAM) -> config.vcf and / or config.snf.  budget: the inflated BAM bytes one
+    device pass may load (default: device_budget).  stats: a dict that receives the run's split (passes, per-pass inflated bytes and
+    times, VCF and SNF write times).  Returns the number of VCF records written."""
+    if getattr(config, "gpus", 1) > 1:
+        raise CallSampleError("--gpus > 1 is not supported for calling a sample: one GPU calls the whole BAM")
+    check_outputs(config)
+    st = stats if stats is not None else {}
+    t0 = time.perf_counter()
+    path = config.input[0] if isinstance(config.input, (list, tuple)) else config.input
+    bam = bamio.BamFile(path)
+    config.task_read_id_offset_mult = read_id_offset_mult(total_mapped(bam))
+    contig_lengths, planned = tasks.plan(bam.contigs, config)
+    config.contig_lengths = contig_lengths
+    tr_all = {}
+    if config.tandem_repeats is not None:
+        tr_all = tasks.load_tandem_repeats(config.tandem_repeats, config.tandem_repeat_region_pad)
+        with_tr = sum(name in tr_all for name, _ in contig_lengths)
+        if with_tr < len(contig_lengths):
+            log.info(f"Info: {with_tr} of {len(contig_lengths)} contigs in the input sample have associated tandem repeat annotations.")
+            if with_tr == 0:
+                raise CallSampleError("A tandem repeat annotations file was provided, but no matching annotations were found for any contig in "
+                                      "the sample input file. Please check if the contig naming scheme in the tandem repeat annotations "
+                                      "matches with the one in the input sample file.")
+    config.sample_ids_vcf = [(0, "SAMPLE" if config.sample_id is None else config.sample_id)]
+    ctx = tasks.device_context(device)
+    reference = tasks.reference_for(ctx, config.reference) if getattr(config, "reference", None) else None
+    if budget is None:
+        budget = device_budget(device)
+    st.update(passes=0, pass_inflated_bytes=[], load_bam_s=[], run_s=[], finalize_s=0.0, vcf_write_s=0.0, snf_write_s=0.0, read_s=0.0)
+    st["index_s"] = time.perf_counter() - t0
+    parts, written = [], 0
+    with contextlib.ExitStack() as stack:
+        writer = None
+        if config.vcf is not None:
+            handle = vcf.open_output(config, ctx)
+            if config.vcf_output_bgz:
+                stack.enter_context(handle)               # compressed and indexed when the run ends without an error
+            else:
+                stack.callback(handle.close)
+            writer = vcf.VCFWriter(config, handle, reference)
+            writer.write_header(contig_lengths)
+        for group in group_passes(task_inputs(bam, planned, st), budget):
+            done, split = run_pass(ctx, bam, group, config, tr_all, device)
+            st["passes"] += 1
+            st["pass_inflated_bytes"].append(sum(g[6] for g in group))
+            st["load_bam_s"].append(split["load_bam_s"])
+            st["run_s"].append(split["run_s"])
+            st["finalize_s"] += split["finalize_s"]
+            t1 = time.perf_counter()
+            if writer is not None:
+                if reference is not None:
+                    reference.prefetch(vcf.reference_intervals([c for _, calls in done for c in calls], config))
+                for _, calls in done:
+                    for c in calls:
+                        written += writer.write_call(c)
+            t2 = time.perf_counter()
+            parts.extend(task.snf_part for task, _ in done if task.snf_part is not None)
+            st["vcf_write_s"] += t2 - t1
+        t1 = time.perf_counter()
+    st["vcf_write_s"] += time.perf_counter() - t1          # the .vcf.gz compression and .tbi when the handle closes
+    if config.snf is not None:
+        t1 = time.perf_counter()
+        with open(config.snf, "wb") as f:
+            n = snf.write_results(f, config, parts, [name for name, _ in contig_lengths])
+        st["snf_write_s"] = time.perf_counter() - t1
+        log.info(f"Wrote {n} SV candidates to {config.snf} (for multi-sample calling).")
+    if config.vcf is not None:
+        log.info(f"Wrote {written} called SVs to {config.vcf}")
+    st["wall_s"] = time.perf_counter() - t0
+    return written

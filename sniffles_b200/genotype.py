@@ -156,32 +156,14 @@ def rewrite_line(target, config):
     return "\t".join(target.raw_vcf_line.split("\t")[:8] + [config.genotype_format, vcf.format_genotype(genotype_of(target, config), config.phase)])
 
 
-def should_process_contig(contig, length, config):
-    """util.should_process_contig (util.py:150-164)"""
-    regions = getattr(config, "regions_by_contig", None) or {}
-    if config.contig and contig not in config.contig:
-        return False
-    if regions and contig not in regions:
-        return False
-    if not config.all_contigs and length < 1_000_000:
-        return bool((config.contig and contig in config.contig) or (contig in regions))
-    return True
-
-
 def plan(contigs, targets, config):
-    """one task per processed contig (task_count_multiplier 0, sniffles:289-358): [(task id, contig, start, end, [Target])]; task ids
-    count every planned task, as the reference numbers them"""
+    """the task plan of tasks.plan (one task per processed contig, sniffles:289-358) with each task's targets: [(task id, contig, start,
+    end, [Target])], a task holding the targets of its contig with start <= pos < end"""
+    from . import tasks
     by_contig = {}
     for t in targets:
         by_contig.setdefault(t.contig, []).append(t)
-    out, task_id = [], 0
-    for name, length in contigs:
-        if not should_process_contig(name, length, config) or length - 1 <= 0:
-            continue
-        end = length - 1
-        out.append((task_id, name, 0, end, [t for t in by_contig.get(name, []) if 0 <= t.pos < end]))
-        task_id += 1
-    return out
+    return [(tid, name, s, e, [t for t in by_contig.get(name, []) if s <= t.pos < e]) for tid, name, s, e in tasks.plan(contigs, config)[1]]
 
 
 def encode(targets, task_index, name_to_id):

@@ -118,6 +118,33 @@ def load_tandem_repeats(filename, padding):
     return contigs_tr
 
 
+def should_process_contig(contig, length, config):
+    """util.should_process_contig (util.py:150-164): --contig, --regions and, without --all-contigs, the 1 Mb rule"""
+    regions = getattr(config, "regions_by_contig", None) or {}
+    if config.contig and contig not in config.contig:
+        return False
+    if regions and contig not in regions:
+        return False
+    if not config.all_contigs and length < 1_000_000:
+        return bool((config.contig and contig in config.contig) or (contig in regions))
+    return True
+
+
+def plan(contigs, config):
+    """the task plan of a BAM header for call_sample and genotype_vcf (sniffles:311-358 with task_count_multiplier 0): contigs = [(name,
+    length)] in header order.  Returns (processed, planned): processed = [(name, length)] of every contig should_process_contig keeps (the
+    VCF header's contigs and the SNF's contig list); planned = [(task id, name, 0, length - 1)], one task per processed contig longer than
+    one base, task ids counted over the planned tasks only, as the reference numbers them."""
+    processed, planned = [], []
+    for name, length in contigs:
+        if not should_process_contig(name, length, config):
+            continue
+        processed.append((name, length))
+        if length - 1 > 0:
+            planned.append((len(planned), name, 0, length - 1))
+    return processed, planned
+
+
 @dataclass
 class Task:
     id: int
@@ -222,15 +249,45 @@ class Task:
         return postprocess.finalize_candidates(candidates, keep_qc_fails, config, self.coverage_average_total)
 
 
+def first_unanchored_bnd(calls):
+    """the first BND candidate of a task with no non-BND candidate before it, or None.  postprocessing.coverage (postprocessing.py:81-90)
+    leaves `end` unbound for such a BND and raises UnboundLocalError, which fails the whole task in the reference's worker."""
+    return calls[0] if calls and calls[0].svtype == "BND" else None
+
+
+class CallTaskError(RuntimeError):
+    """the task fails as the reference's worker fails it (parallel.py:747-752): none of its records or SNF candidates are written"""
+
+
 class CallTask(Task):
+    # with config.snf, the task's SNF part after execute: (task id, contig, block index {block: (offset, length)}, part bytes, candidate
+    # count, coverage_average_total) -- what CallResult carries to SNFile.write_results (parallel.py:279-294); snf.write_results joins them
+    snf_part: Optional[tuple] = None
+
     def execute(self, worker=None):
-        """parallel.py:256-297 (VCF path; SNF parts are a "next" row)"""
+        """parallel.py:256-297.  Returns (calls, read_count): the calls the VCF gets, QC fails dropped unless --no-qc, sorted by position
+        with config.sort.  With config.snf the task also builds its SNF part in memory (`snf_part`), as the reference writes its
+        temporary part file: every candidate after finalize, QC fails included, stored by SNFWriter, each block's `_COVERAGE` from
+        snfb_coverage_bins over the block loaded on the task's device context, then write_and_index."""
         config = self.config
         self.bind(worker)
         qc = not (config.snf is not None or config.no_qc)
         _, read_count = self.build_leadtab()
         cands = self.call_candidates(qc, config)
+        bad = first_unanchored_bnd(cands)
+        if bad is not None:
+            raise CallTaskError(f"candidate {bad.id} is a BND with no earlier non-BND candidate in its task")
         calls = self.finalize_candidates(cands, not qc, config)
+        if config.snf is not None:
+            import io
+            from . import snf
+            buf = io.BytesIO()
+            part = snf.SNFWriter(config, buf)
+            for c in calls:
+                part.store(c)
+            part.annotate_block_coverages(self._ctx().coverage_bins(self.task_index, config.coverage_binsize_combine))
+            part.write_and_index()
+            self.snf_part = (self.id, self.contig, dict(part.index), buf.getvalue(), len(calls), self.coverage_average_total)
         if not config.no_qc:
             calls = [c for c in calls if c.qc]
         if config.sort:
@@ -257,11 +314,9 @@ class GenotypeTask(Task):
         cands = self.call_candidates(False, config)
         calls = self.finalize_candidates(cands, True, config)
         targets = list(self.genotype_svs or [])
-        seen = False
-        for c in calls:          # postprocessing.coverage over the candidates raises UnboundLocalError before any target is looked at
-            if c.svtype == "BND" and not seen:
-                raise GenotypeTaskError(f"candidate {c.id} is a BND with no earlier non-BND candidate in its task")
-            seen = seen or c.svtype != "BND"
+        bad = first_unanchored_bnd(calls)   # postprocessing.coverage over the candidates raises UnboundLocalError before any target is looked at
+        if bad is not None:
+            raise GenotypeTaskError(f"candidate {bad.id} is a BND with no earlier non-BND candidate in its task")
         for t in targets:
             if t.svtype not in genotype.SVTYPE_CODE:
                 genotype.log.warning(f"Unsupported SVTYPE: {t.svtype}")
