@@ -107,7 +107,7 @@ typedef struct snfb_rec {
     uint32_t n_cigar;     /* words of this record (CIGAR16: pad words inside included)   */
     int32_t  l_seq;       /* query_length (bases stored in seq)                         */
     uint32_t sa_len;
-    uint32_t _pad1;
+    uint32_t region;      /* index into the region table (snfb_set_regions); ignored while that table is empty */
     uint64_t cigar_off;   /* in words of the block's cigar_fmt (CIGAR16: a multiple of 8) */
     uint64_t seq_off;     /* in bytes                                                   */
     uint64_t var_off;     /* in bytes                                                   */
@@ -306,7 +306,7 @@ typedef struct snfb_ctx snfb_ctx;
 
 int         snfb_version(void);
 /* sizeof of the ABI structs, for binding self-checks: 0 rec, 1 task, 2 contig, 3 records, 4 config, 5 lead, 6 cand, 7 gather_view,
- * 8 gt_in, 9 gt_out, 10 ref_contig, 11 ref_input, 12 ref_query */
+ * 8 gt_in, 9 gt_out, 10 ref_contig, 11 ref_input, 12 ref_query, 13 region */
 size_t      snfb_sizeof(int which);
 uint64_t    snfb_hash_name(const char* s, size_t n);
 int         snfb_ctx_create(int device, snfb_ctx** out);
@@ -341,7 +341,7 @@ typedef struct snfb_bam_span {
     uint64_t cbeg, cend;      /* byte offsets of BGZF block starts inside bgzf[] */
     uint32_t ubeg, uend;      /* offsets inside those blocks' inflated data */
     uint32_t task;
-    uint32_t _pad;
+    uint32_t region;          /* index into the region table (snfb_set_regions); ignored while that table is empty */
 } snfb_bam_span;
 typedef struct snfb_bam_input {
     const uint8_t* bgzf; uint64_t n_bytes;
@@ -350,6 +350,25 @@ typedef struct snfb_bam_input {
     const snfb_task* task; const snfb_contig* contig; const int32_t* tr; const int32_t* mask; const uint32_t* mask_task_off;
 } snfb_bam_input;
 int         snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in);
+/* ---- regions (--regions / --region): LeadProvider.build_leadtab over a task's list of regions (leadprov.py:445-470) ----
+ * A task keeps one contig and clusters as one unit; its regions are segments of its records.  For each region in table order the
+ * reference runs bam.fetch(contig, start, end), keeps the reads with start <= reference_start < end and records a lead only when
+ * start <= lead.ref_start < end of the region it came from.  A read two regions take is read twice: two records, two read ids, its
+ * coverage and NM counted twice.  config.average_regional_nm is the mean over the LAST region's reads only (nm_sum is reset per
+ * iter_region, leadprov.py:475-577).
+ * The table applies to the next snfb_load_records / snfb_load_bam on the context only: a load not preceded by this call has no table
+ * (n = 0 is the same), and then snfb_rec.region / snfb_bam_span.region are ignored and every task is its own single region
+ * [task.start, task.end).  With a table:
+ *   - regions are grouped by task, in the task's order (start > end or start < 0 is refused: the host fails that task instead);
+ *   - snfb_rec.region (host records) and snfb_bam_span.region (device ingest) name a region of the record's / span's own task;
+ *     records come grouped by (task, region, BAM order) and spans by (task, region), each region's spans in file order;
+ *   - the record filters, the fetch overlap test of the ingest and the lead filters use the record's region;
+ *   - task.start / task.end only clip the N mask: the host clips the runs to the regions and passes [0, contig_len].
+ * When some task has more than one region, the block is not coordinate sorted inside that task (a region's fetch also returns the
+ * reads that start before it and overlap it); stage A then builds a coordinate-ordered copy of (pos, end, flags) with a stable radix
+ * sort on (task, pos) (timing mark "cov_order") that every coverage reader uses. */
+typedef struct snfb_region { int32_t task, start, end, _pad; } snfb_region;
+int         snfb_set_regions(snfb_ctx* ctx, const snfb_region* regions, uint32_t n);
 /* what the last snfb_load_bam built: out[0] records, out[1] CIGAR16 words, out[2] var bytes, out[3] seq bytes, out[4] raw records seen,
  * out[5] BGZF blocks, out[6] inflated bytes, out[7] compressed bytes */
 int         snfb_ingest_sizes(snfb_ctx* ctx, uint64_t out[8]);

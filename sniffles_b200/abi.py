@@ -15,7 +15,7 @@ LF_REVERSE, LF_IS_SA, LF_SVLEN_NONE, LF_BND_FIRST, LF_BND_REVERSE, LF_HAS_SEQ = 
 REC_DTYPE = np.dtype([
     ("task", "<i4"), ("pos", "<i4"), ("flag", "<u2"), ("mapq", "u1"), ("aux_flags", "u1"),
     ("hp", "u1"), ("l_qname", "u1"), ("_pad0", "<u2"), ("nm", "<i4"), ("ps", "<i4"),
-    ("n_cigar", "<u4"), ("l_seq", "<i4"), ("sa_len", "<u4"), ("_pad1", "<u4"),
+    ("n_cigar", "<u4"), ("l_seq", "<i4"), ("sa_len", "<u4"), ("region", "<u4"),
     ("cigar_off", "<u8"), ("seq_off", "<u8"), ("var_off", "<u8")])
 assert REC_DTYPE.itemsize == 64
 
@@ -52,7 +52,8 @@ class Records(C.Structure):
                 ("cigar_evt_min", C.c_uint32), ("_pad2", C.c_uint32)]
 
 
-SPAN_DTYPE = np.dtype([("cbeg", "<u8"), ("cend", "<u8"), ("ubeg", "<u4"), ("uend", "<u4"), ("task", "<u4"), ("_pad", "<u4")])      # snfb_bam_span
+SPAN_DTYPE = np.dtype([("cbeg", "<u8"), ("cend", "<u8"), ("ubeg", "<u4"), ("uend", "<u4"), ("task", "<u4"), ("region", "<u4")])      # snfb_bam_span
+REGION_DTYPE = np.dtype([("task", "<i4"), ("start", "<i4"), ("end", "<i4"), ("_pad", "<i4")])      # snfb_region
 assert SPAN_DTYPE.itemsize == 32
 
 

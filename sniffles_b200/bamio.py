@@ -328,19 +328,25 @@ class BamFile:
                         for c in bins[b] if c[1] > min_off)
         return [(a, b) for a, b in _merge_ranges((max(beg, min_off), stop) for beg, stop in chunks) if b > a]
 
-    def device_input(self, regions, split=True):
+    def device_input(self, regions, split=True, tags=None):
         """regions: [(contig, start, end)] = the tasks, in task order.  Returns (bgzf, spans): the compressed bytes of every BGZF block the
         regions need (file order, each block once) and abi.SPAN_DTYPE rows — the merged index chunks of each task, cut at the linear
-        index's record-aligned offsets so that every ~16 kb window is its own parallel walk on the device."""
-        pieces = []                                      # (task, vbeg, vend)
-        for t, (contig, start, end) in enumerate(regions):
-            anchors = self._anchors(self.name_to_id[contig]) if split else []
+        index's record-aligned offsets so that every ~16 kb window is its own parallel walk on the device.  tags: per query (task, region)
+        for the spans (default: query k is task k, region 0); several queries of a task share its BGZF blocks, shipped once."""
+        pieces = []                                      # (task, vbeg, vend, region)
+        tags = tags if tags is not None else [(t, 0) for t in range(len(regions))]
+        anchors_of = {}                                  # per contig, sorted once: each chunk bisects into them
+        for (t, g), (contig, start, end) in zip(tags, regions):
+            rid = self.name_to_id[contig]
+            if split and rid not in anchors_of:
+                anchors_of[rid] = self._anchors(rid)
+            anchors = anchors_of.get(rid, [])
             for vb, ve in self.merged_chunks(contig, start, end):
-                cuts = [vb] + [a for a in anchors if vb < a < ve] + [ve]
-                pieces.extend((t, cuts[k], cuts[k + 1]) for k in range(len(cuts) - 1))
+                cuts = [vb] + anchors[bisect.bisect_right(anchors, vb):bisect.bisect_left(anchors, ve)] + [ve]
+                pieces.extend((t, cuts[k], cuts[k + 1], g) for k in range(len(cuts) - 1))
         # file intervals [cb, ce) that hold the blocks of the pieces; a piece that ends inside a block needs that block too
         iv, bs_cache = [], {}
-        for _, vb, ve in pieces:
+        for _, vb, ve, _ in pieces:
             cb, ce = vb >> 16, ve >> 16
             if ve & 0xffff:
                 if ce not in bs_cache:
@@ -367,26 +373,26 @@ class BamFile:
                 raise ValueError("virtual offset outside the loaded intervals")
             return base[k] + (c - starts[k])
         spans = np.zeros(len(pieces), abi.SPAN_DTYPE)
-        for i, (t, vb, ve) in enumerate(pieces):
-            spans[i] = (to_buf(vb >> 16), to_buf(ve >> 16), vb & 0xffff, ve & 0xffff, t, 0)
+        for i, (t, vb, ve, g) in enumerate(pieces):
+            spans[i] = (to_buf(vb >> 16), to_buf(ve >> 16), vb & 0xffff, ve & 0xffff, t, g)
         return bgzf, spans
 
 
 def pack_records(contigs, recs, tasks, with_seq=True, tandem_repeats=None) -> RecordBlock:
     """records (already grouped by task, coordinate sorted inside a task) -> packed block of include/snfb.h.
-    tasks: list of (contig index, start, end, task_id); recs: list of (task index, record dict)."""
+    tasks: list of (contig index, start, end, task_id); recs: list of (task index, record dict[, region index])."""
     n = len(recs)
     rec = np.zeros(n, abi.REC_DTYPE)
     cig, var, seq = [], [], []
     co = vo = so = 0
-    for i, (t, r) in enumerate(recs):
+    for i, (t, r, *g) in enumerate(recs):
         a = r["aux"]
         sa = a.get("SA", b"")
         flags = (abi.AUX_NM if "NM" in a else 0) | (abi.AUX_HP if "HP" in a else 0) | (abi.AUX_PS if "PS" in a else 0) | (abi.AUX_SA if "SA" in a else 0)
         if len(r["qname"]) > 255:
             raise ValueError("query name longer than 255 bytes")
         rec[i] = (t, r["pos"], r["flag"], r["mapq"], flags, int(a.get("HP", 0)) & 255, len(r["qname"]), 0,
-                  int(a.get("NM", 0)), int(a.get("PS", 0)), len(r["cigar"]), r["l_seq"], len(sa), 0, co, so, vo)
+                  int(a.get("NM", 0)), int(a.get("PS", 0)), len(r["cigar"]), r["l_seq"], len(sa), g[0] if g else 0, co, so, vo)
         cig.append(r["cigar"])
         var.append(np.frombuffer(r["qname"] + sa, "u1"))
         s = r["seq"] if with_seq else np.zeros((r["l_seq"] + 1) // 2, "u1")

@@ -17,7 +17,7 @@ EXPORTS = ["snfb_version", "snfb_sizeof", "snfb_hash_name", "snfb_ctx_create", "
            "snfb_last_timings", "snfb_device_candidates", "snfb_device_alt", "snfb_launch_count",
            "snfb_pin_host", "snfb_unpin_host", "snfb_pack_cigar16", "snfb_rerun_count", "snfb_coverage_bins",
            "snfb_nccl_unique_id", "snfb_comm_init", "snfb_allgather_candidates", "snfb_selftest_sqrt_frac", "snfb_poa", "snfb_combine_groups", "snfb_selftest_edit_distance",
-           "snfb_load_bam", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf", "snfb_deflate_bgzf",
+           "snfb_load_bam", "snfb_set_regions", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf", "snfb_deflate_bgzf",
            "snfb_genotype_targets", "snfb_load_reference", "snfb_reference_runs", "snfb_fetch_reference"]
 
 
@@ -40,6 +40,7 @@ def lib():
         L.snfb_set_config.argtypes = [C.c_void_p, C.POINTER(abi.Config)]
         L.snfb_load_records.argtypes = [C.c_void_p, C.POINTER(abi.Records)]
         L.snfb_load_bam.argtypes = [C.c_void_p, C.POINTER(abi.BamInput)]
+        L.snfb_set_regions.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
         L.snfb_ingest_sizes.argtypes = [C.c_void_p, C.c_void_p]
         L.snfb_ingest_fetch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.snfb_inflate_bgzf.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
@@ -174,6 +175,12 @@ class Context:
             rs.on_device = 2
         self._block = block          # keep host arrays alive during the async copy
         self._check(self._lib.snfb_load_records(self._h, C.byref(rs)), "snfb_load_records")
+
+    def set_regions(self, regions=None):
+        """snfb_set_regions: abi.REGION_DTYPE rows (grouped by task) for the next load; None or empty clears the table"""
+        r = np.ascontiguousarray(regions if regions is not None else np.zeros(0, abi.REGION_DTYPE), dtype=abi.REGION_DTYPE)
+        self._regions = r
+        self._check(self._lib.snfb_set_regions(self._h, r.ctypes.data if len(r) else None, len(r)), "snfb_set_regions")
 
     def load_bam(self, bgzf: np.ndarray, spans: np.ndarray, tables):
         """Device BAM ingest (snfb_load_bam): `bgzf` = whole BGZF blocks (uint8), `spans` = abi.SPAN_DTYPE rows (bamio.BamFile.device_input

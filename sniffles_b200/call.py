@@ -86,27 +86,38 @@ def group_passes(items, budget, size=lambda item: item[-1]):
         yield group
 
 
-def task_inputs(bam, planned, stats=None):
-    """per planned task, in task order: (task id, contig, start, end, BGZF bytes, spans, inflated bytes) of bamio.BamFile.device_input;
-    the time spent reading is added to stats["read_s"]"""
+def task_inputs(bam, planned, stats=None, regions_by_contig=None):
+    """per planned task, in task order: (task id, contig, start, end, BGZF bytes, spans, inflated bytes, regions) of
+    bamio.BamFile.device_input over the task's fetch windows (tasks.fetch_windows; regions: those windows when the contig has regions, else
+    None).  A task whose regions pysam would refuse is logged and left out, as the reference's worker fails it.  The time spent reading
+    is added to stats["read_s"]"""
     for tid, name, s, e in planned:
         t0 = time.perf_counter()
-        z, spans = bam.device_input([(name, s, e)])
+        rg = (regions_by_contig or {}).get(name)
+        try:
+            windows = tasks.fetch_windows(name, s, e, rg)
+        except ValueError as err:
+            log.error(f"Error in worker process while executing CallTask(id={tid}, contig={name}, start={s}, end={e}): {err}")
+            continue
+        z, spans = bam.device_input([(name, a, b) for a, b in windows], tags=[(0, g) for g in range(len(windows))])
         n = inflated_bytes(z)
         if stats is not None:
             stats["read_s"] += time.perf_counter() - t0
-        yield tid, name, s, e, z, spans, n
+        yield tid, name, s, e, z, spans, n, (windows if rg else None)
 
 
-def join_inputs(inputs):
+def join_inputs(inputs, n_regions=None):
     """the device_input of several tasks as one snfb_load_bam input: the BGZF bytes back to back, each task's spans shifted to its bytes
-    and numbered by its place in the pass"""
-    parts, rows, base = [], [], 0
+    and numbered by its place in the pass; n_regions: per task the number of its regions, whose span tags move to the pass's region table"""
+    parts, rows, base, rbase = [], [], 0, 0
     for k, (z, spans) in enumerate(inputs):
         sp = spans.copy()
         sp["cbeg"] += base
         sp["cend"] += base
         sp["task"] = k
+        if n_regions is not None:
+            sp["region"] += rbase
+            rbase += n_regions[k]
         parts.append(z)
         rows.append(sp)
         base += len(z)
@@ -118,13 +129,19 @@ def run_pass(ctx, bam, group, config, tr_all, device=0):
     """one device pass over `group` (items of task_inputs): mask_block, snfb_load_bam, snfb_run, then every task as a CallTask on the
     pass's BlockRun.  Returns [(CallTask, calls)] in task order and the pass's split {"load_bam_s", "run_s", "finalize_s"}."""
     tr = {k: [(int(a), int(b)) for a, b in tr_all[g[1]]] for k, g in enumerate(group) if g[1] in tr_all}
-    block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[name], s, e, tid) for tid, name, s, e, *_ in group], tandem_repeats=tr or None)
-    tasks.mask_block(block, config, ctx)
+    # a task with regions: its records carry their region's window, its own bounds only clip the N mask (the host clips it to the regions)
+    bounds = [(0, bam.get_reference_length(name)) if rg else (s, e) for _, name, s, e, _, _, _, rg in group]
+    block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[g[1]], a, b, g[0]) for g, (a, b) in zip(group, bounds)], tandem_repeats=tr or None)
+    by_task = [(k, g[7] or [(g[2], g[3])]) for k, g in enumerate(group)]
+    has_regions = any(g[7] for g in group)
+    mask_regions = {k: g[7] for k, g in enumerate(group) if g[7]}
+    tasks.mask_block(block, config, ctx, mask_regions) if mask_regions else tasks.mask_block(block, config, ctx)
     ctx.set_config(abi.Config.from_sniffles(config))
-    bgzf, spans = join_inputs([(g[4], g[5]) for g in group])
+    bgzf, spans = join_inputs([(g[4], g[5]) for g in group], [len(w) for _, w in by_task] if has_regions else None)
     split = {}
     try:
         t0 = time.perf_counter()
+        ctx.set_regions(tasks.region_table(by_task) if has_regions else None)
         n_rec = ctx.load_bam(bgzf, spans, block)["n_rec"]
         t1 = time.perf_counter()
         res = ctx.run(want_leads=True, want_cands=True, want_seqs=True)
@@ -190,7 +207,7 @@ def call_sample(config, device=0, budget=None, stats=None):
                 stack.callback(handle.close)
             writer = vcf.VCFWriter(config, handle, reference)
             writer.write_header(contig_lengths)
-        for group in group_passes(task_inputs(bam, planned, st), budget):
+        for group in group_passes(task_inputs(bam, planned, st, config.regions_by_contig), budget, size=lambda item: item[6]):
             done, split = run_pass(ctx, bam, group, config, tr_all, device)
             st["passes"] += 1
             st["pass_inflated_bytes"].append(sum(g[6] for g in group))

@@ -4,8 +4,53 @@ config namespace (Task, QC, genotyping, writers) runs unchanged.  Table-driven r
 copy of the reference's argparse set-up; only flags that reach the hot path, the QC/genotype
 epilogue or the writers are declared."""
 import argparse
+import logging
 import os
 import tempfile
+
+log = logging.getLogger(__name__)
+
+
+def _bed_region(line):
+    """(contig, start, end) of a BED line's first three tab-separated fields; ValueError when they are missing or not integers"""
+    fields = line.split("\t")
+    if len(fields) < 3:
+        raise ValueError(f"{len(fields)} tab-separated field(s), 3 needed")
+    return fields[0], int(fields[1]), int(fields[2])
+
+
+def _string_region(text):
+    """(contig, start, end) of `contig:start-end`; ValueError for any other shape"""
+    parts = text.split(":")
+    if len(parts) != 2:
+        raise ValueError("expected one ':'")
+    bounds = parts[1].split("-")
+    if len(bounds) != 2:
+        raise ValueError("expected one '-'")
+    return parts[0], int(bounds[0]), int(bounds[1])
+
+
+def regions_by_contig(config):
+    """the regions of --regions (a BED file; lines starting with '#' and blank lines skipped) or, without it, of the --region strings:
+    {contig: [(contig, start, end), ...]} in input order, never sorted or merged.  An entry that does not parse is skipped with a warning;
+    a missing BED file raises FileNotFoundError; --contig together with --regions exits.  Pinned against the reference's parser by
+    tests/golden/regions/expected.json."""
+    if config.contig and config.regions:
+        raise SystemExit("Please provide either --contig or --regions, not both.")
+    if config.regions is not None:
+        with open(config.regions, "r") as f:
+            entries = [(line, _bed_region) for line in f.readlines() if not line.startswith("#") and line.strip() != ""]
+    else:
+        entries = [(text, _string_region) for text in config.region or []]
+    out = {}
+    for text, parse in entries:
+        try:
+            r = parse(text)
+        except ValueError as e:
+            log.warning(f"skipping region {text!r}: {e}")
+            continue
+        out.setdefault(r[0], []).append(r)
+    return out
 
 
 def _tobool(v):
@@ -156,7 +201,7 @@ class SnifflesConfig(argparse.Namespace):
         if not self.tmp_dir or not os.path.exists(self.tmp_dir):
             self.tmp_dir = tempfile.gettempdir()
         self.task_count_multiplier = 0
-        self.regions_by_contig = {}
+        self.regions_by_contig = regions_by_contig(self)
         # --minsvlen: "~N" = soft cap (config.py:507-517)
         ms = str(self.minsvlen)
         self.minsvlen_hard_cap = not ms.startswith("~")

@@ -107,12 +107,17 @@ struct snfb_ctx {
     DevBuf b_ref, b_ref_work; std::vector<refseq::Contig> ref_ctg; bool have_ref = false;     // the unwrapped reference genome; tables / counters / N-run scratch
     HostBuf h_ref_runs, h_ref_coff, h_ref_out; uint64_t ref_n_runs = 0;                       // N runs and per-contig offsets; gather staging
     std::vector<snfb_task> tasks;
+    // region table (snfb_set_regions): host copy, device copy followed by each task's last region index; cov_view: some task's regions
+    // are not increasing and disjoint, so stage A builds the coordinate-ordered (pos, end, flags) the coverage readers search
+    std::vector<snfb_region> regions, next_regions; DevBuf b_region; uint32_t n_region = 0; bool cov_view = false;
     // capacities and the three arenas carved by them
     Caps cap; bool force_no_cuts = false;
     DevBuf b_ctr, arena_r, arena_l, arena_c;            // counters; per-record arrays; per-lead arrays (stages A + B); stage C
     // per-record (arena_r)
     int32_t* rec_pos; int32_t* rec_end; uint8_t* rec_flags; double* rec_nm; uint32_t* rec_nlead; uint32_t* rec_lead_off; uint32_t* sa_list; extract::RecScan* scanrec; extract::RecClip* clip; int32_t* rec_big;
     uint32_t* task_first; uint32_t* task_last; uint32_t* task_reads; unsigned long long* task_cov; int32_t* task_span; double* task_nm; double* nm_part; unsigned* nm_cnt; extract::Seg* sa_seg; uint32_t* scan_tmp_r;
+    // the coordinate-ordered copy of (rec_pos, rec_end, rec_flags) and its sort scratch (one element each unless cov_view)
+    int32_t* v_pos; int32_t* v_end; uint8_t* v_flags; uint64_t* v_k0; uint64_t* v_k1; uint32_t* v_v0; uint32_t* v_v1; uint32_t* v_hist; uint32_t* v_scan; unsigned long long* v_n;
     // per-lead (arena_l): stage A leads + the whole of stage B
     snfb_lead* leads; extract::Event* ev_buf; snfb_lead* sorted_leads; uint32_t* radix_hist;
     cluster::B B{};
@@ -152,6 +157,19 @@ static int bits_for(uint32_t n) { int b = 0; while ((1ull << b) < n) ++b; return
 __global__ void k_gather_leads(const snfb_lead* __restrict__ leads, const uint32_t* __restrict__ sval, snfb_lead* __restrict__ out, const unsigned long long* n_ptr, unsigned long long cap) {
     const unsigned long long n = *n_ptr < cap ? *n_ptr : cap;
     for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) out[i] = leads[sval[i]];
+}
+// sort keys of the coordinate-ordered record view: (task, pos) with the sign of pos flipped so that unsigned order is numeric order
+__global__ void k_view_keys(const snfb_rec* __restrict__ rec, const int32_t* __restrict__ rec_pos, unsigned long long n, uint64_t* __restrict__ key, uint32_t* __restrict__ val, unsigned long long* n_out) {
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
+        key[i] = ((uint64_t)(uint32_t)__ldg(&rec[i].task) << 32) | (uint64_t)((uint32_t)rec_pos[i] ^ 0x80000000u); val[i] = (uint32_t)i;
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) *n_out = n;
+}
+__global__ void k_view_gather(const uint32_t* __restrict__ ord, unsigned long long n, const int32_t* __restrict__ pos, const int32_t* __restrict__ end, const uint8_t* __restrict__ flags,
+                              int32_t* __restrict__ v_pos, int32_t* __restrict__ v_end, uint8_t* __restrict__ v_flags) {
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const uint32_t j = ord[i]; v_pos[i] = pos[j]; v_end[i] = end[j]; v_flags[i] = flags[j];
+    }
 }
 // mean coverage per bin of `binsize` bases over the whole contig (snf.py:248-267): sum over the bin's positions of the per-base
 // depth / binsize, from the per-record (start, end) arrays: one thread per record adds its overlap with every bin it touches
@@ -241,7 +259,7 @@ size_t snfb_sizeof(int which) {
     switch (which) { case 0: return sizeof(snfb_rec); case 1: return sizeof(snfb_task); case 2: return sizeof(snfb_contig); case 3: return sizeof(snfb_records);
                      case 4: return sizeof(snfb_config); case 5: return sizeof(snfb_lead); case 6: return sizeof(snfb_cand); case 7: return sizeof(snfb_gather_view);
                      case 8: return sizeof(snfb_gt_in); case 9: return sizeof(snfb_gt_out);
-                     case 10: return sizeof(snfb_ref_contig); case 11: return sizeof(snfb_ref_input); case 12: return sizeof(snfb_ref_query); default: return 0; }
+                     case 10: return sizeof(snfb_ref_contig); case 11: return sizeof(snfb_ref_input); case 12: return sizeof(snfb_ref_query); case 13: return sizeof(snfb_region); default: return 0; }
 }
 
 uint64_t snfb_hash_name(const char* s, size_t n) {
@@ -343,6 +361,15 @@ static int check_tables(snfb_ctx* ctx, const snfb_records* R) {
         if (k.contig_len < 0 || k.start > k.end) return fail(ctx, "task table: bad region");
         if ((long long)k.contig_len >= ((long long)1 << 26) * (long long)(ctx->have_cfg ? ctx->cfg.cluster_binsize : 100)) return fail(ctx, "contig too long for the bin field of the sort key (contig_len / cluster_binsize must stay below 2^26)");
     }
+    if (ctx->n_region) {
+        for (uint32_t g = 0; g < ctx->n_region; ++g) {
+            const snfb_region& r = ctx->regions[g];
+            const std::string who = "region " + std::to_string(g) + " (task " + std::to_string(r.task) + ")";
+            if (r.task < 0 || (uint32_t)r.task >= R->n_task) return fail(ctx, "region table: " + who + ": task index out of range");
+            if (g && r.task < ctx->regions[g - 1].task) return fail(ctx, "region table: " + who + ": regions must be grouped by task in task order");
+            if (r.start < 0 || r.start > r.end) return fail(ctx, "region table: " + who + ": start < 0 or start > end");
+        }
+    }
     if (R->n_mask && R->mask && R->mask_task_off) {
         for (uint32_t t = 0; t < R->n_task; ++t) if (R->mask_task_off[t] > R->mask_task_off[t + 1] || R->mask_task_off[t + 1] > R->n_mask) return fail(ctx, "mask_task_off must be non-decreasing and end at n_mask");
         // the probes binary-search a task's runs and the contig mean subtracts each run once: they must be sorted and disjoint
@@ -370,6 +397,22 @@ static int upload_tables(snfb_ctx* ctx, const snfb_records* R) {
         CUDA_TRY(cudaMemcpyAsync(ctx->b_trp.p, pm.data(), 4 * (size_t)R->n_tr, cudaMemcpyHostToDevice, ctx->st));
         CUDA_TRY(cudaStreamSynchronize(ctx->st));     // pm is a stack-owned staging vector
     }
+    ctx->cov_view = false;
+    if (ctx->n_region) {
+        // the table, then per task the index of its last region (-1: none).  Block order is coordinate order inside a task only when it
+        // has one region: a later region's fetch also returns the reads that start before it and overlap it, even when the regions are
+        // sorted and disjoint
+        std::vector<int32_t> last(R->n_task, -1);
+        for (uint32_t g = 0; g < ctx->n_region; ++g) {
+            const snfb_region& r = ctx->regions[g];
+            if (last[r.task] >= 0) ctx->cov_view = true;
+            last[r.task] = (int32_t)g;
+        }
+        if (ctx->b_region.ensure(sizeof(snfb_region) * ctx->n_region + 4 * (size_t)R->n_task)) return fail(ctx, "out of device memory (region table)");
+        CUDA_TRY(cudaMemcpyAsync(ctx->b_region.p, ctx->regions.data(), sizeof(snfb_region) * ctx->n_region, cudaMemcpyHostToDevice, ctx->st));
+        CUDA_TRY(cudaMemcpyAsync(ctx->b_region.as<uint8_t>() + sizeof(snfb_region) * ctx->n_region, last.data(), 4 * (size_t)R->n_task, cudaMemcpyHostToDevice, ctx->st));
+        CUDA_TRY(cudaStreamSynchronize(ctx->st));     // last is a stack-owned staging vector
+    }
     ctx->n_mask = (R->mask && R->mask_task_off) ? R->n_mask : 0;
     if (ctx->n_mask) {
         std::vector<uint32_t> mt(ctx->n_mask);
@@ -383,14 +426,31 @@ static int upload_tables(snfb_ctx* ctx, const snfb_records* R) {
     return 0;
 }
 
+int snfb_set_regions(snfb_ctx* ctx, const snfb_region* regions, uint32_t n) {
+    if (!ctx || (n && !regions)) return 1;
+    ctx->next_regions.assign(regions, regions + n);
+    return 0;
+}
+// a load takes the table snfb_set_regions left for it, or none
+static void take_regions(snfb_ctx* ctx) { ctx->regions.swap(ctx->next_regions); ctx->next_regions.clear(); ctx->n_region = (uint32_t)ctx->regions.size(); }
+static const snfb_region* dev_regions(snfb_ctx* ctx) { return ctx->n_region ? ctx->b_region.as<snfb_region>() : nullptr; }
+static const int32_t* dev_last_region(snfb_ctx* ctx) { return ctx->n_region ? reinterpret_cast<const int32_t*>(ctx->b_region.as<uint8_t>() + sizeof(snfb_region) * ctx->n_region) : nullptr; }
+
 int snfb_load_records(snfb_ctx* ctx, const snfb_records* R) {
     if (!ctx || !R) return 1;
     cudaSetDevice(ctx->device);
     ctx->loaded = false; ctx->stage_a_done = ctx->stage_b_done = ctx->stage_c_done = false; ctx->force_no_cuts = false;
+    take_regions(ctx);
     if (R->n_task == 0 || R->n_task > 65535) return fail(ctx, "n_task must be in 1..65535");
     if (R->n_rec >= (1ull << 28)) return fail(ctx, "too many records in one block (2^28)");
     if (!R->task || (R->n_rec && (!R->rec || !R->cigar))) return fail(ctx, "null table in the record block");
     if (check_tables(ctx, R)) return 1;
+    if (ctx->n_region && R->on_device != SNFB_MEM_DEVICE)           // device-resident records are checked by k_rec_index (bad_records)
+        for (uint64_t i = 0; i < R->n_rec; ++i) {
+            const uint32_t g = R->rec[i].region;
+            if (g >= ctx->n_region || ctx->regions[g].task != R->rec[i].task)
+                return fail(ctx, "record " + std::to_string(i) + " (task " + std::to_string(R->rec[i].task) + "): region " + std::to_string(g) + " is not a region of its task");
+        }
     ctx->n_rec = R->n_rec; ctx->n_cigar = R->n_cigar; ctx->n_var = R->n_var; ctx->n_seq = R->n_seq;
     ctx->n_task = R->n_task; ctx->n_contig = R->n_contig; ctx->n_tr = R->n_tr; ctx->on_device = R->on_device == SNFB_MEM_DEVICE; ctx->seq_on_demand = R->on_device == SNFB_MEM_HOST_SEQ_ON_DEMAND; ctx->h_seq = ctx->seq_on_demand ? R->seq : nullptr;
     ctx->n_ev = 0;
@@ -534,6 +594,7 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
     if (!ctx || !in) return 1;
     cudaSetDevice(ctx->device);
     ctx->loaded = false; ctx->from_bam = false; ctx->stage_a_done = ctx->stage_b_done = ctx->stage_c_done = false; ctx->force_no_cuts = false;
+    take_regions(ctx);
     if (in->n_task == 0 || in->n_task > 65535) return fail(ctx, "n_task must be in 1..65535");
     if (!in->task || (in->n_bytes && !in->bgzf) || (in->n_span && !in->span)) return fail(ctx, "null table in the BAM input");
     snfb_records T; memset(&T, 0, sizeof(T));
@@ -558,9 +619,13 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
         };
         uint64_t ub = 0, ue = 0;
         if (!resolve(sp.cbeg, sp.ubeg, &ub) || !resolve(sp.cend, sp.uend, &ue) || ue < ub) return fail(ctx, "span: a virtual offset does not name a BGZF block of the buffer");
+        const uint32_t rg = ctx->n_region ? sp.region : 0u;
+        if (ctx->n_region && (rg >= ctx->n_region || (uint32_t)ctx->regions[rg].task != sp.task))
+            return fail(ctx, "span " + std::to_string(i) + " (task " + std::to_string(sp.task) + "): region " + std::to_string(rg) + " is not a region of its task");
         if (i && spans[i - 1].task > sp.task) return fail(ctx, "spans must be listed task by task");
-        if (i && spans[i - 1].task == sp.task && spans[i - 1].uend > ub) return fail(ctx, "spans of a task must be in file order and must not overlap");
-        spans[i].ubeg = ub; spans[i].uend = ue; spans[i].task = sp.task; spans[i]._pad = 0;
+        if (i && spans[i - 1].task == sp.task && spans[i - 1].region > rg) return fail(ctx, "spans of a task must be listed region by region");
+        if (i && spans[i - 1].task == sp.task && spans[i - 1].region == rg && spans[i - 1].uend > ub) return fail(ctx, "spans of a region must be in file order and must not overlap");
+        spans[i].ubeg = ub; spans[i].uend = ue; spans[i].task = sp.task; spans[i].region = rg;
     }
     if (upload_tables(ctx, &T)) return 1;
     // counters, block and span tables
@@ -576,7 +641,7 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
     if (nb) launch_inflate(ctx, d_blk, (unsigned)nb, d_ctr);
     mark(ctx, "walk_records", 0);
     if (ns) {
-        launch(ctx->launches, ingest::k_walk, (unsigned)((ns + 127) / 128), 128, 0, st, raw, raw_len, d_span, (unsigned)ns, 0, span_cnt, nullptr, nullptr, 0, d_ctr);
+        launch(ctx->launches, ingest::k_walk, (unsigned)((ns + 127) / 128), 128, 0, st, raw, raw_len, d_span, (unsigned)ns, 0, span_cnt, nullptr, nullptr, nullptr, 0, d_ctr);
         prims::exclusive_scan(ctx->launches, span_cnt, span_base, scan_tmp0, nullptr, ns, &d_ctr->n_raw, st);
     }
     if (ctx->h_ing.ensure(2 * sizeof(ingest::IngestCounters))) return fail(ctx, "out of pinned memory");
@@ -588,19 +653,19 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
     const uint64_t n_raw = hc->n_raw;
     if (n_raw >= (1ull << 28)) return fail(ctx, "too many records in one block (2^28)");
     // per-raw-record work arrays
-    ingest::RawRec* recs = nullptr; uint32_t *keep = nullptr, *idx = nullptr, *groups = nullptr, *grp_off = nullptr, *var16 = nullptr, *var_off = nullptr, *seq16 = nullptr, *seq_off = nullptr, *scan_tmp = nullptr;
-    if (carve(ctx->b_ing_work, [&](Carver& c) { recs = c.take<ingest::RawRec>(n_raw + 1); keep = c.take<uint32_t>(n_raw + 1); idx = c.take<uint32_t>(n_raw + 1); groups = c.take<uint32_t>(n_raw + 1); grp_off = c.take<uint32_t>(n_raw + 1);
+    ingest::RawRec* recs = nullptr; uint32_t *raw_region = nullptr, *keep = nullptr, *idx = nullptr, *groups = nullptr, *grp_off = nullptr, *var16 = nullptr, *var_off = nullptr, *seq16 = nullptr, *seq_off = nullptr, *scan_tmp = nullptr;
+    if (carve(ctx->b_ing_work, [&](Carver& c) { recs = c.take<ingest::RawRec>(n_raw + 1); raw_region = c.take<uint32_t>(n_raw + 1); keep = c.take<uint32_t>(n_raw + 1); idx = c.take<uint32_t>(n_raw + 1); groups = c.take<uint32_t>(n_raw + 1); grp_off = c.take<uint32_t>(n_raw + 1);
                                                 var16 = c.take<uint32_t>(n_raw + 1); var_off = c.take<uint32_t>(n_raw + 1); seq16 = c.take<uint32_t>(n_raw + 1); seq_off = c.take<uint32_t>(n_raw + 1); scan_tmp = c.take<uint32_t>(prims::scan_tmp_elems(n_raw + 1) + 16); }))
         return fail(ctx, "out of device memory (ingest work arrays)");
     const uint32_t evt = evt_need(ctx);
     uint64_t n_rec = 0, n_groups = 0, n_var16 = 0, n_seq16 = 0;
     if (n_raw) {
         const unsigned warp_grid = (unsigned)std::min<uint64_t>((n_raw + 7) / 8, (uint64_t)NUM_SMS * 16);
-        launch(ctx->launches, ingest::k_walk, (unsigned)((ns + 127) / 128), 128, 0, st, raw, raw_len, d_span, (unsigned)ns, 1, span_cnt, span_base, recs, n_raw, d_ctr);
+        launch(ctx->launches, ingest::k_walk, (unsigned)((ns + 127) / 128), 128, 0, st, raw, raw_len, d_span, (unsigned)ns, 1, span_cnt, span_base, recs, raw_region, n_raw, d_ctr);
         mark(ctx, "parse_records", 0);
-        launch(ctx->launches, ingest::k_parse, (unsigned)((n_raw + 127) / 128), 128, 0, st, raw, recs, (unsigned)n_raw, ctx->b_task.as<snfb_task>(), d_ctr);
+        launch(ctx->launches, ingest::k_parse, (unsigned)((n_raw + 127) / 128), 128, 0, st, raw, recs, raw_region, (unsigned)n_raw, ctx->b_task.as<snfb_task>(), dev_regions(ctx), d_ctr);
         mark(ctx, "record_sizes", 0);
-        launch(ctx->launches, ingest::k_rec_sizes, warp_grid, 256, 0, st, raw, recs, (unsigned)n_raw, ctx->b_task.as<snfb_task>(), evt, keep, groups, var16, seq16, d_ctr);
+        launch(ctx->launches, ingest::k_rec_sizes, warp_grid, 256, 0, st, raw, recs, raw_region, (unsigned)n_raw, ctx->b_task.as<snfb_task>(), dev_regions(ctx), evt, keep, groups, var16, seq16, d_ctr);
         prims::exclusive_scan(ctx->launches, keep, idx, scan_tmp, nullptr, n_raw, &d_ctr->n_keep, st);
         prims::exclusive_scan(ctx->launches, groups, grp_off, scan_tmp, nullptr, n_raw, &d_ctr->n_groups, st);
         prims::exclusive_scan(ctx->launches, var16, var_off, scan_tmp, nullptr, n_raw, &d_ctr->n_var, st);
@@ -617,7 +682,7 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
     CUDA_TRY(cudaMemsetAsync(ctx->b_cigar.as<uint16_t>() + 8 * n_groups, 0, 2 * 24, st));
     if (n_raw) {
         const unsigned warp_grid = (unsigned)std::min<uint64_t>((n_raw + 7) / 8, (uint64_t)NUM_SMS * 16);
-        launch(ctx->launches, ingest::k_pack, warp_grid, 256, 0, st, raw, recs, (unsigned)n_raw, evt, keep, idx, grp_off, groups, var_off, seq_off, ctx->b_rec.as<snfb_rec>(), ctx->b_cigar.as<uint16_t>(), ctx->b_var.as<uint8_t>(), ctx->b_seq.as<uint8_t>());
+        launch(ctx->launches, ingest::k_pack, warp_grid, 256, 0, st, raw, recs, raw_region, (unsigned)n_raw, evt, keep, idx, grp_off, groups, var_off, seq_off, ctx->b_rec.as<snfb_rec>(), ctx->b_cigar.as<uint16_t>(), ctx->b_var.as<uint8_t>(), ctx->b_seq.as<uint8_t>());
     }
     mark(ctx, nullptr);
     ctx->n_ev_load = ctx->n_ev;
@@ -656,6 +721,11 @@ static void carve_r(snfb_ctx* ctx, Carver& c) {
     ctx->nm_part = c.take<double>(cpt * nt + 1); ctx->nm_cnt = c.take<unsigned>(cpt * nt + 1);
     ctx->sa_seg = c.take<extract::Seg>((size_t)extract::MAXSEG * extract::SA_THREADS * extract::SA_BLOCKS);
     ctx->scan_tmp_r = c.take<uint32_t>(prims::scan_tmp_elems(n) + 16);
+    const size_t nv = ctx->cov_view ? n : 1;
+    ctx->v_pos = c.take<int32_t>(nv); ctx->v_end = c.take<int32_t>(nv); ctx->v_flags = c.take<uint8_t>(nv);
+    ctx->v_k0 = c.take<uint64_t>(nv); ctx->v_k1 = c.take<uint64_t>(nv); ctx->v_v0 = c.take<uint32_t>(nv); ctx->v_v1 = c.take<uint32_t>(nv);
+    ctx->v_hist = c.take<uint32_t>(prims::radix_hist_elems(nv) + 16); ctx->v_scan = c.take<uint32_t>(prims::scan_tmp_elems(std::max<size_t>(nv, prims::radix_hist_elems(nv))) + 16);
+    ctx->v_n = c.take<unsigned long long>(1);
 }
 static void carve_l(snfb_ctx* ctx, Carver& c) {
     const size_t n = (size_t)ctx->cap.lead + 8; cluster::B& b = ctx->B;
@@ -696,7 +766,8 @@ static void bind_inputs(snfb_ctx* ctx) {
     cluster::B& b = ctx->B;
     b.leads = ctx->leads; b.rec = ctx->d_rec; b.task = ctx->b_task.as<snfb_task>(); b.contig = ctx->b_contig.as<snfb_contig>();
     b.tr = ctx->n_tr ? ctx->b_tr.as<int32_t>() : nullptr; b.tr_pmax = ctx->b_trp.as<int32_t>();
-    b.rec_pos = ctx->rec_pos; b.rec_end = ctx->rec_end; b.rec_flags = ctx->rec_flags; b.rec_nm = ctx->rec_nm; b.rec_nlead = ctx->rec_nlead; b.rec_lead_off = ctx->rec_lead_off;
+    // the coverage readers binary-search these: block order, or the coordinate-ordered copy stage A builds when block order is not
+    b.rec_pos = ctx->cov_view ? ctx->v_pos : ctx->rec_pos; b.rec_end = ctx->cov_view ? ctx->v_end : ctx->rec_end; b.rec_flags = ctx->cov_view ? ctx->v_flags : ctx->rec_flags; b.rec_nm = ctx->rec_nm; b.rec_nlead = ctx->rec_nlead; b.rec_lead_off = ctx->rec_lead_off;
     b.task_first = ctx->task_first; b.task_last = ctx->task_last; b.task_maxspan = ctx->task_span;
     b.mask = ctx->n_mask ? ctx->b_mask.as<int32_t>() : nullptr; b.mask_task_off = ctx->n_mask ? ctx->b_mask_off.as<uint32_t>() : nullptr;
     b.n_task = ctx->n_task; b.n_bound = ctx->cap.lead; b.ctr = ctx->b_ctr.as<DevCounters>(); b.cfg = ctx->cfg;
@@ -717,7 +788,7 @@ static int enqueue_stage_a(snfb_ctx* ctx) {
     CUDA_TRY(cudaMemsetAsync(ctx->task_nm, 0, 8 * nt, st));
     extract::WalkParams S{};
     S.scan = ctx->scanrec; S.n_rec = (uint32_t)nrec; S.cigar = ctx->d_cigar; S.task = b.task;
-    S.rec_end = ctx->rec_end; S.rec_nlead = ctx->rec_nlead; S.rec_big = ctx->rec_big;
+    S.rec_end = ctx->rec_end; S.rec_nlead = ctx->rec_nlead; S.rec_big = ctx->rec_big; S.rec = ctx->d_rec; S.region = dev_regions(ctx);
     S.ev = ctx->ev_buf; S.ev_cap = ctx->cap.lead; S.n_ev = &ctr->n_ev; S.ctr = ctr; S.minsv = cf.minsvlen_screen;
     if (evt_need(ctx) < ctx->evt_min) {
         // the block's E bits were set for longer events than this configuration looks at: lower the threshold in place
@@ -732,7 +803,7 @@ static int enqueue_stage_a(snfb_ctx* ctx) {
         I.scan = ctx->scanrec; I.clip = ctx->clip; I.rec_end = ctx->rec_end; I.rec_flags = ctx->rec_flags; I.rec_nm = ctx->rec_nm; I.rec_nlead = ctx->rec_nlead; I.ctr = ctr;
         I.mapq_min = cf.mapq; I.alen_min = cf.min_alignment_length; I.excl = cf.exclude_flags; I.want_nm = (cf.qc_nm_measure || cf.phase) ? 1 : 0;
         I.n_cigar = ctx->n_cigar; I.n_var = ctx->n_var; I.n_seq = ctx->n_seq; I.check_seq = ctx->seq_on_demand ? 0 : 1;
-        I.sa_list = ctx->sa_list; I.n_sa = &ctr->n_sa;
+        I.sa_list = ctx->sa_list; I.n_sa = &ctr->n_sa; I.region = dev_regions(ctx); I.last_region = dev_last_region(ctx); I.n_region = ctx->n_region;
         launch(ctx->launches, extract::k_rec_index, (unsigned)((nrec + 255) / 256), 256, 0, st, I);
         // the CIGAR walk: bytes = the CIGAR16 arena (bench.py counts the passing records' groups)
         mark(ctx, "k_scan", 2 * ctx->n_cigar);
@@ -751,12 +822,22 @@ static int enqueue_stage_a(snfb_ctx* ctx) {
         mark(ctx, "k_sa");
         extract::SaParams A{};
         A.rec = ctx->d_rec; A.clip = ctx->clip; A.var = ctx->d_var; A.task = b.task; A.contig = b.contig; A.n_contig = ctx->n_contig;
-        A.sa_list = ctx->sa_list; A.n_sa = &ctr->n_sa; A.rec_end = ctx->rec_end; A.rec_nlead = ctx->rec_nlead; A.leads = E.leads; A.lead_cap = ctx->cap.lead; A.ctr = ctr; A.cfg = cf; A.seg_scratch = ctx->sa_seg;
+        A.sa_list = ctx->sa_list; A.n_sa = &ctr->n_sa; A.rec_end = ctx->rec_end; A.rec_nlead = ctx->rec_nlead; A.leads = E.leads; A.lead_cap = ctx->cap.lead; A.ctr = ctr; A.cfg = cf; A.seg_scratch = ctx->sa_seg; A.region = dev_regions(ctx);
         launch(ctx->launches, extract::k_sa, extract::SA_BLOCKS, extract::SA_THREADS, 0, st, A);
         mark(ctx, "k_task_nm");
         const int cpt = (int)((nrec + extract::NM_CHUNK - 1) / extract::NM_CHUNK);
         launch(ctx->launches, extract::k_nm_partial, dim3(cpt, nt), 256, 0, st, ctx->rec_flags, ctx->rec_nm, ctx->task_first, ctx->task_last, ctx->nm_part, ctx->nm_cnt);
         launch(ctx->launches, extract::k_task_nm, nt, 256, 0, st, ctx->task_first, ctx->task_last, ctx->nm_part, ctx->nm_cnt, cpt, ctx->task_nm);
+        if (ctx->cov_view) {
+            // records grouped by region are out of coordinate order inside a task: a stable sort of (task, pos) gives the order the
+            // coverage readers binary-search (duplicates of a read stay adjacent, each counted)
+            mark(ctx, "cov_order");
+            launch(ctx->launches, k_view_keys, grid_for(nrec, 256), 256, 0, st, ctx->d_rec, ctx->rec_pos, (unsigned long long)nrec, ctx->v_k0, ctx->v_v0, ctx->v_n);
+            prims::RadixTemp vt{ ctx->v_hist, ctx->v_scan };
+            bool vfirst = true;
+            prims::radix_sort(ctx->launches, ctx->v_k0, ctx->v_v0, ctx->v_k1, ctx->v_v1, vt, ctx->v_n, nrec, 32 + bits_for(nt), &vfirst, st);
+            launch(ctx->launches, k_view_gather, grid_for(nrec, 256), 256, 0, st, vfirst ? ctx->v_v0 : ctx->v_v1, (unsigned long long)nrec, ctx->rec_pos, ctx->rec_end, ctx->rec_flags, ctx->v_pos, ctx->v_end, ctx->v_flags);
+        }
     }
     mark(ctx, "scan_rec_leads");
     prims::exclusive_scan(ctx->launches, ctx->rec_nlead, ctx->rec_lead_off, ctx->scan_tmp_r, nullptr, nrec, &ctr->n_leads, st);

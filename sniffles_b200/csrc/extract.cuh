@@ -19,6 +19,13 @@ constexpr int MAXSEG = 40;     // primary + supplementary segments per read held
 
 // rec_flags bits
 constexpr uint8_t RF_PASS = 1, RF_HAS_NM = 2;   // bits 2..3: hp
+constexpr uint8_t RF_NM_MEAN = 16;              // the read's nm enters config.average_regional_nm: it has one and belongs to its task's last region
+
+// the fetch window a record was read for: its region with a region table (snfb_set_regions, leadprov.py:445-470), else its task's
+__device__ __forceinline__ int2 rec_window(const snfb_region* region, const snfb_task* task, const snfb_rec* rec, uint32_t i, int t) {
+    if (region) { const snfb_region g = region[__ldg(&rec[i].region)]; return make_int2(g.start, g.end); }
+    return make_int2(task[t].start, task[t].end);
+}
 
 struct Seg {
     int contig, ref_start, ref_end, qry_start, qry_end;
@@ -283,6 +290,7 @@ struct IndexParams {
     RecScan* scan; RecClip* clip; int32_t* rec_end; uint8_t* rec_flags; double* rec_nm; uint32_t* rec_nlead;
     uint32_t* sa_list; unsigned long long* n_sa;     // passing records with an SA tag (k_sa's work list)
     DevCounters* ctr; int mapq_min, alen_min, excl, want_nm;
+    const snfb_region* region; const int32_t* last_region; uint32_t n_region;      // region table (null: none) and each task's last region
 };
 
 // the clip ops at the two ends of a CIGAR16 record of n words, word(k) = word k: query_alignment_start / end (qas, qae, starting from
@@ -332,7 +340,8 @@ __device__ __forceinline__ bool index_record(const IndexParams& P, uint32_t i) {
     const int nm = (int)c1.x; const uint32_t n = c1.z; const int l_seq = (int)c1.w; const uint32_t sa_len = c2.x;
     const unsigned long long cigar_off = (unsigned long long)c2.z | ((unsigned long long)c2.w << 32);
     const unsigned long long seq_off = (unsigned long long)c3.x | ((unsigned long long)c3.y << 32), var_off = (unsigned long long)c3.z | ((unsigned long long)c3.w << 32);
-    const bool bad_core = (uint32_t)task >= P.n_task || (cigar_off & 7) || cigar_off + n > P.n_cigar;
+    const uint32_t rg = c2.y;
+    const bool bad_core = (uint32_t)task >= P.n_task || (cigar_off & 7) || cigar_off + n > P.n_cigar || (P.region && (rg >= P.n_region || P.region[rg].task != task));
     const bool bad = bad_core || var_off + l_qname + sa_len > P.n_var || l_seq < 0
                      || (P.check_seq && seq_off + (unsigned long long)((l_seq + 1) / 2) > P.n_seq);
     if (bad) atomicAdd(&P.ctr->bad_records, 1ULL);
@@ -343,7 +352,11 @@ __device__ __forceinline__ bool index_record(const IndexParams& P, uint32_t i) {
     }
     P.rec_pos[i] = pos;
     if (i == 0) P.task_first[task] = 0;
-    else { const int2 pv = __ldg(reinterpret_cast<const int2*>(P.rec + i - 1)); if (pv.x != task) { P.task_first[task] = i; if ((uint32_t)pv.x < P.n_task) P.task_last[pv.x] = i; } else if (pv.y > pos) atomicAdd(&P.ctr->unsorted, 1ULL); }
+    else {
+        const int2 pv = __ldg(reinterpret_cast<const int2*>(P.rec + i - 1));
+        if (pv.x != task) { P.task_first[task] = i; if ((uint32_t)pv.x < P.n_task) P.task_last[pv.x] = i; }
+        else if (pv.y > pos && (!P.region || __ldg(&P.rec[i - 1].region) == rg)) atomicAdd(&P.ctr->unsorted, 1ULL);     // sorted inside a region segment
+    }
     if (i + 1 == P.n_rec) P.task_last[task] = P.n_rec;
     // clips at the two ends: from the first and the last group (two independent loads), word by word only when the clips leave them
     const uint16_t* cg = P.cigar + cigar_off;
@@ -357,8 +370,8 @@ __device__ __forceinline__ bool index_record(const IndexParams& P, uint32_t i) {
     }
     if (miss) { qas = 0; qae = l_seq; clip_left = 0; clip_right = 0; clip_walk(n, [&](uint32_t k) { return (unsigned)__ldg(cg + k); }, qas, qae, clip_left, clip_right); }
     const int alen = qae - qas;
-    const snfb_task tk = P.task[task];
-    const bool pass = !((int)mapq < P.mapq_min || (flag & 256u) || alen < P.alen_min) && !(P.excl && (flag & (unsigned)P.excl)) && pos >= tk.start && pos < tk.end && n > 0;
+    const int2 win = P.region ? make_int2(P.region[rg].start, P.region[rg].end) : make_int2(P.task[task].start, P.task[task].end);
+    const bool pass = !((int)mapq < P.mapq_min || (flag & 256u) || alen < P.alen_min) && !(P.excl && (flag & (unsigned)P.excl)) && pos >= win.x && pos < win.y && n > 0;
     const bool has_nm = pass && P.want_nm && (aux & SNFB_AUX_NM);
     if (!(aux & SNFB_AUX_HP)) hp = 0;
     if (pass && hp > 2) { hp = 0; atomicAdd(&P.ctr->soft_errors, 1ULL); }
@@ -367,7 +380,8 @@ __device__ __forceinline__ bool index_record(const IndexParams& P, uint32_t i) {
     store16(P.scan + i, s);
     RecClip c; c.alen = alen; c.qas = qas; c.clip_left = clip_left; c.clip_right = clip_right;
     store16(P.clip + i, c);
-    P.rec_flags[i] = pass ? (uint8_t)(RF_PASS | (has_nm ? RF_HAS_NM : 0) | (hp << 2)) : (uint8_t)0;
+    const bool nm_mean = has_nm && (!P.region || P.last_region[task] == (int)rg);     // nm_sum is reset per region (leadprov.py:475-577)
+    P.rec_flags[i] = pass ? (uint8_t)(RF_PASS | (has_nm ? RF_HAS_NM : 0) | (hp << 2) | (nm_mean ? RF_NM_MEAN : 0)) : (uint8_t)0;
     P.rec_nm[i] = has_nm ? (double)nm : -1.0;        // k_rec_post turns it into (nm - big) / (alen + 1)
     P.rec_end[i] = -1; P.rec_nlead[i] = 0;       // k_cigar_walk overwrites both for a passing record
     return pass && (aux & SNFB_AUX_SA);
@@ -410,6 +424,7 @@ struct Event { uint32_t rec; uint32_t len; uint32_t pos_q; int32_t pos_r; uint32
 struct WalkParams {
     const RecScan* scan; uint32_t n_rec;
     const uint16_t* cigar; const snfb_task* task;
+    const snfb_rec* rec; const snfb_region* region;          // region table (null: none): a lead's window is its record's region
     int32_t* rec_end; uint32_t* rec_nlead; int32_t* rec_big;
     Event* ev; unsigned long long ev_cap; unsigned long long* n_ev;      // n_ev: event slots handed out, holes included
     DevCounters* ctr;
@@ -588,8 +603,8 @@ __global__ void __launch_bounds__(WALK_THREADS, 4) k_cigar_walk(const __grid_con
                 const uint32_t f_rec = t0 + (uint32_t)o_j;
                 int tk_start = 0, tk_end = 0; uint32_t n = 0, big = 0;
                 if (gv && (((v.x | v.y | v.z | v.w) & 0x40004000u) != 0)) {      // count the group's signatures
-                    const snfb_task& tk = P.task[rs[o_j].w & 0xffffu];
-                    tk_start = tk.start; tk_end = tk.end;
+                    const int2 win = rec_window(P.region, P.task, P.rec, f_rec, (int)(rs[o_j].w & 0xffffu));
+                    tk_start = win.x; tk_end = win.y;
                     group_events(v, q, (int)r, P.minsv, tk_start, tk_end, big, [&](unsigned, unsigned, uint32_t, int) { ++n; });
                 }
                 const uint32_t n_incl = prims::warp_incl_scan(n), n_ex = n_incl - n, n_tot = __shfl_sync(FULL, n_incl, 31);
@@ -731,6 +746,7 @@ struct SaParams {
     snfb_lead* leads; unsigned long long lead_cap; DevCounters* ctr;
     Seg* seg_scratch;                 // MAXSEG segments per thread of the grid
     snfb_config cfg;
+    const snfb_region* region;        // region table (null: none)
 };
 constexpr int SA_THREADS = 128, SA_BLOCKS = NUM_SMS * 8;
 // one thread per record with an SA tag: the text parse is serial per record, so the parallelism is across records.
@@ -758,7 +774,7 @@ __global__ void __launch_bounds__(SA_THREADS) k_sa(const SaParams P) {
         SaArgs a; a.rec = rec; a.qas = rc.qas; a.qae = rc.qas + rc.alen; a.alen = rc.alen; a.ref_end = P.rec_end[rec]; a.hp = hp;
         a.base_flags = (rev ? SNFB_LF_REVERSE : 0u) | (mapq << 16); a.qh = qname_hash_thread(P.var + var_off, l_qname); a.nlead = P.rec_nlead[rec]; a.rev = rev; a.is_supp = flag & 2048u;
         a.sa = P.var + var_off + l_qname; a.sa_len = (int)sa_len; a.clip_left = rc.clip_left; a.clip_right = rc.clip_right; a.pos = r_pos; a.l_seq = l_seq; a.mapq = (int)mapq;
-        a.aux_flags = (int)aux; a.task = r_task; a.tk_contig = tk.contig; a.tk_start = tk.start; a.tk_end = tk.end; a.contig = P.contig; a.n_contig = P.n_contig;
+        a.aux_flags = (int)aux; a.task = r_task; a.tk_contig = tk.contig; const int2 win = rec_window(P.region, P.task, P.rec, rec, r_task); a.tk_start = win.x; a.tk_end = win.y; a.contig = P.contig; a.n_contig = P.n_contig;
         a.leads = P.leads; a.lead_cap = P.lead_cap; a.n_slots = &P.ctr->n_slots; a.slots = &slots;
         a.mapq_min = s_cfg.mapq; a.dev_keep_lowqual_splits = s_cfg.dev_keep_lowqual_splits; a.max_splits_base = s_cfg.max_splits_base; a.max_splits_kb = s_cfg.max_splits_kb;
         const unsigned added = process_sa(&s_cfg, sg, a, &soft, &overflow);
@@ -780,7 +796,7 @@ __global__ void __launch_bounds__(256) k_nm_partial(const uint8_t* __restrict__ 
     if (lo >= end) return;                                  // whole block exits together
     const uint32_t hi = lo + NM_CHUNK < end ? lo + NM_CHUNK : end;
     double s = 0; unsigned c = 0;
-    for (uint32_t i = lo + threadIdx.x; i < hi; i += 256) if ((rec_flags[i] & (RF_PASS | RF_HAS_NM)) == (RF_PASS | RF_HAS_NM)) { s += rec_nm[i]; ++c; }
+    for (uint32_t i = lo + threadIdx.x; i < hi; i += 256) if (rec_flags[i] & RF_NM_MEAN) { s += rec_nm[i]; ++c; }
     ssum[threadIdx.x] = s; scnt[threadIdx.x] = c; __syncthreads();
     for (int o = 128; o; o >>= 1) { if (threadIdx.x < o) { ssum[threadIdx.x] += ssum[threadIdx.x + o]; scnt[threadIdx.x] += scnt[threadIdx.x + o]; } __syncthreads(); }
     if (threadIdx.x == 0) { part_sum[(size_t)t * gridDim.x + blockIdx.x] = ssum[0]; part_cnt[(size_t)t * gridDim.x + blockIdx.x] = scnt[0]; }

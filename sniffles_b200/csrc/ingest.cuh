@@ -21,7 +21,7 @@ namespace ingest {
 
 // DEFLATE payload in the compressed buffer, its inflated size and CRC-32 (the block's gzip trailer), where it lands
 struct BgzfBlock { unsigned long long in_off; unsigned in_len; unsigned isize; unsigned long long out_off; unsigned crc; unsigned _pad; };
-struct Span { unsigned long long ubeg, uend; unsigned task; unsigned _pad; };                                      // record-aligned range of the inflated stream owned by one task
+struct Span { unsigned long long ubeg, uend; unsigned task; unsigned region; };                                   // record-aligned range of the inflated stream owned by one task (and region)
 // first_bad_inv = ~(block << 8 | INF_* code) of the lowest failing block: an atomicMax of the complement, so the zeroed counters need no
 // other initial value and the block reported does not depend on which group failed first
 struct IngestCounters { unsigned long long bad_blocks, first_bad_inv, bad_chain, malformed, bad_cigar, n_raw, n_keep, n_groups, n_var, n_seq16; };
@@ -56,35 +56,43 @@ __global__ void __launch_bounds__(INF_WARPS * 32) k_inflate(const uint8_t* __res
     }
 }
 
-// mode 0: span_cnt[s] = records in the span; mode 1: rec_body[base[s] + k] / rec_bs / rec_task
+// the fetch window of a raw record: its region with a region table (snfb_set_regions), else its task's
+__device__ __forceinline__ int2 fetch_window(const snfb_task* task, const snfb_region* region, unsigned t, const uint32_t* raw_region, unsigned i) {
+    if (region) { const snfb_region g = region[raw_region[i]]; return make_int2(g.start, g.end); }
+    return make_int2(task[t].start, task[t].end);
+}
+
+// mode 0: span_cnt[s] = records in the span; mode 1: rec_body[base[s] + k] / rec_bs / rec_task, and the span's region
 __global__ void k_walk(const uint8_t* __restrict__ raw, unsigned long long raw_len, const Span* __restrict__ spans, unsigned n_spans, int mode,
-                       uint32_t* __restrict__ span_cnt, const uint32_t* __restrict__ span_base, RawRec* __restrict__ recs, unsigned long long rec_cap, IngestCounters* ctr) {
+                       uint32_t* __restrict__ span_cnt, const uint32_t* __restrict__ span_base, RawRec* __restrict__ recs, uint32_t* __restrict__ raw_region, unsigned long long rec_cap, IngestCounters* ctr) {
     const unsigned s = blockIdx.x * blockDim.x + threadIdx.x; if (s >= n_spans) return;
     const Span sp = spans[s];
     unsigned long long off = sp.ubeg; uint32_t n = 0; const uint32_t base = mode ? span_base[s] : 0u;
     while (off + 4 <= sp.uend && off + 4 <= raw_len) {
         const uint32_t bs = ld32u(raw, off);
         if (bs < 32u || off + 4ull + bs > raw_len) { if (!mode) atomicAdd(&ctr->bad_chain, 1ULL); break; }
-        if (mode && (unsigned long long)base + n < rec_cap) { RawRec& r = recs[base + n]; r.body = off + 4; r.body_len = bs; r.task = sp.task; }
+        if (mode && (unsigned long long)base + n < rec_cap) { RawRec& r = recs[base + n]; r.body = off + 4; r.body_len = bs; r.task = sp.task; raw_region[base + n] = sp.region; }
         ++n; off += 4ull + bs;
     }
     if (!mode) { if (off != sp.uend && off + 4 <= raw_len) atomicAdd(&ctr->bad_chain, 1ULL); span_cnt[s] = n; }      // a span must end on a record boundary
 }
 
-__global__ void k_parse(const uint8_t* __restrict__ raw, RawRec* __restrict__ recs, unsigned n_raw, const snfb_task* __restrict__ task, IngestCounters* ctr) {
+__global__ void k_parse(const uint8_t* __restrict__ raw, RawRec* __restrict__ recs, const uint32_t* __restrict__ raw_region, unsigned n_raw, const snfb_task* __restrict__ task,
+                        const snfb_region* __restrict__ region, IngestCounters* ctr) {
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x; if (i >= n_raw) return;
     const unsigned long long body = recs[i].body; const uint32_t bs = recs[i].body_len; const unsigned t = recs[i].task;
     RawRec r; parse_record(raw, body, bs, &r); r.task = t;
     if (r.status == ST_MALFORMED) atomicAdd(&ctr->malformed, 1ULL);
     else {
         const snfb_task k = task[t];
-        if (r.ref_id != k.contig || r.pos >= k.end) r.status = ST_FILTERED;      // bam.fetch(contig, start, end): the overlap test on the start side needs the CIGAR (k_rec_sizes)
+        if (r.ref_id != k.contig || r.pos >= fetch_window(task, region, t, raw_region, i).y) r.status = ST_FILTERED;      // bam.fetch(contig, start, end): the overlap test on the start side needs the CIGAR (k_rec_sizes)
     }
     recs[i] = r;
 }
 
 // warp per raw record
-__global__ void __launch_bounds__(256) k_rec_sizes(const uint8_t* __restrict__ raw, RawRec* __restrict__ recs, unsigned n_raw, const snfb_task* __restrict__ task, uint32_t evt_min,
+__global__ void __launch_bounds__(256) k_rec_sizes(const uint8_t* __restrict__ raw, RawRec* __restrict__ recs, const uint32_t* __restrict__ raw_region, unsigned n_raw, const snfb_task* __restrict__ task,
+                                                   const snfb_region* __restrict__ region, uint32_t evt_min,
                                                    uint32_t* __restrict__ keep, uint32_t* __restrict__ groups, uint32_t* __restrict__ var16, uint32_t* __restrict__ seq16, IngestCounters* ctr) {
     const int lane = threadIdx.x & 31;
     for (unsigned i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n_raw; i += (gridDim.x * blockDim.x) >> 5) {
@@ -94,7 +102,7 @@ __global__ void __launch_bounds__(256) k_rec_sizes(const uint8_t* __restrict__ r
             long long reflen = 0; int bad = 0;
             const uint32_t words = c16_convert<32>(raw, r.cig_src, r.n_cig, nullptr, evt_min, lane, &reflen, &bad);
             if (bad) { if (lane == 0) { atomicAdd(&ctr->bad_cigar, 1ULL); recs[i].status = ST_MALFORMED; } }
-            else if ((long long)r.pos + (reflen > 1 ? reflen : 1) > (long long)task[r.task].start) {
+            else if ((long long)r.pos + (reflen > 1 ? reflen : 1) > (long long)fetch_window(task, region, r.task, raw_region, i).x) {
                 kp = 1; g = (words + 7u) >> 3; vb = ((uint32_t)r.l_qname + r.sa_len + 15u) >> 4; sq = ((uint32_t)((r.l_seq + 1) / 2) + 15u) >> 4;
             } else if (lane == 0) recs[i].status = ST_FILTERED;
         }
@@ -103,7 +111,7 @@ __global__ void __launch_bounds__(256) k_rec_sizes(const uint8_t* __restrict__ r
 }
 
 // warp per raw record; the four scans gave every kept record its index and its arena offsets
-__global__ void __launch_bounds__(256) k_pack(const uint8_t* __restrict__ raw, const RawRec* __restrict__ recs, unsigned n_raw, uint32_t evt_min,
+__global__ void __launch_bounds__(256) k_pack(const uint8_t* __restrict__ raw, const RawRec* __restrict__ recs, const uint32_t* __restrict__ raw_region, unsigned n_raw, uint32_t evt_min,
                                               const uint32_t* __restrict__ keep, const uint32_t* __restrict__ idx, const uint32_t* __restrict__ grp_off, const uint32_t* __restrict__ groups,
                                               const uint32_t* __restrict__ var_off16, const uint32_t* __restrict__ seq_off16,
                                               snfb_rec* __restrict__ out_rec, uint16_t* __restrict__ out_cigar, uint8_t* __restrict__ out_var, uint8_t* __restrict__ out_seq) {
@@ -129,7 +137,7 @@ __global__ void __launch_bounds__(256) k_pack(const uint8_t* __restrict__ raw, c
         if (lane == 0) {
             snfb_rec o; memset(&o, 0, sizeof(o));
             o.task = (int32_t)r.task; o.pos = r.pos; o.flag = r.flag; o.mapq = r.mapq; o.aux_flags = r.aux_flags; o.hp = r.hp; o.l_qname = r.l_qname; o.nm = r.nm; o.ps = r.ps;
-            o.n_cigar = words; o.l_seq = r.l_seq; o.sa_len = r.sa_len; o.cigar_off = co; o.seq_off = so; o.var_off = vo;
+            o.n_cigar = words; o.l_seq = r.l_seq; o.sa_len = r.sa_len; o.cigar_off = co; o.seq_off = so; o.var_off = vo; o.region = raw_region[i];
             out_rec[idx[i]] = o;
         }
     }

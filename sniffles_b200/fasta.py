@@ -267,12 +267,49 @@ class Reference:
         return self._runs[contig]
 
 
-def mask_block(block, reference):
-    """the N-mask tables of a record block (RecordBlock.set_n_mask) from `reference` for each of its tasks"""
+    def region_runs(self, contig, regions, length):
+        """the runs _mask_N_coverage applies to a task with regions (leadprov.py:432-439): the mask is zero outside the regions and each
+        region's slice mask[start:end] of the contig-long vector (`length` bases) takes fasta.fetch(contig, start, end).  So the runs are
+        clipped to the regions.  One region whose fetch or slice assignment raises (the contig missing from the FASTA, or a fetch that
+        does not fit its slice, numpy broadcasting a single base over it) leaves the whole task unmasked, with the reference's warning."""
+        try:
+            if contig not in self._row:
+                raise KeyError(f"sequence '{contig}' not present")
+            if contig not in self._slot:
+                raise KeyError(f"sequence '{contig}' not loaded on this device")
+            L = int(self._row[contig]["length"])
+            runs = self._runs[contig]
+            keep = []
+            for s, e in regions:
+                n_slice, n_fetch = max(0, min(e, length) - s), max(0, min(e, L) - s)
+                if n_fetch != n_slice and n_fetch != 1:
+                    raise ValueError(f"could not broadcast input array from shape ({n_fetch},) into shape ({n_slice},)")
+                if n_fetch == 1 and n_slice > 1:          # one base broadcast over the slice: all N or none
+                    k = int(np.searchsorted(runs[:, 1], s, side="right")) if len(runs) else 0
+                    if k < len(runs) and runs[k, 0] <= s:
+                        keep.append((s, min(e, length)))
+                    continue
+                keep.extend((max(int(a), s), min(int(b), e, length)) for a, b in runs if a < e and b > s)
+        except (KeyError, ValueError) as e:
+            logging.warning(f"Unable to mask N regions in coverage vector, reference could not be fetched: {e}")
+            return None
+        merged = []
+        for a, b in sorted(x for x in keep if x[1] > x[0]):
+            if merged and a <= merged[-1][1]:
+                merged[-1][1] = max(merged[-1][1], b)
+            else:
+                merged.append([a, b])
+        return np.asarray(merged, dtype=np.int32).reshape(-1, 2)
+
+
+def mask_block(block, reference, regions=None):
+    """the N-mask tables of a record block (RecordBlock.set_n_mask) from `reference` for each of its tasks; regions: {task index: [(start,
+    end), ...]} for the tasks that have regions (Reference.region_runs)"""
     per = {}
     for t, task in enumerate(block.task):
         name = block.contig_names[int(task["contig"])]
-        runs = reference.task_runs(name, int(task["start"]), int(task["end"]))
+        rg = (regions or {}).get(t)
+        runs = reference.task_runs(name, int(task["start"]), int(task["end"])) if rg is None else reference.region_runs(name, rg, int(task["contig_len"]))
         if runs is not None and len(runs):
             per[t] = [(int(a), int(b)) for a, b in runs]
     block.set_n_mask(per)

@@ -225,21 +225,44 @@ def genotype_vcf(config, device=0):
     log.info(f"Opening for reading: {config.genotype_vcf} (read {len(targets)} SVs to be genotyped)")
     path = config.input[0] if isinstance(config.input, (list, tuple)) else config.input
     bam = bamio.BamFile(path)
-    planned = [p for p in plan(bam.contigs, targets, config) if p[4]]        # a task without targets writes nothing
+    planned = []
+    for p in plan(bam.contigs, targets, config):
+        if not p[4]:                                    # a task without targets writes nothing
+            continue
+        tid, name, s, e, _ = p
+        regions = config.regions_by_contig.get(name)
+        try:
+            windows = tasks.fetch_windows(name, s, e, regions)
+        except ValueError as err:                       # the task fails in the reference's worker: its targets are not written
+            log.error(f"Error in worker process while executing GenotypeTask(id={tid}, contig={name}, start={s}, end={e}): {err}")
+            continue
+        planned.append((p, windows if regions else None))
     tr_all = tasks.load_tandem_repeats(config.tandem_repeats, config.tandem_repeat_region_pad) if config.tandem_repeats else {}
     ctx = tasks.device_context(device)
     with vcf.open_output(config, ctx) as handle:
         handle.write(rewrite_header(header, config))
         if not planned:
             return 0
-        tr = {k: [(int(a), int(b)) for a, b in tr_all[name]] for k, (_, name, _, _, _) in enumerate(planned) if name in tr_all}
-        block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[name], s, e, tid) for tid, name, s, e, _ in planned], tandem_repeats=tr or None)
-        tasks.mask_block(block, config, ctx)            # target coverage is N-masked as in GenotypeTask's LeadProvider
+        tr = {k: [(int(a), int(b)) for a, b in tr_all[p[1]]] for k, (p, _) in enumerate(planned) if p[1] in tr_all}
+        # a task with regions: its records carry their region's window, its own bounds only clip the N mask (clipped to the regions here)
+        bounds = [(0, bam.get_reference_length(p[1])) if rg else (p[2], p[3]) for p, rg in planned]
+        block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[p[1]], a, b, p[0]) for (p, _), (a, b) in zip(planned, bounds)], tandem_repeats=tr or None)
+        # target coverage is N-masked as in GenotypeTask's LeadProvider; without regions the call is the one it always was
+        mask_regions = {k: rg for k, (_, rg) in enumerate(planned) if rg}
+        tasks.mask_block(block, config, ctx, mask_regions) if mask_regions else tasks.mask_block(block, config, ctx)
         ctx.set_config(abi.Config.from_sniffles(config))
-        bgzf, spans = bam.device_input([(name, s, e) for _, name, s, e, _ in planned])
+        by_task = [(k, rg or [(p[2], p[3])]) for k, (p, rg) in enumerate(planned)]
+        queries, tags, n = [], [], 0
+        for (k, w), (p, _) in zip(by_task, planned):
+            queries += [(p[1], a, b) for a, b in w]
+            tags += [(k, n + g) for g in range(len(w))]
+            n += len(w)
+        has_regions = any(rg for _, rg in planned)
+        bgzf, spans = bam.device_input(queries, tags=tags)
+        ctx.set_regions(tasks.region_table(by_task) if has_regions else None)
         n_rec = ctx.load_bam(bgzf, spans, block)["n_rec"]
         res = ctx.run(want_leads=True, want_cands=True, want_seqs=True)
         rec_nm = abi.view(res._rec_nm_ptr, "<f8", n_rec).copy() if getattr(res, "_rec_nm_ptr", None) else None
         br = tasks.BlockRun(block, res, tasks.cand_ranges(res.cand, len(block.task)), rec_nm)
-        br.genotype = device_targets(ctx, [(k, p[4]) for k, p in enumerate(planned)], bam.name_to_id, config)
-        return write_tasks(handle, br, [p + (k,) for k, p in enumerate(planned)], config)
+        br.genotype = device_targets(ctx, [(k, p[4]) for k, (p, _) in enumerate(planned)], bam.name_to_id, config)
+        return write_tasks(handle, br, [p + (k,) for k, (p, _) in enumerate(planned)], config)

@@ -134,7 +134,7 @@ class SNFWriter:
             bi = off // self.config.snf_block_size
             for i in range(per_block):
                 k = bi * per_block + i
-                if k < len(coverage_bins):
+                if -len(coverage_bins) <= k < len(coverage_bins):      # numpy indexing: a block before 0 wraps, one out of range is skipped
                     self.blocks[off]["_COVERAGE"][off + i * step] = round(float(coverage_bins[k]))
 
     def write_and_index(self):                       # snf.py:108-120

@@ -38,15 +38,34 @@ def reference_for(ctx, path):
     return _REF[key]
 
 
-def mask_block(block, config, ctx):
+def mask_block(block, config, ctx, regions=None):
     """with config.reference: the block's N-mask tables from the reference loaded on `ctx` (LeadProvider._mask_N_coverage,
-    leadprov.py:420-443), before the block is loaded; without it the block is left as it is"""
+    leadprov.py:420-443), before the block is loaded; without it the block is left as it is.  regions: {task index: [(start, end)]}"""
     if getattr(config, "reference", None):
         ref = reference_for(ctx, config.reference)
         if ref is not None:
             from . import fasta
-            fasta.mask_block(block, ref)
+            fasta.mask_block(block, ref, regions)
     return block
+
+
+def fetch_windows(contig, start, end, regions):
+    """the (start, end) of every bam.fetch a task makes, in order: its regions [(contig, start, end)] as given (LeadProvider.build_leadtab, leadprov.py:445-470),
+    else its own [start, end) (parallel.py:101).  A window pysam's parse_region refuses raises its ValueError (restated, not pinned: start <
+    0, or start > end), which fails the task in the reference's worker."""
+    windows = [(int(r[1]), int(r[2])) for r in regions] if regions else [(int(start), int(end))]
+    for s, e in windows:
+        if s < 0:
+            raise ValueError(f"start out of range ({s})")
+        if s > e:
+            raise ValueError(f"invalid coordinates: start ({s}) > stop ({e})")
+    return windows
+
+
+def region_table(windows_by_task):
+    """abi.REGION_DTYPE rows of [(task index, [(start, end), ...])] in task order, or None when no task has regions"""
+    rows = [(t, s, e, 0) for t, w in windows_by_task for s, e in w]
+    return np.array(rows, dtype=abi.REGION_DTYPE) if windows_by_task else None
 
 
 @dataclass
@@ -181,13 +200,15 @@ class Task:
         from . import bamio
         cidx = bam.name_to_id[self.contig]
         tr = {0: [(int(a), int(b)) for a, b in self.tandem_repeats]} if self.tandem_repeats else None
-        return bamio.pack_records(bam.contigs, list(recs), [(cidx, int(self.start), int(self.end), int(self.id))], tandem_repeats=tr)
+        # with regions the records carry their region's window; the task's own bounds then only clip the N mask, which the host clips
+        s, e = (0, bam.contigs[cidx][1]) if self.regions else (int(self.start), int(self.end))
+        return bamio.pack_records(bam.contigs, list(recs), [(cidx, s, e, int(self.id))], tandem_repeats=tr)
 
-    def _own_block(self):
-        """records of [start, end) from the task's BAM (`self.bam`: an open bamio.BamFile or a path; default config.input), decoded and
-        packed on the HOST (device_ingest=False; also what the tests compare the device ingest with)"""
+    def _own_block(self, windows):
+        """records of every fetch window from the task's BAM (`self.bam`: an open bamio.BamFile or a path; default config.input), region by
+        region, decoded and packed on the HOST (device_ingest=False; also what the tests compare the device ingest with)"""
         bam = self._open()
-        return self._tables(bam, [(0, r) for r in bam.fetch(self.contig, self.start, self.end)])
+        return self._tables(bam, [(0, r, g) for g, (s, e) in enumerate(windows) for r in bam.fetch(self.contig, s, e)])
 
     def _ctx(self):
         return device_context(self.device)
@@ -204,15 +225,19 @@ class Task:
         if self.block_run is None:
             ctx = self._ctx()
             ctx.set_config(abi.Config.from_sniffles(self.config))
+            windows = fetch_windows(self.contig, self.start, self.end, self.regions)
+            regions = {0: windows} if self.regions else None
             if self.device_ingest:
                 # the reference's `bam.fetch(contig, start, end)` (parallel.py:95-98, leadprov.py:488) with htslib's work on the GPU: the host
                 # only resolves the BAI index; BGZF inflate, record decode, region filter and CIGAR16 packing are snfb_load_bam
                 bam = self._open()
-                block = mask_block(self._tables(bam), self.config, ctx)
-                bgzf, spans = bam.device_input([(self.contig, int(self.start), int(self.end))])
+                block = mask_block(self._tables(bam), self.config, ctx, regions)
+                bgzf, spans = bam.device_input([(self.contig, s, e) for s, e in windows], tags=[(0, g) for g in range(len(windows))])
+                ctx.set_regions(region_table([(0, windows)]) if regions else None)
                 n_rec = ctx.load_bam(bgzf, spans, block)["n_rec"]
             else:
-                block = mask_block(self._own_block(), self.config, ctx)
+                block = mask_block(self._own_block(windows), self.config, ctx, regions)
+                ctx.set_regions(region_table([(0, windows)]) if regions else None)
                 ctx.load(block, cigar16=False)                   # BAM words: the library converts them (snfb_load_records)
                 n_rec = len(block.rec)
             res = ctx.extract_leads()                            # snfb_extract_leads
