@@ -1,12 +1,64 @@
 """`python -m sniffles_b200 ARGS`: the reference's command line (sniffles:64-148) for the two run modes that read one BAM -- calling a
 sample (`-i sample.bam -v out.vcf [--snf out.snf]`, call.call_sample) and force calling (`--genotype-vcf`, genotype.genotype_vcf).
-Combine mode (.snf / .tsv input) and CRAM input are not run from here."""
+Combine mode (.snf / .tsv input) and CRAM input are not run from here.
+
+Calling a sample on N GPUs is one process per GPU:
+
+    torchrun --standalone --nproc-per-node N -m sniffles_b200 -i sample.bam -v out.vcf --gpus N
+
+Every rank calls its share of the tasks and rank 0 writes the files, which are those of `--gpus 1`.  Only rank 0 logs the run's INFO
+lines; the other ranks log warnings and errors, prefixed with their rank."""
 import datetime
 import logging
+import os
 import sys
 
 from . import call, genotype
 from .config import SnifflesConfig
+
+# how long a rank waits in a collective: the ranks finish their tasks at different times and wait for the last one in the gather
+RANK_TIMEOUT = datetime.timedelta(hours=12)
+
+
+def _rank_logging(rank):
+    """ranks above 0 log warnings and errors only, each line prefixed with the rank"""
+    if rank == 0:
+        return
+    root = logging.getLogger()
+    root.setLevel(logging.WARNING)
+    for h in root.handlers:
+        fmt = h.formatter._fmt if h.formatter is not None else logging.BASIC_FORMAT
+        h.setFormatter(logging.Formatter(f"rank {rank}: {fmt}"))
+
+
+def _main_ranks(config, world, log):
+    """one rank of a torchrun launch with WORLD_SIZE > 1: every rank reaches the same verdict on the launch, and returns the same code"""
+    import torch
+    rank, local = int(os.environ.get("RANK", 0)), int(os.environ.get("LOCAL_RANK", 0))
+    _rank_logging(rank)
+    local_world, n_dev = int(os.environ.get("LOCAL_WORLD_SIZE", world)), torch.cuda.device_count()
+    refusal = None
+    if config.mode != "call_sample":
+        refusal = f"--genotype-vcf runs on one GPU: run it without torchrun ({world} ranks would each write {config.vcf})"
+    elif config.gpus != world:
+        refusal = f"--gpus {config.gpus} does not match the {world} processes torchrun started (--nproc-per-node)"
+    elif local_world > n_dev:               # LOCAL_RANK < device count on every rank of this node
+        refusal = f"{local_world} processes on this node, but {n_dev} visible GPU(s): run one process per GPU"
+    if refusal is not None:
+        log.error(f"{refusal} (Fatal error, exiting.)")
+        return 1
+    import torch.distributed as tdist
+    torch.cuda.set_device(local)
+    tdist.init_process_group("gloo", timeout=RANK_TIMEOUT)
+    try:
+        call.call_sample(config, device=local)
+        code = 0
+    except call.CallSampleError as e:
+        log.error(f"{e} (Fatal error, exiting.)")
+        code = 1
+    finally:
+        tdist.destroy_process_group()
+    return code
 
 
 def main(argv=None):
@@ -21,6 +73,9 @@ def main(argv=None):
                   f"(supplied were: {sorted(exts)}) (Fatal error, exiting.)")
         return 1
     config.input = config.input[0]
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    if world > 1:
+        return _main_ranks(config, world, log)
     try:
         if config.mode == "genotype_vcf":
             genotype.genotype_vcf(config)

@@ -6,7 +6,8 @@
     BGZF block bamio.BamFile.device_input selects for them) fit a budget.  A pass is one mask_block, one snfb_load_bam and one snfb_run;
     its tasks then run as tasks.CallTask on the pass's BlockRun, and their VCF records and SNF parts are written before the next pass
     loads (host memory stays bounded, and snfb_coverage_bins reads the block loaded on the context);
-  * the VCF goes through vcf.open_output (a .vcf.gz gets BGZF compressed on the GPU and a .tbi), the SNF through snf.write_results."""
+  * the VCF goes through vcf.open_output (a .vcf.gz gets BGZF compressed on the GPU and a .tbi), the SNF through snf.write_results;
+  * with --gpus N > 1, under torchrun, every rank runs its share of the tasks and rank 0 writes the files (call_sample_ranks)."""
 import contextlib
 import logging
 import math
@@ -86,11 +87,11 @@ def group_passes(items, budget, size=lambda item: item[-1]):
         yield group
 
 
-def task_inputs(bam, planned, stats=None, regions_by_contig=None):
+def task_inputs(bam, planned, stats=None, regions_by_contig=None, failed=None):
     """per planned task, in task order: (task id, contig, start, end, BGZF bytes, spans, inflated bytes, regions) of
     bamio.BamFile.device_input over the task's fetch windows (tasks.fetch_windows; regions: those windows when the contig has regions, else
-    None).  A task whose regions pysam would refuse is logged and left out, as the reference's worker fails it.  The time spent reading
-    is added to stats["read_s"]"""
+    None).  A task whose regions pysam would refuse is logged and left out, as the reference's worker fails it (and listed in `failed` as
+    (task id, contig, error class name)).  The time spent reading is added to stats["read_s"]"""
     for tid, name, s, e in planned:
         t0 = time.perf_counter()
         rg = (regions_by_contig or {}).get(name)
@@ -98,6 +99,8 @@ def task_inputs(bam, planned, stats=None, regions_by_contig=None):
             windows = tasks.fetch_windows(name, s, e, rg)
         except ValueError as err:
             log.error(f"Error in worker process while executing CallTask(id={tid}, contig={name}, start={s}, end={e}): {err}")
+            if failed is not None:
+                failed.append((tid, name, type(err).__name__))
             continue
         z, spans = bam.device_input([(name, a, b) for a, b in windows], tags=[(0, g) for g in range(len(windows))])
         n = inflated_bytes(z)
@@ -125,9 +128,10 @@ def join_inputs(inputs, n_regions=None):
     return bgzf, np.concatenate(rows) if rows else np.zeros(0, abi.SPAN_DTYPE)
 
 
-def run_pass(ctx, bam, group, config, tr_all, device=0):
+def run_pass(ctx, bam, group, config, tr_all, device=0, contigs=None, failed=None):
     """one device pass over `group` (items of task_inputs): mask_block, snfb_load_bam, snfb_run, then every task as a CallTask on the
-    pass's BlockRun.  Returns [(CallTask, calls)] in task order and the pass's split {"load_bam_s", "run_s", "finalize_s"}."""
+    pass's BlockRun.  Returns [(CallTask, calls)] in task order and the pass's split {"load_bam_s", "run_s", "finalize_s"}.  contigs: the
+    names tasks.reference_for loads (None: all); failed: receives (task id, contig, error class name) of every task that fails."""
     tr = {k: [(int(a), int(b)) for a, b in tr_all[g[1]]] for k, g in enumerate(group) if g[1] in tr_all}
     # a task with regions: its records carry their region's window, its own bounds only clip the N mask (the host clips it to the regions)
     bounds = [(0, bam.get_reference_length(name)) if rg else (s, e) for _, name, s, e, _, _, _, rg in group]
@@ -135,7 +139,7 @@ def run_pass(ctx, bam, group, config, tr_all, device=0):
     by_task = [(k, g[7] or [(g[2], g[3])]) for k, g in enumerate(group)]
     has_regions = any(g[7] for g in group)
     mask_regions = {k: g[7] for k, g in enumerate(group) if g[7]}
-    tasks.mask_block(block, config, ctx, mask_regions) if mask_regions else tasks.mask_block(block, config, ctx)
+    tasks.mask_block(block, config, ctx, mask_regions or None, contigs)
     ctx.set_config(abi.Config.from_sniffles(config))
     bgzf, spans = join_inputs([(g[4], g[5]) for g in group], [len(w) for _, w in by_task] if has_regions else None)
     split = {}
@@ -159,21 +163,18 @@ def run_pass(ctx, bam, group, config, tr_all, device=0):
             calls, _ = task.execute()
         except tasks.CallTaskError as err:      # logged and left out, as the reference's worker leaves a failed task out
             log.error(f"Error in worker process while executing CallTask(id={tid}, contig={name}, start={s}, end={e}): {err}")
+            if failed is not None:
+                failed.append((tid, name, type(err).__name__))
             continue
         done.append((task, calls))
     split["finalize_s"] = time.perf_counter() - t2
     return done, split
 
 
-def call_sample(config, device=0, budget=None, stats=None):
-    """the call_sample run mode: config.input (one indexed BAM) -> config.vcf and / or config.snf.  budget: the inflated BAM bytes one
-    device pass may load (default: device_budget).  stats: a dict that receives the run's split (passes, per-pass inflated bytes and
-    times, VCF and SNF write times).  Returns the number of VCF records written."""
-    if getattr(config, "gpus", 1) > 1:
-        raise CallSampleError("--gpus > 1 is not supported for calling a sample: one GPU calls the whole BAM")
-    check_outputs(config)
-    st = stats if stats is not None else {}
-    t0 = time.perf_counter()
+def plan_sample(config):
+    """what every run does before its first pass, the same on every rank: open config.input, set config.task_read_id_offset_mult,
+    config.contig_lengths and config.sample_ids_vcf, plan the tasks and load the tandem repeats with the reference's fatal check.
+    Returns (bam, processed contigs [(name, length)], planned tasks [(task id, name, start, end)], {contig: tandem repeats})."""
     path = config.input[0] if isinstance(config.input, (list, tuple)) else config.input
     bam = bamio.BamFile(path)
     config.task_read_id_offset_mult = read_id_offset_mult(total_mapped(bam))
@@ -190,6 +191,38 @@ def call_sample(config, device=0, budget=None, stats=None):
                                       "the sample input file. Please check if the contig naming scheme in the tandem repeat annotations "
                                       "matches with the one in the input sample file.")
     config.sample_ids_vcf = [(0, "SAMPLE" if config.sample_id is None else config.sample_id)]
+    return bam, contig_lengths, planned, tr_all
+
+
+def _world_size():
+    """the size of the initialised torch.distributed process group, 1 without one"""
+    try:
+        import torch.distributed as tdist
+    except ImportError:
+        return 1
+    return tdist.get_world_size() if tdist.is_available() and tdist.is_initialized() else 1
+
+
+def call_sample(config, device=0, budget=None, stats=None):
+    """the call_sample run mode: config.input (one indexed BAM) -> config.vcf and / or config.snf.  budget: the inflated BAM bytes one
+    device pass may load (default: device_budget).  stats: a dict that receives the run's split (passes, per-pass inflated bytes and
+    times, VCF and SNF write times).  Returns the number of VCF records written.
+
+    With --gpus N > 1 the run is one process per GPU (torchrun --nproc-per-node N -m sniffles_b200 ... --gpus N): it needs an initialised
+    process group of N ranks and goes through call_sample_ranks."""
+    gpus = getattr(config, "gpus", 1)
+    if gpus > 1:
+        world = _world_size()
+        if world == 1:
+            raise CallSampleError(f"--gpus {gpus} runs one process per GPU: launch with torchrun --nproc-per-node {gpus} -m sniffles_b200 ... "
+                                  f"--gpus {gpus}")
+        if world != gpus:
+            raise CallSampleError(f"--gpus {gpus} does not match the {world} ranks of the process group")
+        return call_sample_ranks(config, device, budget, stats)
+    check_outputs(config)
+    st = stats if stats is not None else {}
+    t0 = time.perf_counter()
+    bam, contig_lengths, planned, tr_all = plan_sample(config)
     ctx = tasks.device_context(device)
     reference = tasks.reference_for(ctx, config.reference) if getattr(config, "reference", None) else None
     if budget is None:
@@ -236,3 +269,144 @@ def call_sample(config, device=0, budget=None, stats=None):
         log.info(f"Wrote {written} called SVs to {config.vcf}")
     st["wall_s"] = time.perf_counter() - t0
     return written
+
+
+def run_rank_tasks(config, device, budget, rank, world):
+    """one rank's share of a multi-GPU run: the plan every rank makes alike (plan_sample), the tasks dist.lpt_assign gives this rank over
+    dist.task_weights, then the loop of call_sample over them in task-id order, each task's VCF records formatted here into text.  With
+    --reference only the contigs of this rank's tasks are loaded, and the N mask and the VCF writer use that one object.  Returns the
+    payload rank 0 merges (write_rank_outputs): {"rank", "tasks": [(task id, VCF text, records, SNF part or None)], "failed": [(task id,
+    contig, error class name)], "nm": (last task id, average_regional_nm, qc_nm_threshold) or None, "stats", "error": None}."""
+    import io
+    from . import dist
+    t0 = time.perf_counter()
+    st = dict(passes=0, pass_inflated_bytes=[], load_bam_s=[], run_s=[], finalize_s=0.0, vcf_write_s=0.0, read_s=0.0)
+    bam, contig_lengths, planned, tr_all = plan_sample(config)
+    weights = dist.task_weights(bam, planned, config.regions_by_contig)
+    owner = dist.lpt_assign(weights, world)
+    mine = [p for p, o in zip(planned, owner) if o == rank]
+    contigs = sorted({name for _, name, _, _ in mine})
+    ctx = tasks.device_context(device)
+    reference = tasks.reference_for(ctx, config.reference, contigs) if getattr(config, "reference", None) and mine else None
+    if budget is None:
+        budget = device_budget(device)
+    st.update(tasks=len(mine), weight=sum(w for w, o in zip(weights, owner) if o == rank), index_s=time.perf_counter() - t0)
+    out, failed, nm = [], [], None
+    for group in group_passes(task_inputs(bam, mine, st, config.regions_by_contig, failed), budget, size=lambda item: item[6]):
+        done, split = run_pass(ctx, bam, group, config, tr_all, device, contigs, failed)
+        # the config holds the N-mismatch mean of the pass's last task: the SNF header of rank 0 takes that of the run's last task
+        nm = (group[-1][0], config.average_regional_nm, config.qc_nm_threshold)
+        st["passes"] += 1
+        st["pass_inflated_bytes"].append(sum(g[6] for g in group))
+        st["load_bam_s"].append(split["load_bam_s"])
+        st["run_s"].append(split["run_s"])
+        st["finalize_s"] += split["finalize_s"]
+        t1 = time.perf_counter()
+        if config.vcf is not None and reference is not None:
+            reference.prefetch(vcf.reference_intervals([c for _, calls in done for c in calls], config))
+        for task, calls in done:
+            text, n = "", 0
+            if config.vcf is not None:
+                buf = io.StringIO()
+                writer = vcf.VCFWriter(config, buf, reference)
+                n = sum(writer.write_call(c) for c in calls)
+                text = buf.getvalue()
+            out.append((task.id, text, n, task.snf_part))
+        st["vcf_write_s"] += time.perf_counter() - t1
+    bam.close()
+    st["inflated_bytes"] = sum(st["pass_inflated_bytes"])
+    st["wall_s"] = time.perf_counter() - t0
+    return {"rank": rank, "tasks": out, "failed": failed, "nm": nm, "stats": st, "error": None}
+
+
+def write_rank_outputs(config, contig_lengths, payloads, ctx=None):
+    """rank 0's merge of every rank's payload (run_rank_tasks): when any rank failed, no file is written and CallSampleError names the
+    first failed rank and its message; otherwise the VCF header, then every task's records in task-id
+    order through vcf.open_output (a .vcf.gz compressed on the device of `ctx`), and the SNF through snf.write_results.  Returns (records
+    written, VCF write seconds, SNF write seconds)."""
+    failed = [p for p in payloads if p["error"] is not None]
+    if failed:
+        raise CallSampleError(f"rank {failed[0]['rank']}: {failed[0]['error']}")
+    done = sorted((t for p in payloads for t in p["tasks"]), key=lambda t: t[0])
+    last = max((p["nm"] for p in payloads if p["nm"] is not None), default=None, key=lambda x: x[0])
+    if last is not None:
+        config.average_regional_nm, config.qc_nm_threshold = last[1], last[2]
+    written, vcf_s, snf_s = 0, 0.0, 0.0
+    if config.vcf is not None:
+        t0 = time.perf_counter()
+        with contextlib.ExitStack() as stack:
+            handle = vcf.open_output(config, ctx)
+            if config.vcf_output_bgz:
+                stack.enter_context(handle)           # compressed and indexed when the writing ends without an error
+            else:
+                stack.callback(handle.close)
+            vcf.VCFWriter(config, handle).write_header(contig_lengths)
+            for _, text, n, _ in done:
+                handle.write(text)
+                written += n
+        vcf_s = time.perf_counter() - t0
+    if config.snf is not None:
+        t0 = time.perf_counter()
+        with open(config.snf, "wb") as f:
+            n = snf.write_results(f, config, [t[3] for t in done if t[3] is not None], [name for name, _ in contig_lengths])
+        snf_s = time.perf_counter() - t0
+        log.info(f"Wrote {n} SV candidates to {config.snf} (for multi-sample calling).")
+    if config.vcf is not None:
+        log.info(f"Wrote {written} called SVs to {config.vcf}")
+    return written, vcf_s, snf_s
+
+
+def _error_text(e):
+    return str(e) if isinstance(e, CallSampleError) else f"{type(e).__name__}: {e}"
+
+
+def call_sample_ranks(config, device, budget=None, stats=None):
+    """call_sample over the ranks of an initialised torch.distributed process group (one process per GPU; gloo, since the only
+    collectives carry host objects).  Rank 0 checks the outputs and broadcasts the verdict; every rank plans alike, runs its own tasks
+    (run_rank_tasks) and sends its payload to rank 0 with gather_object, an error included, so that every rank reaches the gather.  Rank 0
+    writes the files (write_rank_outputs) and broadcasts (ok, records written or the error): every rank returns the same count or raises
+    the same CallSampleError.  Rank 0 holds every rank's VCF text and SNF parts at once, host memory in proportion to the output files.
+
+    stats on rank 0: the keys of call_sample for rank 0's own work, plus "ranks" (per rank its split, tasks, inflated bytes, index weight
+    and failed tasks), "gather_s" and "write_s"."""
+    import torch.distributed as tdist
+    rank, world = tdist.get_rank(), tdist.get_world_size()
+    t0 = time.perf_counter()
+    verdict = [None]
+    if rank == 0:
+        try:
+            check_outputs(config)
+        except CallSampleError as e:
+            verdict[0] = str(e)
+    tdist.broadcast_object_list(verdict, src=0)
+    if verdict[0] is not None:
+        raise CallSampleError(verdict[0])
+    try:
+        payload = run_rank_tasks(config, device, budget, rank, world)
+    except Exception as e:                   # into the payload: a rank that raised before the gather would leave the others waiting
+        log.error(_error_text(e))
+        payload = {"rank": rank, "tasks": [], "failed": [], "nm": None, "stats": {}, "error": _error_text(e)}
+    t1 = time.perf_counter()
+    gathered = [None] * world if rank == 0 else None
+    tdist.gather_object(payload, gathered, dst=0)
+    status = [None]
+    if rank == 0:
+        t2 = time.perf_counter()
+        try:
+            written, vcf_s, snf_s = write_rank_outputs(config, getattr(config, "contig_lengths", []), gathered, tasks.device_context(device))
+            status[0] = (True, written)
+        except Exception as e:
+            status[0] = (False, _error_text(e))
+        t3 = time.perf_counter()
+        if status[0][0] and stats is not None:
+            stats.update({k: v for k, v in payload["stats"].items() if k not in ("tasks", "weight", "inflated_bytes")})
+            stats["vcf_write_s"] += vcf_s
+            stats["snf_write_s"] = snf_s
+            stats["ranks"] = [dict(p["stats"], failed=p["failed"]) for p in gathered]
+            stats["gather_s"], stats["write_s"] = t2 - t1, t3 - t2
+            stats["wall_s"] = t3 - t0
+    tdist.broadcast_object_list(status, src=0)
+    ok, value = status[0]
+    if not ok:
+        raise CallSampleError(value)
+    return value

@@ -1,7 +1,13 @@
 """Multi-GPU plumbing (SURVEY.md §8e): the path shards by contig — one process per GPU, contigs
 assigned longest-first, no data-path collective — and ends with ONE all-gather that concatenates
 the per-rank candidate buffers before VCF emission.  torch.distributed is used for the
-collective only (NCCL over NVLink on the GPU box, gloo in the CPU tests)."""
+collective only (NCCL over NVLink on the GPU box, gloo in the CPU tests).
+
+Calling a sample on several GPUs (call.call_sample_ranks) weighs its tasks with task_weights,
+assigns them with lpt_assign, and gathers each rank's finished VCF text and SNF parts instead."""
+import bisect
+import os
+
 import numpy as np
 
 
@@ -15,6 +21,43 @@ def lpt_assign(weights, n_ranks):
         owner[c] = r
         load[r] += weights[c]
     return owner
+
+
+def _block_bounds(bam):
+    """the BGZF block starts the BAM index names (every chunk bound, linear-index entry and CSI loffset), and the file's end, sorted"""
+    starts = {os.path.getsize(bam.path)}
+    for bins, lin, loff in bam.index:
+        for b, chunks in bins.items():
+            if b != bam.meta_bin:                    # the pseudo-bin holds counts, not offsets
+                starts.update(v >> 16 for c in chunks for v in c)
+        starts.update(v >> 16 for v in (lin or ()))
+        starts.update(v >> 16 for v in (loff or {}).values())
+    return sorted(starts)
+
+
+def task_weights(bam, planned, regions_by_contig=None):
+    """per planned task [(task id, contig, start, end)] of tasks.plan, the compressed BAM bytes its fetches read: the BGZF blocks of
+    every bamio.BamFile.merged_chunks range over the task's tasks.fetch_windows.  Read from the index alone, so a rank that weighs the
+    tasks reads no BGZF block: a range that ends inside a block counts that block up to the next block start the index names.  A task
+    whose windows are refused weighs 0: it fails on whichever rank runs it."""
+    from . import tasks
+    bounds = _block_bounds(bam)
+
+    def chunk_bytes(vb, ve):
+        cb, ce = vb >> 16, ve >> 16
+        if ve & 0xffff:
+            ce = bounds[min(bisect.bisect_right(bounds, ce), len(bounds) - 1)]
+        return max(ce - cb, 0)
+
+    out = []
+    for _, name, s, e in planned:
+        try:
+            windows = tasks.fetch_windows(name, s, e, (regions_by_contig or {}).get(name))
+        except ValueError:
+            out.append(0)
+            continue
+        out.append(sum(chunk_bytes(vb, ve) for a, b in windows for vb, ve in bam.merged_chunks(name, a, b)))
+    return out
 
 
 def subset_block(block, task_ids):

@@ -21,28 +21,31 @@ def device_context(device: int = 0) -> binding.Context:
     return _CTX[device]
 
 
-_REF = {}      # per (device context, FASTA path): the fasta.Reference loaded on it, or None when it could not be loaded
+_REF = {}      # per (device context, FASTA path, loaded contigs): the fasta.Reference loaded on it, or None when it could not be loaded
 
 
-def reference_for(ctx, path):
-    """the reference FASTA resident on `ctx`, loaded on first use.  A FASTA that cannot be opened or read (a missing or stale index, a
-    damaged BGZF block) is logged once as the reference logs it (vcf.py:116-119) and the run goes on without it."""
-    key = (ctx, str(path))
+def reference_for(ctx, path, contigs=None):
+    """the reference FASTA resident on `ctx`, loaded on first use.  contigs: the names to load (None: all), as one rank of a multi-GPU
+    run loads only the contigs of its tasks; every caller of a run passes the same names, so the N mask and the VCF writer share one
+    object.  A FASTA that cannot be opened or read (a missing or stale index, a damaged BGZF block) is logged once as the reference logs
+    it (vcf.py:116-119) and the run goes on without it."""
+    key = (ctx, str(path), None if contigs is None else tuple(sorted(set(contigs))))
     if key not in _REF:
         from . import fasta
         try:
-            _REF[key] = fasta.Reference(path, ctx)
+            _REF[key] = fasta.Reference(path, ctx, contigs=contigs)
         except (OSError, ValueError, RuntimeError) as e:
             logging.error(f"Unable to open reference file {path}: {e}")
             _REF[key] = None
     return _REF[key]
 
 
-def mask_block(block, config, ctx, regions=None):
+def mask_block(block, config, ctx, regions=None, contigs=None):
     """with config.reference: the block's N-mask tables from the reference loaded on `ctx` (LeadProvider._mask_N_coverage,
-    leadprov.py:420-443), before the block is loaded; without it the block is left as it is.  regions: {task index: [(start, end)]}"""
+    leadprov.py:420-443), before the block is loaded; without it the block is left as it is.  regions: {task index: [(start, end)]};
+    contigs: the names reference_for loads (None: all)"""
     if getattr(config, "reference", None):
-        ref = reference_for(ctx, config.reference)
+        ref = reference_for(ctx, config.reference, contigs)
         if ref is not None:
             from . import fasta
             fasta.mask_block(block, ref, regions)
