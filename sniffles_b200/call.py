@@ -128,10 +128,11 @@ def join_inputs(inputs, n_regions=None):
     return bgzf, np.concatenate(rows) if rows else np.zeros(0, abi.SPAN_DTYPE)
 
 
-def run_pass(ctx, bam, group, config, tr_all, device=0, contigs=None, failed=None):
-    """one device pass over `group` (items of task_inputs): mask_block, snfb_load_bam, snfb_run, then every task as a CallTask on the
-    pass's BlockRun.  Returns [(CallTask, calls)] in task order and the pass's split {"load_bam_s", "run_s", "finalize_s"}.  contigs: the
-    names tasks.reference_for loads (None: all); failed: receives (task id, contig, error class name) of every task that fails."""
+def load_pass(ctx, bam, group, config, tr_all, contigs=None):
+    """the device half of a pass over `group` (items of task_inputs): mask_block, set_config, set_regions, snfb_load_bam and snfb_run,
+    the k-th task of the group being task index k of the block.  Returns the pass's tasks.BlockRun and its split {"load_bam_s", "run_s"};
+    a load or run the library refuses raises CallSampleError naming the pass's contigs and inflated bytes.  contigs: the names
+    tasks.reference_for loads (None: all)."""
     tr = {k: [(int(a), int(b)) for a, b in tr_all[g[1]]] for k, g in enumerate(group) if g[1] in tr_all}
     # a task with regions: its records carry their region's window, its own bounds only clip the N mask (the host clips it to the regions)
     bounds = [(0, bam.get_reference_length(name)) if rg else (s, e) for _, name, s, e, _, _, _, rg in group]
@@ -139,7 +140,8 @@ def run_pass(ctx, bam, group, config, tr_all, device=0, contigs=None, failed=Non
     by_task = [(k, g[7] or [(g[2], g[3])]) for k, g in enumerate(group)]
     has_regions = any(g[7] for g in group)
     mask_regions = {k: g[7] for k, g in enumerate(group) if g[7]}
-    tasks.mask_block(block, config, ctx, mask_regions or None, contigs)
+    # without regions or a contig subset the N mask is the plain mask_block(block, config, ctx), as --genotype-vcf has always called it
+    tasks.mask_block(block, config, ctx, *((mask_regions or None, contigs) if mask_regions or contigs is not None else ()))
     ctx.set_config(abi.Config.from_sniffles(config))
     bgzf, spans = join_inputs([(g[4], g[5]) for g in group], [len(w) for _, w in by_task] if has_regions else None)
     split = {}
@@ -155,7 +157,15 @@ def run_pass(ctx, bam, group, config, tr_all, device=0, contigs=None, failed=Non
         raise CallSampleError(f"the device pass over contig(s) {names} ({sum(g[6] for g in group)} inflated BAM bytes) failed: {e}") from e
     split["load_bam_s"], split["run_s"] = t1 - t0, t2 - t1
     rec_nm = abi.view(res._rec_nm_ptr, "<f8", n_rec).copy() if getattr(res, "_rec_nm_ptr", None) else None
-    br = tasks.BlockRun(block, res, tasks.cand_ranges(res.cand, len(block.task)), rec_nm)
+    return tasks.BlockRun(block, res, tasks.cand_ranges(res.cand, len(block.task)), rec_nm), split
+
+
+def run_pass(ctx, bam, group, config, tr_all, device=0, contigs=None, failed=None):
+    """one device pass over `group` (items of task_inputs): load_pass, then every task as a CallTask on the pass's BlockRun.  Returns
+    [(CallTask, calls)] in task order and the pass's split {"load_bam_s", "run_s", "finalize_s"}.  contigs: the names
+    tasks.reference_for loads (None: all); failed: receives (task id, contig, error class name) of every task that fails."""
+    br, split = load_pass(ctx, bam, group, config, tr_all, contigs)
+    t2 = time.perf_counter()
     done = []
     for k, (tid, name, s, e, *_) in enumerate(group):
         task = tasks.CallTask(id=tid, sv_id=0, contig=name, start=s, end=e, config=config, block_run=br, task_index=k, device=device)

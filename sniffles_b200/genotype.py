@@ -5,17 +5,22 @@ vcf.py:352-478; result.py:118-130).
     input is read as BGZF text (bamio.BgzfReader), where the reference goes through pysam.VariantFile (DESIGN §4);
   * `plan` makes one task per processed contig, [0, contig_len - 1), holding the contig's targets with start <= pos < end;
   * matching and the coverage probes run on the device (snfb_genotype_targets); `genotype_of` and the rewrite stay on the host;
-  * `genotype_vcf(config)` drives the mode: one device ingest and run for every task, one snfb_genotype_targets call for every target,
-    then the rewritten VCF through vcf.open_output."""
+  * `genotype_vcf(config)` drives the mode in the device passes of call.call_sample: the tasks with targets, in task-id order, grouped
+    so that their inflated BAM bytes fit a budget (call.group_passes over call.task_inputs, so host memory holds one pass's BGZF bytes).
+    A pass is call.load_pass (N mask, snfb_load_bam, snfb_run), one snfb_genotype_targets call for the targets of its tasks, then its
+    tasks' records, rewritten through vcf.open_output, before the next pass loads.  The records come in task order, and in target-file
+    order inside a task, so the output is the same at every budget.  The genotype step's device memory (about 63 bytes per target
+    and 28 per candidate of the pass, kept on the context) sits inside the margin call.device_budget leaves (DESIGN §8)."""
 import io
 import logging
 import os
+import time
 from dataclasses import dataclass
 from typing import Optional
 
 import numpy as np
 
-from . import abi, bamio, vcf
+from . import abi, bamio, binding, vcf
 
 log = logging.getLogger("sniffles_b200.genotype")
 
@@ -218,51 +223,63 @@ def write_tasks(handle, br, jobs, config):
     return written
 
 
-def genotype_vcf(config, device=0):
-    """the --genotype-vcf run mode: returns the number of records written to config.vcf"""
-    from . import tasks
+def genotype_vcf(config, device=0, budget=None, stats=None):
+    """the --genotype-vcf run mode: config.input (one indexed BAM) and config.genotype_vcf -> config.vcf.  Returns the number of records
+    written.  budget: the inflated BAM bytes one device pass may load (default: call.device_budget).  stats: a dict that receives the
+    run's split, with call.call_sample's keys where they apply (passes, pass_inflated_bytes, load_bam_s and run_s per pass, read_s,
+    index_s, wall_s) and parse_s (the target VCF), genotype_s (per pass, the snfb_genotype_targets round trip) and write_s (the tasks'
+    host epilogue and rewrite, the header and the output's close: a .vcf.gz is compressed and indexed then)."""
+    from . import call, tasks
+    st = stats if stats is not None else {}
+    t0 = time.perf_counter()
     header, targets = read_targets(config.genotype_vcf)
     log.info(f"Opening for reading: {config.genotype_vcf} (read {len(targets)} SVs to be genotyped)")
+    st.update(passes=0, pass_inflated_bytes=[], load_bam_s=[], run_s=[], genotype_s=[], read_s=0.0, write_s=0.0, parse_s=time.perf_counter() - t0)
+    t1 = time.perf_counter()
     path = config.input[0] if isinstance(config.input, (list, tuple)) else config.input
     bam = bamio.BamFile(path)
-    planned = []
-    for p in plan(bam.contigs, targets, config):
-        if not p[4]:                                    # a task without targets writes nothing
+    planned, targets_of = [], {}
+    for tid, name, s, e, ts in plan(bam.contigs, targets, config):
+        if not ts:                                      # a task without targets writes nothing
             continue
-        tid, name, s, e, _ = p
-        regions = config.regions_by_contig.get(name)
         try:
-            windows = tasks.fetch_windows(name, s, e, regions)
+            tasks.fetch_windows(name, s, e, config.regions_by_contig.get(name))
         except ValueError as err:                       # the task fails in the reference's worker: its targets are not written
             log.error(f"Error in worker process while executing GenotypeTask(id={tid}, contig={name}, start={s}, end={e}): {err}")
             continue
-        planned.append((p, windows if regions else None))
+        planned.append((tid, name, s, e))
+        targets_of[tid] = ts
     tr_all = tasks.load_tandem_repeats(config.tandem_repeats, config.tandem_repeat_region_pad) if config.tandem_repeats else {}
     ctx = tasks.device_context(device)
+    if budget is None:
+        budget = call.device_budget(device)
+    st["index_s"] = time.perf_counter() - t1
+    written = 0
     with vcf.open_output(config, ctx) as handle:
+        t1 = time.perf_counter()
         handle.write(rewrite_header(header, config))
-        if not planned:
-            return 0
-        tr = {k: [(int(a), int(b)) for a, b in tr_all[p[1]]] for k, (p, _) in enumerate(planned) if p[1] in tr_all}
-        # a task with regions: its records carry their region's window, its own bounds only clip the N mask (clipped to the regions here)
-        bounds = [(0, bam.get_reference_length(p[1])) if rg else (p[2], p[3]) for p, rg in planned]
-        block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[p[1]], a, b, p[0]) for (p, _), (a, b) in zip(planned, bounds)], tandem_repeats=tr or None)
-        # target coverage is N-masked as in GenotypeTask's LeadProvider; without regions the call is the one it always was
-        mask_regions = {k: rg for k, (_, rg) in enumerate(planned) if rg}
-        tasks.mask_block(block, config, ctx, mask_regions) if mask_regions else tasks.mask_block(block, config, ctx)
-        ctx.set_config(abi.Config.from_sniffles(config))
-        by_task = [(k, rg or [(p[2], p[3])]) for k, (p, rg) in enumerate(planned)]
-        queries, tags, n = [], [], 0
-        for (k, w), (p, _) in zip(by_task, planned):
-            queries += [(p[1], a, b) for a, b in w]
-            tags += [(k, n + g) for g in range(len(w))]
-            n += len(w)
-        has_regions = any(rg for _, rg in planned)
-        bgzf, spans = bam.device_input(queries, tags=tags)
-        ctx.set_regions(tasks.region_table(by_task) if has_regions else None)
-        n_rec = ctx.load_bam(bgzf, spans, block)["n_rec"]
-        res = ctx.run(want_leads=True, want_cands=True, want_seqs=True)
-        rec_nm = abi.view(res._rec_nm_ptr, "<f8", n_rec).copy() if getattr(res, "_rec_nm_ptr", None) else None
-        br = tasks.BlockRun(block, res, tasks.cand_ranges(res.cand, len(block.task)), rec_nm)
-        br.genotype = device_targets(ctx, [(k, p[4]) for k, (p, _) in enumerate(planned)], bam.name_to_id, config)
-        return write_tasks(handle, br, [p + (k,) for k, (p, _) in enumerate(planned)], config)
+        st["write_s"] += time.perf_counter() - t1
+        # a pass's targets are matched against the candidates and coverage of the block resident on the context: every step of a pass
+        # ends before the next pass loads
+        for group in call.group_passes(call.task_inputs(bam, planned, st, config.regions_by_contig), budget, size=lambda item: item[6]):
+            br, split = call.load_pass(ctx, bam, group, config, tr_all)
+            st["passes"] += 1
+            st["pass_inflated_bytes"].append(sum(g[6] for g in group))
+            st["load_bam_s"].append(split["load_bam_s"])
+            st["run_s"].append(split["run_s"])
+            t1 = time.perf_counter()
+            try:
+                br.genotype = device_targets(ctx, [(k, targets_of[g[0]]) for k, g in enumerate(group)], bam.name_to_id, config)
+            except binding.SnfbError as e:
+                names = ", ".join(g[1] for g in group)
+                raise call.CallSampleError(f"the target genotyping of the device pass over contig(s) {names} "
+                                           f"({st['pass_inflated_bytes'][-1]} inflated BAM bytes) failed: {e}") from e
+            t2 = time.perf_counter()
+            written += write_tasks(handle, br, [(tid, name, s, e, targets_of[tid], k) for k, (tid, name, s, e, *_) in enumerate(group)], config)
+            st["genotype_s"].append(t2 - t1)
+            st["write_s"] += time.perf_counter() - t2
+        t1 = time.perf_counter()
+    st["write_s"] += time.perf_counter() - t1
+    bam.close()
+    st["wall_s"] = time.perf_counter() - t0
+    return written
