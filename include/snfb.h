@@ -306,7 +306,7 @@ typedef struct snfb_ctx snfb_ctx;
 
 int         snfb_version(void);
 /* sizeof of the ABI structs, for binding self-checks: 0 rec, 1 task, 2 contig, 3 records, 4 config, 5 lead, 6 cand, 7 gather_view,
- * 8 gt_in, 9 gt_out, 10 ref_contig, 11 ref_input, 12 ref_query, 13 region */
+ * 8 gt_in, 9 gt_out, 10 ref_contig, 11 ref_input, 12 ref_query, 13 region, 14 combine_plan_in, 15 combine_plan_out */
 size_t      snfb_sizeof(int which);
 uint64_t    snfb_hash_name(const char* s, size_t n);
 int         snfb_ctx_create(int device, snfb_ctx** out);
@@ -496,6 +496,31 @@ typedef struct snfb_combine_out {
     int32_t*  cov_non;        /* [n_cand][n_samples]; -1 where the sample is included (never probed) */
 } snfb_combine_out;
 int         snfb_combine_groups(snfb_ctx* ctx, const snfb_combine_in* in, snfb_combine_out* out);
+/* ---- the chunk plan of combine mode on the device, then the grouping (CombineTask.execute, parallel.py:484-572) ----
+ * The host decodes the SNF blocks of one or more tasks into flat columns, in the reference's iteration order: task, block, svtype,
+ * sample, part, list position.  `group` carries the per-candidate columns pos, svlen, sample, mate_contig, mate_pos and the ALT arena in
+ * that flat order (n_cand = n_flat), the coverage tables and the grouping parameters, as snfb_combine_groups reads them; its chains,
+ * chunks, n_chain and n_chunk are not read.  task is the task's index (< n_task <= 2^24), row the coverage row of the candidate's
+ * (task, block), rows being numbered in (task, block) order; svtype 0..4 is INS DEL DUP INV BND.  The device
+ *   - drops candidates with support < support_threshold,
+ *   - sorts the rest stably on (task, svtype, block, bin), bin = int(pos / bin_min_size) * bin_min_size (the bins dict of one block),
+ *   - cuts each (task, block, svtype) run into chunks: whole bins, closed at bin_max_candidates (unless exhaustive) or at the last bin,
+ *   - sorts each chunk stably by support, descending (cluster.py:361),
+ *   - builds the chain and chunk tables in device memory (chunk.cov_block = row, pads 0) and runs the grouping of snfb_combine_groups.
+ * Outputs, each with room for n_flat entries: n_cand kept candidates; perm[slot] = the flat index in slot `slot`; the n_chain chains and
+ * n_chunk chunks in the layout snfb_combine_groups reads; group: its four outputs per slot.  Timing marks "combine_plan", "combine_groups". */
+typedef struct snfb_combine_plan_in {
+    uint32_t n_flat, n_task;
+    const uint32_t* task; const uint32_t* row; const int32_t* svtype; const int32_t* support;
+    int32_t support_threshold, bin_min_size, bin_max_candidates, exhaustive;
+    snfb_combine_in group;
+} snfb_combine_plan_in;
+typedef struct snfb_combine_plan_out {
+    uint32_t n_cand, n_chain, n_chunk, pad;
+    uint32_t* perm; snfb_combine_chain* chains; snfb_combine_chunk* chunks;
+    snfb_combine_out group;
+} snfb_combine_plan_out;
+int         snfb_combine_plan(snfb_ctx* ctx, const snfb_combine_plan_in* in, snfb_combine_plan_out* out);
 /* self-check of the exact statistics.stdev arithmetic (host build of the routine the kernels use): the correctly rounded sqrt(P / Q) for
  * P = p_hi * 2^64 + p_lo; slow != 0 selects the limb-by-limb restatement of CPython's _float_sqrt_of_frac, 0 the verified fast path */
 double      snfb_selftest_sqrt_frac(uint64_t p_hi, uint64_t p_lo, uint64_t q, int slow);

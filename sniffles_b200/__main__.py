@@ -1,6 +1,7 @@
-"""`python -m sniffles_b200 ARGS`: the reference's command line (sniffles:64-148) for the two run modes that read one BAM -- calling a
-sample (`-i sample.bam -v out.vcf [--snf out.snf]`, call.call_sample) and force calling (`--genotype-vcf`, genotype.genotype_vcf).
-Combine mode (.snf / .tsv input) and CRAM input are not run from here.
+"""`python -m sniffles_b200 ARGS`: the reference's command line (sniffles:64-148) for its three run modes -- calling a sample
+(`-i sample.bam -v out.vcf [--snf out.snf]`, call.call_sample), force calling (`--genotype-vcf`, genotype.genotype_vcf) and combining
+samples (`-i a.snf b.snf ... -v out.vcf` or `-i samples.tsv -v out.vcf`, combine_run.combine_snfs, on one GPU).  CRAM input is not run
+from here.
 
 Calling a sample on N GPUs is one process per GPU:
 
@@ -13,7 +14,7 @@ import logging
 import os
 import sys
 
-from . import call, genotype
+from . import call, combine_run, genotype
 from .config import SnifflesConfig
 
 # how long a rank waits in a collective: the ranks finish their tasks at different times and wait for the last one in the gather
@@ -61,6 +62,27 @@ def _main_ranks(config, world, log):
     return code
 
 
+def _main_combine(config, log):
+    """combine mode (.snf / .tsv inputs) on one GPU"""
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    refusal = None
+    if world > 1:
+        refusal = f"combine mode (.snf / .tsv input) runs on one GPU: run it without torchrun ({world} ranks would each write {config.vcf})"
+    elif config.combine_consensus:
+        refusal = "--combine-consensus is not supported: the reference's SVGroup.call cannot run with it either (sv.py:387)"
+    elif config.combine_population is not None or config.dev_population_snf is not None:
+        refusal = "--combine-population and --dev-population-snf (population SNFs, allele frequencies) are not supported by sniffles_b200"
+    if refusal is not None:
+        log.error(f"{refusal} (Fatal error, exiting.)")
+        return 1
+    try:
+        combine_run.combine_snfs(config)
+    except combine_run.CombineError as e:
+        log.error(f"{e} (Fatal error, exiting.)")
+        return 1
+    return 0
+
+
 def main(argv=None):
     argv = list(sys.argv[1:] if argv is None else argv)
     config = SnifflesConfig(*argv)
@@ -68,6 +90,12 @@ def main(argv=None):
     config.command = " ".join(["sniffles"] + argv)
     log = logging.getLogger("sniffles_b200.main")
     exts = {f.split(".")[-1].lower() for f in config.input}
+    if len(exts) > 1:
+        log.error(f"Please specify either: A single .bam/.cram file - OR - one or more .snf files - OR - a single .tsv file containing a list of "
+                  f".snf files and optional sample ids as input. (supplied were: {list(exts)}) (Fatal error, exiting.)")
+        return 1
+    if exts <= {"snf", "tsv"}:
+        return _main_combine(config, log)
     if exts != {"bam"} or len(config.input) != 1:
         log.error(f"Please specify a single .bam file as input: combine mode (.snf / .tsv) and CRAM input are not run by sniffles_b200 "
                   f"(supplied were: {sorted(exts)}) (Fatal error, exiting.)")

@@ -155,6 +155,17 @@ class CombineOut(C.Structure):                                  # snfb_combine_o
     _fields_ = [("cand_group", C.c_void_p), ("emit_chunk", C.c_void_p), ("emit_ord", C.c_void_p), ("cov_non", C.c_void_p)]
 
 
+class CombinePlanIn(C.Structure):                               # snfb_combine_plan_in
+    _fields_ = [("n_flat", C.c_uint32), ("n_task", C.c_uint32), ("task", C.c_void_p), ("row", C.c_void_p), ("svtype", C.c_void_p), ("support", C.c_void_p),
+                ("support_threshold", C.c_int32), ("bin_min_size", C.c_int32), ("bin_max_candidates", C.c_int32), ("exhaustive", C.c_int32),
+                ("group", CombineIn)]
+
+
+class CombinePlanOut(C.Structure):                              # snfb_combine_plan_out
+    _fields_ = [("n_cand", C.c_uint32), ("n_chain", C.c_uint32), ("n_chunk", C.c_uint32), ("pad", C.c_uint32),
+                ("perm", C.c_void_p), ("chains", C.c_void_p), ("chunks", C.c_void_p), ("group", CombineOut)]
+
+
 class GatherView(C.Structure):
     _fields_ = [("n_cand", C.c_uint64), ("cand", C.c_void_p), ("n_alt_bytes", C.c_uint64), ("alt", C.c_void_p),
                 ("n_rnames", C.c_uint64), ("rnames", C.c_void_p), ("rnames_off", C.c_void_p),

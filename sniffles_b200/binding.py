@@ -16,7 +16,7 @@ EXPORTS = ["snfb_version", "snfb_sizeof", "snfb_hash_name", "snfb_ctx_create", "
            "snfb_load_records", "snfb_extract_leads", "snfb_cluster_call", "snfb_consensus", "snfb_run",
            "snfb_last_timings", "snfb_device_candidates", "snfb_device_alt", "snfb_launch_count",
            "snfb_pin_host", "snfb_unpin_host", "snfb_pack_cigar16", "snfb_rerun_count", "snfb_coverage_bins",
-           "snfb_nccl_unique_id", "snfb_comm_init", "snfb_allgather_candidates", "snfb_selftest_sqrt_frac", "snfb_poa", "snfb_combine_groups", "snfb_selftest_edit_distance",
+           "snfb_nccl_unique_id", "snfb_comm_init", "snfb_allgather_candidates", "snfb_selftest_sqrt_frac", "snfb_poa", "snfb_combine_groups", "snfb_combine_plan", "snfb_selftest_edit_distance",
            "snfb_load_bam", "snfb_set_regions", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf", "snfb_deflate_bgzf",
            "snfb_genotype_targets", "snfb_load_reference", "snfb_reference_runs", "snfb_fetch_reference"]
 
@@ -68,6 +68,7 @@ def lib():
         L.snfb_reference_runs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
         L.snfb_fetch_reference.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
         L.snfb_combine_groups.argtypes = [C.c_void_p, C.POINTER(abi.CombineIn), C.POINTER(abi.CombineOut)]
+        L.snfb_combine_plan.argtypes = [C.c_void_p, C.POINTER(abi.CombinePlanIn), C.POINTER(abi.CombinePlanOut)]
         L.snfb_selftest_edit_distance.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
         L.snfb_selftest_sqrt_frac.restype = C.c_double
         L.snfb_selftest_sqrt_frac.argtypes = [C.c_uint64, C.c_uint64, C.c_uint64, C.c_int]
@@ -426,15 +427,37 @@ class Context:
         I.n_chain, I.n_chunk, I.n_cand, I.n_samples = len(a["chains"]), len(a["chunks"]), n, S
         for k in ("chains", "chunks", "pos", "svlen", "sample", "mate_contig", "mate_pos", "block_start", "cov"):
             setattr(I, k, a[k].ctypes.data)
-        I.n_cov_block, I.bins_per_block, I.cov_binsize = len(a["block_start"]), a["bins_per_block"], a["cov_binsize"]
-        I.combine_match, I.combine_match_max, I.cluster_merge_bnd = int(config.combine_match), int(config.combine_match_max), int(config.cluster_merge_bnd)
-        I.combine_separate_intra, I.combine_overlap_abs = int(bool(config.combine_separate_intra)), int(config.combine_overlap_abs)
-        I.combine_pctseq = float(getattr(config, "combine_pctseq", 0.0) or 0.0)
-        if I.combine_pctseq != 0.0:
-            I.alt, I.alt_off, I.alt_len, I.n_alt_bytes = a["alt"].ctypes.data, a["alt_off"].ctypes.data, a["alt_len"].ctypes.data, len(a["alt"])
+        _combine_params(I, a, config)
         O.cand_group, O.emit_chunk, O.emit_ord, O.cov_non = (x.ctypes.data for x in out)
         self._check(self._lib.snfb_combine_groups(self._h, C.byref(I), C.byref(O)), "snfb_combine_groups")
         return out
+
+    def combine_plan(self, flat, config):
+        """The chunk plan of combine mode and the grouping on the device (snfb_combine_plan).  flat: the columns of combine.FlatPass
+        (task, row, svtype, support, pos, svlen, sample, mate_contig, mate_pos, ALT arena, coverage tables) in the reference's iteration
+        order.  Returns a dict: perm (slot -> flat index), chains and chunks in plan_arrays' layout, and the four outputs of combine_groups."""
+        n = len(flat["pos"])
+        S = flat["n_samples"]
+        cap = max(n, 1)
+        perm, chains, chunks = np.zeros(cap, "<u4"), np.zeros((cap, 6), "<u4"), np.zeros((cap, 6), "<i4")
+        out = (np.zeros(cap, "<u4"), np.full(cap, -1, "<i4"), np.zeros(cap, "<u4"), np.full((cap, S), -1, "<i4"))
+        I, O = abi.CombinePlanIn(), abi.CombinePlanOut()
+        I.n_flat, I.n_task = n, flat["n_task"]
+        for k in ("task", "row", "svtype", "support"):
+            setattr(I, k, flat[k].ctypes.data)
+        I.support_threshold, I.bin_min_size = int(config.combine_support_threshold), int(config.combine_min_size)
+        I.bin_max_candidates, I.exhaustive = max(25, int(len(config.snf_input_info) * 0.5)), int(bool(config.combine_exhaustive))      # parallel.py:458
+        G = I.group
+        G.n_cand, G.n_samples = n, S
+        for k in ("pos", "svlen", "sample", "mate_contig", "mate_pos", "block_start", "cov"):
+            setattr(G, k, flat[k].ctypes.data)
+        _combine_params(G, flat, config)
+        O.perm, O.chains, O.chunks = perm.ctypes.data, chains.ctypes.data, chunks.ctypes.data
+        O.group.cand_group, O.group.emit_chunk, O.group.emit_ord, O.group.cov_non = (x.ctypes.data for x in out)
+        self._check(self._lib.snfb_combine_plan(self._h, C.byref(I), C.byref(O)), "snfb_combine_plan")
+        m = int(O.n_cand)
+        return dict(perm=perm[:m], chains=chains[:O.n_chain], chunks=chunks[:O.n_chunk], cand_group=out[0][:m], emit_chunk=out[1][:m], emit_ord=out[2][:m],
+                    cov_non=out[3][:m])
 
     def edit_distances(self, pairs):
         """device edit distance of (bytes, bytes) pairs (snfb_selftest_edit_distance)"""
@@ -462,3 +485,13 @@ class Context:
         n = C.c_uint64()
         self._check(self._lib.snfb_device_candidates(self._h, C.byref(p), C.byref(n)), "snfb_device_candidates")
         return p.value, int(n.value)
+
+
+def _combine_params(I, a, config):
+    """the coverage geometry, the grouping parameters and (with --combine-pctseq != 0) the ALT arena of an snfb_combine_in"""
+    I.n_cov_block, I.bins_per_block, I.cov_binsize = len(a["block_start"]), a["bins_per_block"], a["cov_binsize"]
+    I.combine_match, I.combine_match_max, I.cluster_merge_bnd = int(config.combine_match), int(config.combine_match_max), int(config.cluster_merge_bnd)
+    I.combine_separate_intra, I.combine_overlap_abs = int(bool(config.combine_separate_intra)), int(config.combine_overlap_abs)
+    I.combine_pctseq = float(getattr(config, "combine_pctseq", 0.0) or 0.0)
+    if I.combine_pctseq != 0.0:
+        I.alt, I.alt_off, I.alt_len, I.n_alt_bytes = a["alt"].ctypes.data, a["alt_off"].ctypes.data, a["alt_len"].ctypes.data, len(a["alt"])

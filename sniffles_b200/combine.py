@@ -131,6 +131,22 @@ def call_group(group: SVGroup, config, task):
     return call
 
 
+def coverage_rows(sblocks, block_index, config):
+    """[n_samples][bins_per_block] int32 of one block: each sample's `_COVERAGE` from the first part of its block (parallel.py:544-545),
+    -1 where the sample has no block or no such key.  sblocks: per sample in list order, its parts or None"""
+    step = config.coverage_binsize_combine
+    per_block = config.snf_block_size // step
+    rows = np.full((len(sblocks), per_block), -1, np.int32)
+    for si, parts in enumerate(sblocks):
+        if parts is None:
+            continue
+        for k, v in parts[0]["_COVERAGE"].items():
+            j = (int(k) - block_index) // step
+            if 0 <= j < per_block and (int(k) - block_index) % step == 0:
+                rows[si, j] = v
+    return rows
+
+
 @dataclass
 class Plan:
     """flat form of every chain of one or more tasks: what snfb_combine_groups reads"""
@@ -156,8 +172,6 @@ class CombineTask:
         bin_min = cfg.combine_min_size
         bin_max = max(25, int(len(cfg.snf_input_info) * 0.5))
         thr = cfg.combine_support_threshold
-        step = cfg.coverage_binsize_combine
-        per_block = cfg.snf_block_size // step
         ids = [s["internal_id"] for s in cfg.snf_input_info]
         per_type = {t: [] for t in TYPES}                        # chunks of each chain, in block order
         for bpos, block_index in enumerate(self.block_indices):
@@ -165,16 +179,8 @@ class CombineTask:
             if all(b is None for b in sblocks.values()):
                 continue
             cov_row = len(plan.cov_blocks)
-            rows = np.full((len(ids), per_block), -1, np.int32)
-            for si, sid in enumerate(ids):
-                if sblocks[sid] is None:
-                    continue
-                for k, v in sblocks[sid][0]["_COVERAGE"].items():        # the first part only (parallel.py:544-545)
-                    j = (int(k) - block_index) // step
-                    if 0 <= j < per_block and (int(k) - block_index) % step == 0:
-                        rows[si, j] = v
             plan.cov_blocks.append(block_index)
-            plan.cov_rows.append(rows)
+            plan.cov_rows.append(coverage_rows([sblocks[sid] for sid in ids], block_index, cfg))
             for t in TYPES:
                 bins = {}
                 for si, sid in enumerate(ids):
@@ -211,6 +217,19 @@ class CombineTask:
     @staticmethod
     def emit(tasks, plan: Plan, out):
         """out: (cand_group, emit_chunk, emit_ord, cov_non) from the device -> calls per task, in the reference's order"""
+        result = {}
+        for task_index, pairs in CombineTask.emit_batches(tasks, plan, out).items():
+            calls = [c for _, c in pairs]
+            if not getattr(tasks[task_index].config, "no_sort", False):
+                calls.sort(key=lambda c: c.pos)                     # CombineResult.store_calls / finalize (result.py:137-149)
+            result[task_index] = calls
+        return result
+
+    @staticmethod
+    def emit_batches(tasks, plan: Plan, out):
+        """out as for `emit` -> per task index, [(batch, call)] in the reference's emission order.  batch: the position of the block whose
+        iteration emits the call, which the reference stores as one result.store_calls batch (parallel.py:478-481, 568-569): the chunk's
+        block, or the task's last block for the groups kept to the end"""
         cand_group, emit_chunk, emit_ord, cov_non = out
         n_chunk = len(plan.chunks)
         members = {}
@@ -228,17 +247,16 @@ class CombineTask:
         result = {}
         for task_index, task in enumerate(tasks):
             ids = [s["internal_id"] for s in task.config.snf_input_info]
-            calls = []
+            last = len(task.block_indices) - 1
+            pairs = []
             for key, g in sorted(per_task.get(task_index, []), key=lambda kg: kg[0]):
                 cs = [plan.cands[i] for i in members[g]]
                 incl = set(c.sample_internal_id for c in cs)
                 cov = {sid: int(cov_non[g, si]) for si, sid in enumerate(ids) if sid not in incl}
                 call = call_group(SVGroup(cs, incl, cov), task.config, task)
                 if call is not None:
-                    calls.append(call)
-            if not getattr(task.config, "no_sort", False):
-                calls.sort(key=lambda c: c.pos)                     # CombineResult.store_calls / finalize (result.py:137-149)
-            result[task_index] = calls
+                    pairs.append((last if key[0] == 1 else key[1], call))
+            result[task_index] = pairs
         return result
 
     def execute(self, worker=None, readers=None, ctx=None):

@@ -178,6 +178,11 @@ _OPTIONS = [
     (("--combine-pctseq",), dict(type=float, default=0.7)),
     (("--combine-support-threshold",), dict(type=int, default=3)),
     (("--combine-consensus",), dict(action="store_true", default=False)),
+    (("--combine-max-inmemory-results",), dict(type=int, default=20)),
+    (("--combine-population",), dict(type=str, default=None)),
+    (("--re-qc",), dict(type=str, default="auto")),
+    (("--dev-skip-snf-validation",), dict(action="store_true", default=False)),
+    (("--dev-population-snf",), dict(type=str, default=None)),
     (("--dev-combine-medians",), dict(action="store_true", default=False)),
     (("--gpus",), dict(type=int, default=1)),          # new: number of GPUs to shard contigs over
 ]

@@ -259,7 +259,8 @@ size_t snfb_sizeof(int which) {
     switch (which) { case 0: return sizeof(snfb_rec); case 1: return sizeof(snfb_task); case 2: return sizeof(snfb_contig); case 3: return sizeof(snfb_records);
                      case 4: return sizeof(snfb_config); case 5: return sizeof(snfb_lead); case 6: return sizeof(snfb_cand); case 7: return sizeof(snfb_gather_view);
                      case 8: return sizeof(snfb_gt_in); case 9: return sizeof(snfb_gt_out);
-                     case 10: return sizeof(snfb_ref_contig); case 11: return sizeof(snfb_ref_input); case 12: return sizeof(snfb_ref_query); case 13: return sizeof(snfb_region); default: return 0; }
+                     case 10: return sizeof(snfb_ref_contig); case 11: return sizeof(snfb_ref_input); case 12: return sizeof(snfb_ref_query); case 13: return sizeof(snfb_region);
+                     case 14: return sizeof(snfb_combine_plan_in); case 15: return sizeof(snfb_combine_plan_out); default: return 0; }
 }
 
 uint64_t snfb_hash_name(const char* s, size_t n) {
@@ -1256,6 +1257,34 @@ int snfb_poa(snfb_ctx* ctx, const snfb_poa_job* jobs, uint32_t n_jobs, const uin
     return 0;
 }
 
+// k_combine over a plan whose inputs P already holds in device memory: carves the group state and the outputs, launches, copies the four
+// outputs to the host and synchronises
+static int combine_run_groups(snfb_ctx* ctx, const snfb_combine_in* in, combine::P& P, uint32_t n_chain, uint32_t n_chunk, size_t n, bool use_alt, uint32_t max_alt,
+                              DevBuf& b_state, DevBuf& b_out, const snfb_combine_out* out, const char* who) {
+    const size_t S = in->n_samples, W = (S + 31) / 32;
+    const unsigned blocks = (unsigned)std::min<size_t>((n_chain + 3) / 4, NUM_SMS * 4);
+    auto lay_state = [&](Carver& c) {
+        P.g_pos = c.take<double>(n); P.g_len = c.take<double>(n); P.g_mate = c.take<double>(n); P.g_n = c.take<uint32_t>(n); P.g_mc = c.take<int32_t>(n); P.g_incl = c.take<uint32_t>(n * W); P.act = c.take<uint32_t>(n);
+        P.next_chain = c.take<unsigned int>(4); P.g_first = c.take<uint32_t>(n); P.ex_stamp = c.take<uint32_t>(n); if (use_alt) P.hs = c.take<int8_t>((size_t)blocks * 4 * max_alt + 16);
+    };
+    auto lay_out = [&](Carver& c) { P.cand_group = c.take<uint32_t>(n); P.emit_chunk = c.take<int32_t>(n); P.emit_ord = c.take<uint32_t>(n); P.cov_non = c.take<int32_t>(n * S); };
+    if (carve(b_state, lay_state) || carve(b_out, lay_out)) return fail(ctx, std::string(who) + ": out of device memory");
+    P.n_chain = n_chain; P.n_chunk = n_chunk; P.n_cand = (uint32_t)n; P.n_samples = in->n_samples; P.words = (uint32_t)W;
+    P.bins_per_block = in->bins_per_block; P.cov_binsize = in->cov_binsize;
+    P.combine_match = in->combine_match; P.combine_match_max = in->combine_match_max; P.cluster_merge_bnd = in->cluster_merge_bnd; P.separate_intra = in->combine_separate_intra; P.overlap_abs = in->combine_overlap_abs;
+    P.pctseq = use_alt ? in->combine_pctseq : 0.0; P.max_alt = max_alt;
+    cudaStream_t st = ctx->st;
+    CUDA_TRY(cudaMemsetAsync(P.next_chain, 0, 16, st));
+    mark(ctx, "combine_groups");
+    launch(ctx->launches, combine::k_combine, blocks, 128, 0, st, P);
+    mark(ctx, nullptr);
+    CUDA_TRY(cudaMemcpyAsync(out->cand_group, P.cand_group, 4 * n, cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaMemcpyAsync(out->emit_chunk, P.emit_chunk, 4 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->emit_ord, P.emit_ord, 4 * n, cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaMemcpyAsync(out->cov_non, P.cov_non, 4 * n * S, cudaMemcpyDeviceToHost, st));
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, std::string(who) + ": " + cudaGetErrorString(e));
+    return 0;
+}
+
 // multi-sample combine: every (task, svtype) chain of the plan by one warp (combine.cuh); host buffers in, host buffers out
 int snfb_combine_groups(snfb_ctx* ctx, const snfb_combine_in* in, snfb_combine_out* out) {
     if (!ctx || !in || !out) return ctx ? fail(ctx, "snfb_combine_groups: null argument") : 1;
@@ -1276,12 +1305,11 @@ int snfb_combine_groups(snfb_ctx* ctx, const snfb_combine_in* in, snfb_combine_o
       if (c != in->n_cand || k != in->n_chunk) return fail(ctx, "snfb_combine_groups: plan does not cover n_cand / n_chunk");
       for (uint32_t i = 0; i < in->n_cand; ++i) if (in->sample[i] >= in->n_samples) return fail(ctx, "snfb_combine_groups: sample index out of range"); }
     cudaSetDevice(ctx->device);
-    const size_t n = in->n_cand, S = in->n_samples, W = (S + 31) / 32, ncov = (size_t)in->n_cov_block * S * in->bins_per_block;
+    const size_t n = in->n_cand, S = in->n_samples, ncov = (size_t)in->n_cov_block * S * in->bins_per_block;
     const bool use_alt = in->combine_pctseq != 0.0 && in->alt && in->alt_off && in->alt_len;
     uint32_t max_alt = 16;
     if (use_alt) for (uint32_t i = 0; i < in->n_cand; ++i) { if (in->alt_off[i] + in->alt_len[i] > in->n_alt_bytes) return fail(ctx, "snfb_combine_groups: ALT outside alt[]"); max_alt = std::max(max_alt, in->alt_len[i]); }
     max_alt = (max_alt + 15u) & ~15u;
-    const unsigned blocks = (unsigned)std::min<size_t>((in->n_chain + 3) / 4, NUM_SMS * 4);
     // inputs in one buffer, group state in one, outputs in one
     DevBuf b_in, b_state, b_out;
     combine::P P{};
@@ -1290,30 +1318,111 @@ int snfb_combine_groups(snfb_ctx* ctx, const snfb_combine_in* in, snfb_combine_o
         P.mate_contig = c.take<int32_t>(n); P.mate_pos = c.take<int32_t>(n); P.block_start = c.take<long long>(in->n_cov_block + 1); P.cov = c.take<int32_t>(ncov + 1);
         if (use_alt) { P.alt = c.take<uint8_t>(in->n_alt_bytes + 16); P.alt_off = c.take<unsigned long long>(n); P.alt_len = c.take<uint32_t>(n); }
     };
-    auto lay_state = [&](Carver& c) {
-        P.g_pos = c.take<double>(n); P.g_len = c.take<double>(n); P.g_mate = c.take<double>(n); P.g_n = c.take<uint32_t>(n); P.g_mc = c.take<int32_t>(n); P.g_incl = c.take<uint32_t>(n * W); P.act = c.take<uint32_t>(n);
-        P.next_chain = c.take<unsigned int>(4); P.g_first = c.take<uint32_t>(n); P.ex_stamp = c.take<uint32_t>(n); if (use_alt) P.hs = c.take<int8_t>((size_t)blocks * 4 * max_alt + 16);
-    };
-    auto lay_out = [&](Carver& c) { P.cand_group = c.take<uint32_t>(n); P.emit_chunk = c.take<int32_t>(n); P.emit_ord = c.take<uint32_t>(n); P.cov_non = c.take<int32_t>(n * S); };
-    if (carve(b_in, lay_in) || carve(b_state, lay_state) || carve(b_out, lay_out)) return fail(ctx, "snfb_combine_groups: out of device memory");
-    P.n_chain = in->n_chain; P.n_chunk = in->n_chunk; P.n_cand = in->n_cand; P.n_samples = in->n_samples; P.words = (uint32_t)W;
-    P.bins_per_block = in->bins_per_block; P.cov_binsize = in->cov_binsize;
-    P.combine_match = in->combine_match; P.combine_match_max = in->combine_match_max; P.cluster_merge_bnd = in->cluster_merge_bnd; P.separate_intra = in->combine_separate_intra; P.overlap_abs = in->combine_overlap_abs;
+    if (carve(b_in, lay_in)) return fail(ctx, "snfb_combine_groups: out of device memory");
     cudaStream_t st = ctx->st;
     auto up = [&](const void* dst, const void* src, size_t bytes) { if (bytes && src) CUDA_TRY(cudaMemcpyAsync(const_cast<void*>(dst), src, bytes, cudaMemcpyHostToDevice, st)); return 0; };
     if (up(P.chains, in->chains, sizeof(snfb_combine_chain) * in->n_chain) || up(P.chunks, in->chunks, sizeof(snfb_combine_chunk) * in->n_chunk)
         || up(P.pos, in->pos, 4 * n) || up(P.svlen, in->svlen, 4 * n) || up(P.sample, in->sample, 4 * n) || up(P.mate_contig, in->mate_contig, 4 * n) || up(P.mate_pos, in->mate_pos, 4 * n)
         || up(P.block_start, in->block_start, 8 * (size_t)in->n_cov_block) || up(P.cov, in->cov, 4 * ncov)) return 1;
-    P.pctseq = use_alt ? in->combine_pctseq : 0.0; P.max_alt = max_alt;
     if (use_alt && (up(P.alt, in->alt, in->n_alt_bytes) || up(P.alt_off, in->alt_off, 8 * n) || up(P.alt_len, in->alt_len, 4 * n))) return 1;
-    CUDA_TRY(cudaMemsetAsync(P.next_chain, 0, 16, st));
-    mark(ctx, "combine_groups");
-    launch(ctx->launches, combine::k_combine, blocks, 128, 0, st, P);
+    return combine_run_groups(ctx, in, P, in->n_chain, in->n_chunk, in->n_cand, use_alt, max_alt, b_state, b_out, out, "snfb_combine_groups");
+}
+
+// the chunk plan on the device (combine.cuh k_plan_*), then the grouping over the tables it left in device memory
+int snfb_combine_plan(snfb_ctx* ctx, const snfb_combine_plan_in* in, snfb_combine_plan_out* out) {
+    if (!ctx || !in || !out) return ctx ? fail(ctx, "snfb_combine_plan: null argument") : 1;
+    const snfb_combine_in& g = in->group;
+    const uint32_t nf = in->n_flat;
+    out->n_cand = out->n_chain = out->n_chunk = 0;
+    if (nf == 0) return 0;
+    if (!in->task || !in->row || !in->svtype || !in->support || !g.pos || !g.svlen || !g.sample || !g.mate_contig || !g.mate_pos || !out->perm || !out->chains || !out->chunks
+        || !out->group.cand_group || !out->group.emit_chunk || !out->group.emit_ord || !out->group.cov_non) return fail(ctx, "snfb_combine_plan: null array");
+    if (g.n_samples == 0 || g.bins_per_block <= 0 || g.cov_binsize <= 0) return fail(ctx, "snfb_combine_plan: bad sample count / coverage geometry");
+    if (in->n_task == 0 || in->n_task > (1u << 24) || in->bin_min_size <= 0 || in->bin_max_candidates <= 0) return fail(ctx, "snfb_combine_plan: bad task count / bin sizes");
+    for (uint32_t i = 0; i < nf; ++i)
+        if (in->task[i] >= in->n_task || in->row[i] >= g.n_cov_block || in->svtype[i] < 0 || in->svtype[i] > 4 || g.sample[i] >= g.n_samples)
+            return fail(ctx, "snfb_combine_plan: candidate " + std::to_string(i) + " has a task, row, svtype or sample out of range");
+    const size_t S = g.n_samples, ncov = (size_t)g.n_cov_block * S * g.bins_per_block;
+    const bool use_alt = g.combine_pctseq != 0.0 && g.alt && g.alt_off && g.alt_len;
+    uint32_t max_alt = 16;
+    if (use_alt) for (uint32_t i = 0; i < nf; ++i) { if (g.alt_off[i] + g.alt_len[i] > g.n_alt_bytes) return fail(ctx, "snfb_combine_plan: ALT outside alt[]"); max_alt = std::max(max_alt, g.alt_len[i]); }
+    max_alt = (max_alt + 15u) & ~15u;
+    cudaSetDevice(ctx->device);
+    cudaStream_t st = ctx->st;
+    ctx->n_ev = 0;
+    // flat columns, the sort and plan scratch, then the slot-ordered columns and the tables k_combine reads
+    DevBuf b_in, b_plan, b_state, b_out;
+    const uint32_t *f_task, *f_row, *f_sample; const int32_t *f_svtype, *f_support, *f_pos, *f_svlen, *f_mc, *f_mp; const unsigned long long* f_alt_off = nullptr; const uint32_t* f_alt_len = nullptr;
+    uint64_t *k0, *k1; uint32_t *v0, *v1, *keep, *at, *seg_head, *seg_id, *chain_head, *chain_id, *seg_start, *seg_nchunk, *chunk_off, *chunk_of, *scan_tmp; unsigned long long* tot;
+    prims::RadixTemp rt{};
+    combine::P P{};
+    auto lay_in = [&](Carver& c) {
+        f_task = c.take<uint32_t>(nf); f_row = c.take<uint32_t>(nf); f_svtype = c.take<int32_t>(nf); f_support = c.take<int32_t>(nf); f_pos = c.take<int32_t>(nf); f_svlen = c.take<int32_t>(nf);
+        f_sample = c.take<uint32_t>(nf); f_mc = c.take<int32_t>(nf); f_mp = c.take<int32_t>(nf); P.block_start = c.take<long long>(g.n_cov_block + 1); P.cov = c.take<int32_t>(ncov + 1);
+        if (use_alt) { P.alt = c.take<uint8_t>(g.n_alt_bytes + 16); f_alt_off = c.take<unsigned long long>(nf); f_alt_len = c.take<uint32_t>(nf); }
+    };
+    auto lay_plan = [&](Carver& c) {
+        k0 = c.take<uint64_t>(nf); k1 = c.take<uint64_t>(nf); v0 = c.take<uint32_t>(nf); v1 = c.take<uint32_t>(nf); keep = c.take<uint32_t>(nf); at = c.take<uint32_t>(nf);
+        seg_head = c.take<uint32_t>(nf); seg_id = c.take<uint32_t>(nf); chain_head = c.take<uint32_t>(nf); chain_id = c.take<uint32_t>(nf); seg_start = c.take<uint32_t>(nf);
+        seg_nchunk = c.take<uint32_t>(nf); chunk_off = c.take<uint32_t>(nf); chunk_of = c.take<uint32_t>(nf); tot = c.take<unsigned long long>(4);
+        scan_tmp = c.take<uint32_t>(prims::scan_tmp_elems(std::max<unsigned long long>(nf, prims::radix_hist_elems(nf))));
+        rt.hist = c.take<uint32_t>(prims::radix_hist_elems(nf)); rt.scan_tmp = scan_tmp;
+        P.chains = c.take<snfb_combine_chain>(nf); P.chunks = c.take<snfb_combine_chunk>(nf);
+        P.pos = c.take<int32_t>(nf); P.svlen = c.take<int32_t>(nf); P.sample = c.take<uint32_t>(nf); P.mate_contig = c.take<int32_t>(nf); P.mate_pos = c.take<int32_t>(nf);
+        if (use_alt) { P.alt_off = c.take<unsigned long long>(nf); P.alt_len = c.take<uint32_t>(nf); }
+    };
+    if (carve(b_in, lay_in) || carve(b_plan, lay_plan)) return fail(ctx, "snfb_combine_plan: out of device memory");
+    auto up = [&](const void* dst, const void* src, size_t bytes) { if (bytes && src) CUDA_TRY(cudaMemcpyAsync(const_cast<void*>(dst), src, bytes, cudaMemcpyHostToDevice, st)); return 0; };
+    if (up(f_task, in->task, 4 * (size_t)nf) || up(f_row, in->row, 4 * (size_t)nf) || up(f_svtype, in->svtype, 4 * (size_t)nf) || up(f_support, in->support, 4 * (size_t)nf)
+        || up(f_pos, g.pos, 4 * (size_t)nf) || up(f_svlen, g.svlen, 4 * (size_t)nf) || up(f_sample, g.sample, 4 * (size_t)nf) || up(f_mc, g.mate_contig, 4 * (size_t)nf) || up(f_mp, g.mate_pos, 4 * (size_t)nf)
+        || up(P.block_start, g.block_start, 8 * (size_t)g.n_cov_block) || up(P.cov, g.cov, 4 * ncov)) return 1;
+    if (use_alt && (up(P.alt, g.alt, g.n_alt_bytes) || up(f_alt_off, g.alt_off, 8 * (size_t)nf) || up(f_alt_len, g.alt_len, 4 * (size_t)nf))) return 1;
+    // three counts come back to the host (kept candidates, segments and chains, chunks): they size the launches that follow
+    uint64_t h_tot[4];
+    auto counts = [&]() -> int { CUDA_TRY(cudaMemcpyAsync(h_tot, tot, 32, cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st)); return 0; };
+    auto sort = [&](int bits, uint64_t*& k, uint32_t*& v) {
+        uint64_t* ka = k; uint32_t* va = v; uint64_t* kb = k == k0 ? k1 : k0; uint32_t* vb = v == v0 ? v1 : v0; bool in_first = true;
+        prims::radix_sort(ctx->launches, ka, va, kb, vb, rt, tot, nf, bits, &in_first, st);
+        if (!in_first) { k = kb; v = vb; }
+    };
+    mark(ctx, "combine_plan");
+    CUDA_TRY(cudaMemsetAsync(tot, 0, 32, st));
+    launch(ctx->launches, combine::k_plan_keep, grid_for(nf, 256), 256, 0, st, f_support, nf, in->support_threshold, keep);
+    prims::exclusive_scan(ctx->launches, keep, at, scan_tmp, nullptr, nf, tot, st);
+    launch(ctx->launches, combine::k_plan_compact, grid_for(nf, 256), 256, 0, st, keep, at, nf, f_pos, in->bin_min_size, k0, v0);
+    if (counts()) return 1;
+    const uint32_t n = (uint32_t)h_tot[0];
+    if (n == 0) { mark(ctx, nullptr); return 0; }
+    uint64_t* K = k0; uint32_t* V = v0;
+    sort(32, K, V);                                                                   // by bin ...
+    launch(ctx->launches, combine::k_plan_segkey, grid_for(n, 256), 256, 0, st, V, n, f_task, f_svtype, f_row, K);
+    sort(35 + bits_for(in->n_task), K, V);                                            // ... then stably by (task, svtype, block)
+    launch(ctx->launches, combine::k_plan_heads, grid_for(n, 256), 256, 0, st, K, n, seg_head, chain_head);
+    prims::exclusive_scan(ctx->launches, seg_head, seg_id, scan_tmp, nullptr, n, tot + 1, st);
+    prims::exclusive_scan(ctx->launches, chain_head, chain_id, scan_tmp, nullptr, n, tot + 2, st);
+    launch(ctx->launches, combine::k_plan_seg_start, grid_for(n, 256), 256, 0, st, seg_head, seg_id, n, seg_start);
+    if (counts()) return 1;
+    const uint32_t n_seg = (uint32_t)h_tot[1], n_chain = (uint32_t)h_tot[2];
+    launch(ctx->launches, combine::k_plan_cut, grid_for(n_seg, 128), 128, 0, st, seg_start, n_seg, n, V, f_pos, K, in->bin_min_size, in->bin_max_candidates, in->exhaustive,
+           seg_nchunk, (const uint32_t*)nullptr, (snfb_combine_chunk*)nullptr, (uint32_t*)nullptr);
+    prims::exclusive_scan(ctx->launches, seg_nchunk, chunk_off, scan_tmp, nullptr, n_seg, tot + 3, st);
+    launch(ctx->launches, combine::k_plan_cut, grid_for(n_seg, 128), 128, 0, st, seg_start, n_seg, n, V, f_pos, K, in->bin_min_size, in->bin_max_candidates, in->exhaustive,
+           seg_nchunk, (const uint32_t*)chunk_off, const_cast<snfb_combine_chunk*>(P.chunks), chunk_of);
+    launch(ctx->launches, combine::k_plan_chains, grid_for(n, 256), 256, 0, st, chain_head, chain_id, K, chunk_of, n, const_cast<snfb_combine_chain*>(P.chains));
+    if (counts()) return 1;
+    const uint32_t n_chunk = (uint32_t)h_tot[3];
+    launch(ctx->launches, combine::k_plan_chain_len, grid_for(n_chain, 256), 256, 0, st, const_cast<snfb_combine_chain*>(P.chains), n_chain, n, n_chunk);
+    launch(ctx->launches, combine::k_plan_supkey, grid_for(n, 256), 256, 0, st, V, chunk_of, n, f_support, K);
+    sort(32 + bits_for(n_chunk), K, V);                                               // support, descending, inside each chunk
+    launch(ctx->launches, combine::k_plan_gather, grid_for(n, 256), 256, 0, st, V, n, f_pos, f_svlen, f_sample, f_mc, f_mp, f_alt_off, f_alt_len,
+           const_cast<int32_t*>(P.pos), const_cast<int32_t*>(P.svlen), const_cast<uint32_t*>(P.sample), const_cast<int32_t*>(P.mate_contig), const_cast<int32_t*>(P.mate_pos),
+           const_cast<unsigned long long*>(P.alt_off), const_cast<uint32_t*>(P.alt_len));
     mark(ctx, nullptr);
-    CUDA_TRY(cudaMemcpyAsync(out->cand_group, P.cand_group, 4 * n, cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaMemcpyAsync(out->emit_chunk, P.emit_chunk, 4 * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(out->emit_ord, P.emit_ord, 4 * n, cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaMemcpyAsync(out->cov_non, P.cov_non, 4 * n * S, cudaMemcpyDeviceToHost, st));
-    const cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return fail(ctx, std::string("snfb_combine_groups: ") + cudaGetErrorString(e));
+    CUDA_TRY(cudaMemcpyAsync(out->perm, V, 4 * (size_t)n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->chains, P.chains, sizeof(snfb_combine_chain) * n_chain, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->chunks, P.chunks, sizeof(snfb_combine_chunk) * n_chunk, cudaMemcpyDeviceToHost, st));
+    if (combine_run_groups(ctx, &g, P, n_chain, n_chunk, n, use_alt, max_alt, b_state, b_out, &out->group, "snfb_combine_plan")) return 1;
+    out->n_cand = n; out->n_chain = n_chain; out->n_chunk = n_chunk;
     return 0;
 }
 

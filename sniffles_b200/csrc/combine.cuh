@@ -195,6 +195,95 @@ __global__ void __launch_bounds__(128) k_combine(const P p) {
     }
 }
 
+// ---- the chunk plan (parallel.py:484-527) over flat candidates, for snfb_combine_plan ----
+// Flat candidates come in the reference's iteration order (task, block, svtype, sample, part, list position).  The kept ones are sorted
+// stably on (task, svtype, block, bin) by two LSD radix sorts (bin first): within one (task, block, svtype) segment that is the order in
+// which the reference's bins dict hands them out.  One thread per segment then cuts the chunks, and a third stable sort on (chunk, support
+// descending) gives each chunk the order of sorted(key=support, reverse=True) (cluster.py:361).  Segments of one (task, svtype) are
+// consecutive after the sort: they form that chain.
+
+// int(pos / bin_min) * bin_min: C's integer division truncates toward zero as int() does, and the double quotient of two int32 values
+// lies at least 1 / bin_min from any integer it is not equal to, far more than its rounding error, so both truncate alike
+__device__ __forceinline__ int32_t plan_bin(int32_t pos, int32_t bin_min) { return (pos / bin_min) * bin_min; }
+__device__ __forceinline__ uint32_t biased(int32_t v) { return (uint32_t)v ^ 0x80000000u; }      // signed order as unsigned order
+
+__global__ void k_plan_keep(const int32_t* __restrict__ support, uint32_t n, int32_t thr, uint32_t* __restrict__ keep) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) keep[i] = support[i] >= thr ? 1u : 0u;
+}
+// the kept candidates, in flat order, keyed by their bin
+__global__ void k_plan_compact(const uint32_t* __restrict__ keep, const uint32_t* __restrict__ at, uint32_t n, const int32_t* __restrict__ pos, int32_t bin_min,
+                               uint64_t* __restrict__ key, uint32_t* __restrict__ val) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        if (keep[i]) { key[at[i]] = biased(plan_bin(pos[i], bin_min)); val[at[i]] = i; }
+}
+// (task, svtype, coverage row): rows are numbered in (task, block) order, so the row orders the blocks of a task
+__global__ void k_plan_segkey(const uint32_t* __restrict__ val, uint32_t n, const uint32_t* __restrict__ task, const int32_t* __restrict__ svtype,
+                              const uint32_t* __restrict__ row, uint64_t* __restrict__ key) {
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+        const uint32_t v = val[j]; key[j] = ((uint64_t)task[v] << 35) | ((uint64_t)svtype[v] << 32) | row[v];
+    }
+}
+// first position of each segment (same key) and of each chain (same task and svtype)
+__global__ void k_plan_heads(const uint64_t* __restrict__ key, uint32_t n, uint32_t* __restrict__ seg_head, uint32_t* __restrict__ chain_head) {
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+        seg_head[j] = (j == 0 || key[j] != key[j - 1]) ? 1u : 0u;
+        chain_head[j] = (j == 0 || (key[j] >> 32) != (key[j - 1] >> 32)) ? 1u : 0u;
+    }
+}
+__global__ void k_plan_seg_start(const uint32_t* __restrict__ seg_head, const uint32_t* __restrict__ seg_id, uint32_t n, uint32_t* __restrict__ seg_start) {
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) if (seg_head[j]) seg_start[seg_id[j]] = j;
+}
+// the chunk cut of one segment (parallel.py:518-527): bins are added whole; a chunk closes once it holds bin_max candidates (unless
+// exhaustive) or at the segment's last bin.  Without chunk_off it counts the chunks of each segment; with it, it writes them and the chunk
+// of every position.
+__global__ void k_plan_cut(const uint32_t* __restrict__ seg_start, uint32_t n_seg, uint32_t n, const uint32_t* __restrict__ val, const int32_t* __restrict__ pos,
+                           const uint64_t* __restrict__ key, int32_t bin_min, int32_t bin_max, int exhaustive, uint32_t* __restrict__ seg_nchunk,
+                           const uint32_t* __restrict__ chunk_off, snfb_combine_chunk* __restrict__ chunks, uint32_t* __restrict__ chunk_of) {
+    for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n_seg; s += gridDim.x * blockDim.x) {
+        const uint32_t b = seg_start[s], e = s + 1 < n_seg ? seg_start[s + 1] : n;
+        uint32_t k = chunk_off ? chunk_off[s] : 0u, nk = 0, c0 = b, nbins = 0;
+        for (uint32_t j = b; j < e; ++j) {
+            const int32_t bin = plan_bin(pos[val[j]], bin_min);
+            if (j + 1 < e && plan_bin(pos[val[j + 1]], bin_min) == bin) continue;
+            ++nbins;
+            if ((!exhaustive && (int64_t)(j + 1 - c0) >= bin_max) || j + 1 == e) {
+                if (chunk_off) {
+                    chunks[k + nk] = snfb_combine_chunk{ (int32_t)c0, (int32_t)(j + 1 - c0), bin, (int32_t)(nbins * (uint32_t)bin_min), (int32_t)(uint32_t)key[b], 0 };
+                    for (uint32_t q = c0; q <= j; ++q) chunk_of[q] = k + nk;
+                }
+                ++nk; c0 = j + 1; nbins = 0;
+            }
+        }
+        if (!chunk_off) seg_nchunk[s] = nk;
+    }
+}
+__global__ void k_plan_chains(const uint32_t* __restrict__ chain_head, const uint32_t* __restrict__ chain_id, const uint64_t* __restrict__ key, const uint32_t* __restrict__ chunk_of,
+                              uint32_t n, snfb_combine_chain* __restrict__ chains) {
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x)
+        if (chain_head[j]) chains[chain_id[j]] = snfb_combine_chain{ j, 0u, chunk_of[j], 0u, ((key[j] >> 32) & 7u) == 4u ? 1u : 0u, 0u };   // 4: BND
+}
+__global__ void k_plan_chain_len(snfb_combine_chain* __restrict__ chains, uint32_t n_chain, uint32_t n, uint32_t n_chunk) {
+    for (uint32_t c = blockIdx.x * blockDim.x + threadIdx.x; c < n_chain; c += gridDim.x * blockDim.x) {
+        chains[c].n_cand = (c + 1 < n_chain ? chains[c + 1].cand_off : n) - chains[c].cand_off;
+        chains[c].n_chunk = (c + 1 < n_chain ? chains[c + 1].chunk_off : n_chunk) - chains[c].chunk_off;
+    }
+}
+// (chunk, support descending): a stable sort on it is sorted(chunk, key=support, reverse=True) inside every chunk
+__global__ void k_plan_supkey(const uint32_t* __restrict__ val, const uint32_t* __restrict__ chunk_of, uint32_t n, const int32_t* __restrict__ support, uint64_t* __restrict__ key) {
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) key[j] = ((uint64_t)chunk_of[j] << 32) | (0xffffffffu - biased(support[val[j]]));
+}
+// the per-candidate columns of k_combine, in slot order
+__global__ void k_plan_gather(const uint32_t* __restrict__ val, uint32_t n, const int32_t* __restrict__ pos, const int32_t* __restrict__ svlen, const uint32_t* __restrict__ sample,
+                              const int32_t* __restrict__ mate_contig, const int32_t* __restrict__ mate_pos, const unsigned long long* __restrict__ alt_off, const uint32_t* __restrict__ alt_len,
+                              int32_t* __restrict__ o_pos, int32_t* __restrict__ o_svlen, uint32_t* __restrict__ o_sample, int32_t* __restrict__ o_mc, int32_t* __restrict__ o_mp,
+                              unsigned long long* __restrict__ o_alt_off, uint32_t* __restrict__ o_alt_len) {
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+        const uint32_t v = val[j];
+        o_pos[j] = pos[v]; o_svlen[j] = svlen[v]; o_sample[j] = sample[v]; o_mc[j] = mate_contig[v]; o_mp[j] = mate_pos[v];
+        if (alt_off) { o_alt_off[j] = alt_off[v]; o_alt_len[j] = alt_len[v]; }
+    }
+}
+
 // self-check: one warp per pair
 __global__ void k_edit_selftest(const uint8_t* bytes, const unsigned long long* a_off, const uint32_t* a_len, const unsigned long long* b_off, const uint32_t* b_len, uint32_t n_pairs, int8_t* hs, uint32_t max_len, int* out) {
     const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
