@@ -306,7 +306,8 @@ typedef struct snfb_ctx snfb_ctx;
 
 int         snfb_version(void);
 /* sizeof of the ABI structs, for binding self-checks: 0 rec, 1 task, 2 contig, 3 records, 4 config, 5 lead, 6 cand, 7 gather_view,
- * 8 gt_in, 9 gt_out, 10 ref_contig, 11 ref_input, 12 ref_query, 13 region, 14 combine_plan_in, 15 combine_plan_out */
+ * 8 gt_in, 9 gt_out, 10 ref_contig, 11 ref_input, 12 ref_query, 13 region, 14 combine_plan_in, 15 combine_plan_out, 16 pop_table,
+ * 17 pop_query */
 size_t      snfb_sizeof(int which);
 uint64_t    snfb_hash_name(const char* s, size_t n);
 int         snfb_ctx_create(int device, snfb_ctx** out);
@@ -521,6 +522,36 @@ typedef struct snfb_combine_plan_out {
     snfb_combine_out group;
 } snfb_combine_plan_out;
 int         snfb_combine_plan(snfb_ctx* ctx, const snfb_combine_plan_in* in, snfb_combine_plan_out* out);
+/* ---- population allele frequencies of combined calls (--combine-population, snfp.py) ----
+ * snfb_population_load  <- PopulationSNF.open + get_all_blocks (sniffles:433-435, parallel.py:454-455, snf.py:235-243): the variants of a
+ *                          population SNF, in file order, each with its contig index (-1 when the name is not among the run's contigs; such
+ *                          a variant is never matched), the start of the block it is stored under (the index key, not recomputed from pos),
+ *                          svtype 0..4 (INS DEL DUP INV BND), pos, svlen and its ALT bytes alt[alt_off[i] .. + alt_len[i]).  Only the
+ *                          first part of a block is given, as get_all_blocks reads only read_blocks(...)[0].  The table is keyed on the
+ *                          device, sorted stably on (contig, block, svtype) and stays resident on the context until the next load, which
+ *                          replaces it, or snfb_ctx_destroy.  Timing mark: population_load.
+ * snfb_population_match <- PopulationSNF.get_population_AF (snfp.py:131-155) with PopulationVariant.match (snfp.py:91-107) for one batch of
+ *                          calls (contig index or -1, svtype, pos, svlen, ALT bytes): the call's list is the variants of key (contig,
+ *                          int(pos / block_size) * block_size, svtype); a variant matches when dist = |pos_p - pos_c| + ||svlen_p| -
+ *                          |svlen_c|| <= combine_match * sqrt(min(|svlen_p|, |svlen_c|)) and dist <= combine_match_max, and, for INS with
+ *                          combine_pctseq != 0, (svlen_p - editDistance(ALT_p, ALT_c)) / svlen_p > combine_pctseq (edlib.align defaults).
+ *                          best[q] = the file-order index of the variant with the strictly smallest distance, ties to the earlier one in
+ *                          list order; -1 when none matches; -2 when an INS variant with svlen_p == 0 reaches the alignment test, where the
+ *                          reference divides by zero.  Timing mark: population_match. */
+typedef struct snfb_pop_table {
+    uint32_t n, pad;
+    const int32_t* contig; const int32_t* block; const int32_t* svtype; const int32_t* pos; const int32_t* svlen;
+    const uint8_t* alt; const uint64_t* alt_off; const uint32_t* alt_len; uint64_t n_alt_bytes;
+} snfb_pop_table;
+typedef struct snfb_pop_query {
+    uint32_t n, pad;
+    const int32_t* contig; const int32_t* svtype; const int32_t* pos; const int32_t* svlen;
+    const uint8_t* alt; const uint64_t* alt_off; const uint32_t* alt_len; uint64_t n_alt_bytes;
+    int32_t combine_match, combine_match_max, block_size, pad2;
+    double  combine_pctseq;
+} snfb_pop_query;
+int         snfb_population_load(snfb_ctx* ctx, const snfb_pop_table* in);
+int         snfb_population_match(snfb_ctx* ctx, const snfb_pop_query* in, int32_t* best);
 /* self-check of the exact statistics.stdev arithmetic (host build of the routine the kernels use): the correctly rounded sqrt(P / Q) for
  * P = p_hi * 2^64 + p_lo; slow != 0 selects the limb-by-limb restatement of CPython's _float_sqrt_of_frac, 0 the verified fast path */
 double      snfb_selftest_sqrt_frac(uint64_t p_hi, uint64_t p_lo, uint64_t q, int slow);

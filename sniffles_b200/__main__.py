@@ -70,8 +70,8 @@ def _main_combine(config, log):
         refusal = f"combine mode (.snf / .tsv input) runs on one GPU: run it without torchrun ({world} ranks would each write {config.vcf})"
     elif config.combine_consensus:
         refusal = "--combine-consensus is not supported: the reference's SVGroup.call cannot run with it either (sv.py:387)"
-    elif config.combine_population is not None or config.dev_population_snf is not None:
-        refusal = "--combine-population and --dev-population-snf (population SNFs, allele frequencies) are not supported by sniffles_b200"
+    elif config.dev_population_snf is not None:
+        refusal = "--dev-population-snf: writing a population SNF is not supported by sniffles_b200; --combine-population reads one"
     if refusal is not None:
         log.error(f"{refusal} (Fatal error, exiting.)")
         return 1

@@ -166,6 +166,18 @@ class CombinePlanOut(C.Structure):                              # snfb_combine_p
                 ("perm", C.c_void_p), ("chains", C.c_void_p), ("chunks", C.c_void_p), ("group", CombineOut)]
 
 
+class PopTable(C.Structure):                                    # snfb_pop_table
+    _fields_ = [("n", C.c_uint32), ("pad", C.c_uint32), ("contig", C.c_void_p), ("block", C.c_void_p), ("svtype", C.c_void_p), ("pos", C.c_void_p),
+                ("svlen", C.c_void_p), ("alt", C.c_void_p), ("alt_off", C.c_void_p), ("alt_len", C.c_void_p), ("n_alt_bytes", C.c_uint64)]
+
+
+class PopQuery(C.Structure):                                    # snfb_pop_query
+    _fields_ = [("n", C.c_uint32), ("pad", C.c_uint32), ("contig", C.c_void_p), ("svtype", C.c_void_p), ("pos", C.c_void_p), ("svlen", C.c_void_p),
+                ("alt", C.c_void_p), ("alt_off", C.c_void_p), ("alt_len", C.c_void_p), ("n_alt_bytes", C.c_uint64),
+                ("combine_match", C.c_int32), ("combine_match_max", C.c_int32), ("block_size", C.c_int32), ("pad2", C.c_int32),
+                ("combine_pctseq", C.c_double)]
+
+
 class GatherView(C.Structure):
     _fields_ = [("n_cand", C.c_uint64), ("cand", C.c_void_p), ("n_alt_bytes", C.c_uint64), ("alt", C.c_void_p),
                 ("n_rnames", C.c_uint64), ("rnames", C.c_void_p), ("rnames_off", C.c_void_p),

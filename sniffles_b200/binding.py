@@ -18,7 +18,8 @@ EXPORTS = ["snfb_version", "snfb_sizeof", "snfb_hash_name", "snfb_ctx_create", "
            "snfb_pin_host", "snfb_unpin_host", "snfb_pack_cigar16", "snfb_rerun_count", "snfb_coverage_bins",
            "snfb_nccl_unique_id", "snfb_comm_init", "snfb_allgather_candidates", "snfb_selftest_sqrt_frac", "snfb_poa", "snfb_combine_groups", "snfb_combine_plan", "snfb_selftest_edit_distance",
            "snfb_load_bam", "snfb_set_regions", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf", "snfb_deflate_bgzf",
-           "snfb_genotype_targets", "snfb_load_reference", "snfb_reference_runs", "snfb_fetch_reference"]
+           "snfb_genotype_targets", "snfb_load_reference", "snfb_reference_runs", "snfb_fetch_reference",
+           "snfb_population_load", "snfb_population_match"]
 
 
 def lib():
@@ -69,6 +70,8 @@ def lib():
         L.snfb_fetch_reference.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
         L.snfb_combine_groups.argtypes = [C.c_void_p, C.POINTER(abi.CombineIn), C.POINTER(abi.CombineOut)]
         L.snfb_combine_plan.argtypes = [C.c_void_p, C.POINTER(abi.CombinePlanIn), C.POINTER(abi.CombinePlanOut)]
+        L.snfb_population_load.argtypes = [C.c_void_p, C.POINTER(abi.PopTable)]
+        L.snfb_population_match.argtypes = [C.c_void_p, C.POINTER(abi.PopQuery), C.c_void_p]
         L.snfb_selftest_edit_distance.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
         L.snfb_selftest_sqrt_frac.restype = C.c_double
         L.snfb_selftest_sqrt_frac.argtypes = [C.c_uint64, C.c_uint64, C.c_uint64, C.c_int]
@@ -459,6 +462,35 @@ class Context:
         return dict(perm=perm[:m], chains=chains[:O.n_chain], chunks=chunks[:O.n_chunk], cand_group=out[0][:m], emit_chunk=out[1][:m], emit_ord=out[2][:m],
                     cov_non=out[3][:m])
 
+    def population_load(self, contig, block, svtype, pos, svlen, alts):
+        """The population table on the device (snfb_population_load): per variant in file order its contig index (-1: not among the
+        run's contigs), block key, svtype 0..4, pos, svlen and ALT bytes.  It replaces any table loaded before."""
+        cols = [np.ascontiguousarray(v, "<i4") for v in (contig, block, svtype, pos, svlen)]
+        arena = alt_arena(alts)
+        T = abi.PopTable()
+        T.n = len(cols[0])
+        T.contig, T.block, T.svtype, T.pos, T.svlen = (v.ctypes.data for v in cols)
+        T.alt, T.alt_off, T.alt_len, T.n_alt_bytes = arena[0].ctypes.data, arena[1].ctypes.data, arena[2].ctypes.data, len(arena[0]) - 1
+        self._check(self._lib.snfb_population_load(self._h, C.byref(T)), "snfb_population_load")
+
+    def population_match(self, contig, svtype, pos, svlen, alts, combine_match, combine_match_max, combine_pctseq, block_size):
+        """PopulationSNF.get_population_AF on the device for one batch of calls (snfb_population_match): per call the file-order index of
+        the matching population variant, -1 for none, -2 where the reference would divide by a zero svlen"""
+        cols = [np.ascontiguousarray(v, "<i4") for v in (contig, svtype, pos, svlen)]
+        n = len(cols[0])
+        if n == 0:
+            return np.zeros(0, "<i4")
+        arena = alt_arena(alts)
+        Q = abi.PopQuery()
+        Q.n = n
+        Q.contig, Q.svtype, Q.pos, Q.svlen = (v.ctypes.data for v in cols)
+        Q.alt, Q.alt_off, Q.alt_len, Q.n_alt_bytes = arena[0].ctypes.data, arena[1].ctypes.data, arena[2].ctypes.data, len(arena[0]) - 1
+        Q.combine_match, Q.combine_match_max, Q.block_size = int(combine_match), int(combine_match_max), int(block_size)
+        Q.combine_pctseq = float(combine_pctseq or 0.0)
+        best = np.zeros(n, "<i4")
+        self._check(self._lib.snfb_population_match(self._h, C.byref(Q), best.ctypes.data), "snfb_population_match")
+        return best
+
     def edit_distances(self, pairs):
         """device edit distance of (bytes, bytes) pairs (snfb_selftest_edit_distance)"""
         n = len(pairs)
@@ -485,6 +517,15 @@ class Context:
         n = C.c_uint64()
         self._check(self._lib.snfb_device_candidates(self._h, C.byref(p), C.byref(n)), "snfb_device_candidates")
         return p.value, int(n.value)
+
+
+def alt_arena(alts):
+    """[bytes] -> (arena with one spare byte, u64 offsets, u32 lengths)"""
+    lens = np.fromiter((len(a) for a in alts), "<u4", len(alts))
+    offs = np.zeros(len(alts), "<u8")
+    if len(alts):
+        offs[1:] = np.cumsum(lens[:-1], dtype=np.uint64)
+    return np.frombuffer(b"".join(alts) + b"\0", np.uint8).copy(), offs, lens
 
 
 def _combine_params(I, a, config):

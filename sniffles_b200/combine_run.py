@@ -7,12 +7,17 @@ sniffles:371-481, parallel.py:372-572 and result.py:133-243.
   * tasks run in passes of consecutive tasks whose candidate count fits a budget: the host unpickles a pass's SNF blocks into flat columns
     (FlatPass), one snfb_combine_plan call plans the chunks and groups them on the device, and combine.CombineTask.emit_batches calls the
     groups on the host;
+  * with --combine-population, the population SNF's variants of the planned contigs are loaded to the device once, and every call a pass
+    makes gets POPULATION_AF / POPULATION_SIZE from one snfb_population_match call (SVGroup.call, sv.py:475-479);
   * each task's calls are ordered as CombineResult orders them, or, above --combine-max-inmemory-results inputs, as CombineResultTmpFile
     keeps them (a sorted batch's calls below the task's highest stored position are dropped), and written through vcf.open_output.
 
 Deviations from the reference: an SNF that is missing, unreadable or whose header has no contig_lengths is refused with a message instead
 of a traceback; a header without snf_format_version (as this package's SNF writer leaves it) is taken as the current version; the dropped
-calls of CombineResultTmpFile are counted and logged, not written to an `-unsorted.part.vcf`."""
+calls of CombineResultTmpFile are counted and logged, not written to an `-unsorted.part.vcf`; a population SNF that is missing, has no
+`population` header record or holds blocks that are not PopulationVariant lists is refused before any output is opened; an INS population
+variant with svlen 0 that reaches the alignment test, where the reference's worker divides by zero, stops the run with a message naming
+it."""
 import contextlib
 import logging
 import os
@@ -21,6 +26,7 @@ import time
 import numpy as np
 
 from . import call, combine, postprocess, snf, tasks, vcf
+from .snf import TYPES
 
 log = logging.getLogger("sniffles_b200.combine")
 
@@ -311,12 +317,85 @@ def check_outputs(config):
         raise CombineError(str(e)) from None
 
 
+class Population:
+    """the population SNF of --combine-population: its variants in the contigs of the run, flattened in file order (contig, block in
+    index order, svtype, list position), with the columns snfb_population_load reads"""
+
+    def __init__(self, path, contigs):
+        where = f"the population SNF {path} (--combine-population)"
+        try:
+            r = snf.PopulationReader(path)
+        except (OSError, ValueError, KeyError, UnicodeDecodeError) as e:
+            raise CombineError(f"Unable to read {where}: {e}") from e
+        try:
+            if not isinstance(r.population, dict):
+                raise CombineError(f"{where} has no population record in its header: it is not a population SNF")
+            self.info, self.contig_ids = r.population, {name: k for k, name in enumerate(contigs)}
+            self.variants = []
+            cols = {k: [] for k in ("contig", "block", "svtype", "pos", "svlen")}
+            self.alts = []
+            for name in contigs:
+                try:
+                    blocks = r.blocks(name)
+                except Exception as e:               # a truncated member, a pickle of unknown classes, ...
+                    raise CombineError(f"Unable to read the blocks of contig {name} in {where}: {e}") from e
+                for block, blk in blocks:
+                    for ti, t in enumerate(TYPES):
+                        lst = blk.get(t, []) if isinstance(blk, dict) else None
+                        if not isinstance(lst, list) or not all(isinstance(v, r.variant_class) for v in lst):
+                            raise CombineError(f"Block {name}:{block} of {where} does not hold PopulationVariant lists: it is not a population SNF")
+                        for v in lst:
+                            self.variants.append(v)
+                            cols["contig"].append(self.contig_ids[name])
+                            cols["block"].append(block)
+                            cols["svtype"].append(ti)
+                            cols["pos"].append(v.pos)
+                            cols["svlen"].append(v.svlen)
+                            self.alts.append(alt_bytes(v.alt))
+        finally:
+            r.close()
+        self.cols = {k: np.asarray(v, "<i4") for k, v in cols.items()}
+        self.path = path
+
+    def load(self, ctx):
+        c = self.cols
+        ctx.population_load(c["contig"], c["block"], c["svtype"], c["pos"], c["svlen"], self.alts)
+
+    def annotate(self, ctx, calls, config):
+        """PopulationSNF.get_population_AF for every call on the device, then POPULATION_AF = round(af, 5) and POPULATION_SIZE =
+        genotyped_sample_count, or 0 / 0 without a match (sv.py:475-479)"""
+        if not calls:
+            return
+        best = ctx.population_match([self.contig_ids.get(c.contig, -1) for c in calls], [TYPES.index(c.svtype) for c in calls],
+                                    [c.pos for c in calls], [c.svlen for c in calls], [alt_bytes(c.alt) for c in calls],
+                                    config.combine_match, config.combine_match_max, config.combine_pctseq, config.snf_block_size)
+        for c, b in zip(calls, best.tolist()):
+            if b == -2:                                  # a minimum length of 0 admits distance 0 only: the variant is at the call's position
+                vid = next((v.id for v in self.variants if v.contig == c.contig and v.svtype == "INS" and v.svlen == 0 and v.pos == c.pos), "?")
+                raise CombineError(f"The call {c.id} at {c.contig}:{c.pos} reaches the alignment test of population variant {vid} in {self.path}, "
+                                   f"whose svlen is 0: the reference stops on this division by zero")
+            set_population_info(c, self.variants[b] if b >= 0 else None)
+
+
+def alt_bytes(a):
+    return a.encode("latin-1") if isinstance(a, str) else bytes(a or b"")
+
+
+def set_population_info(call, variant):
+    """the two INFO values SVGroup.call sets (sv.py:475-479): round(af, 5) and the genotyped sample count, or the integers 0 and 0"""
+    af, sz = (round(variant.af, 5), variant.genotyped_sample_count) if variant is not None else (0, 0)
+    call.set_info("POPULATION_AF", af)
+    call.set_info("POPULATION_SIZE", sz)
+
+
 def combine_snfs(config, device=0, budget=None, stats=None):
     """the combine run mode: config.input (SNF files or one .tsv) -> config.vcf.  budget: the candidates one pass may hold (default
     PASS_CANDIDATES).  stats: a dict that receives the wall-clock split (header_s, decode_s, device_s, call_group_s, write_s, passes and
-    per-pass task and candidate counts, dropped).  Returns the number of VCF records written."""
+    per-pass task and candidate counts, dropped; with --combine-population population_s for the decode and load of the population SNF and
+    population_match_s for its matches).  Returns the number of VCF records written."""
     st = stats if stats is not None else {}
-    st.update(passes=0, pass_tasks=[], pass_candidates=[], header_s=0.0, decode_s=0.0, device_s=0.0, call_group_s=0.0, write_s=0.0, dropped=0)
+    st.update(passes=0, pass_tasks=[], pass_candidates=[], header_s=0.0, decode_s=0.0, device_s=0.0, call_group_s=0.0, write_s=0.0, dropped=0,
+              population_s=0.0, population_match_s=0.0)
     t0 = time.perf_counter()
     config.mode = "combine"
     check_outputs(config)
@@ -334,8 +413,21 @@ def combine_snfs(config, device=0, budget=None, stats=None):
                 log.warning("Result will be unsorted and uncompressed")
     log.info(f"Verified headers for {len(config.snf_input_info)} .snf files.")
     st["header_s"] = time.perf_counter() - t0
+    pop = None
+    if config.combine_population:                        # sniffles:433-435, parallel.py:454-455: opened and checked before any output
+        tp = time.perf_counter()
+        pop = Population(config.combine_population, list(dict.fromkeys(t.contig for t in planned)))
+        st["population_s"] += time.perf_counter() - tp
     readers = {}
     ctx = tasks.device_context(device)
+    if pop is not None:
+        tp = time.perf_counter()
+        try:
+            pop.load(ctx)
+        except Exception as e:
+            raise CombineError(f"Loading the population SNF {pop.path} (--combine-population) to the device failed: {e}") from e
+        st["population_s"] += time.perf_counter() - tp
+        log.info(f"Population SNF {pop.path}: {len(pop.variants)} variants in the run's contigs")
     if budget is None:
         budget = PASS_CANDIDATES
     written = 0
@@ -351,7 +443,7 @@ def combine_snfs(config, device=0, budget=None, stats=None):
             writer.write_header(contig_lengths)
             for group in call.group_passes(_decoded(config, planned, readers, st), budget, size=lambda fp: len(fp.cands)):
                 fp = join(group)
-                written += _run_pass(ctx, fp, config, reqc, writer, tmpfile, st)
+                written += _run_pass(ctx, fp, config, reqc, writer, tmpfile, st, pop)
             t1 = time.perf_counter()
         st["write_s"] += time.perf_counter() - t1
     finally:
@@ -373,8 +465,9 @@ def _decoded(config, planned, readers, st):
         yield fp
 
 
-def _run_pass(ctx, fp, config, reqc, writer, tmpfile, st):
-    """one device call for the pass's tasks, SVGroup.call on the host, the records written; returns the records written"""
+def _run_pass(ctx, fp, config, reqc, writer, tmpfile, st, pop=None):
+    """one device call for the pass's tasks, SVGroup.call on the host, the population annotation of every call the pass made (one device
+    call), the records written; returns the records written"""
     from . import binding
     flat = fp.arrays()
     t0 = time.perf_counter()
@@ -388,7 +481,14 @@ def _run_pass(ctx, fp, config, reqc, writer, tmpfile, st):
         if reqc[c.sample_internal_id]:
             requalify(c, config)
     batches = combine.CombineTask.emit_batches(fp.tasks, plan, out)
+    tp = time.perf_counter()
+    if pop is not None:                                  # SVGroup.call annotates each call before any result ordering drops one
+        try:
+            pop.annotate(ctx, [c for k in range(len(fp.tasks)) for _, c in batches[k]], config)
+        except binding.SnfbError as e:
+            raise CombineError(f"the population match of the pass from task {fp.tasks[0].id} failed: {e}") from e
     t2 = time.perf_counter()
+    st["population_match_s"] += t2 - tp
     written = 0
     for k in range(len(fp.tasks)):
         calls, dropped = stored_calls(batches[k], tmpfile, config.sort)
@@ -399,6 +499,6 @@ def _run_pass(ctx, fp, config, reqc, writer, tmpfile, st):
     st["pass_tasks"].append(len(fp.tasks))
     st["pass_candidates"].append(len(fp.cands))
     st["device_s"] += t1 - t0
-    st["call_group_s"] += t2 - t1
+    st["call_group_s"] += tp - t1
     st["write_s"] += time.perf_counter() - t2
     return written

@@ -24,6 +24,7 @@
 #include "consensus.cuh"
 #include "poa.cuh"
 #include "combine.cuh"
+#include "population.cuh"
 #include "ingest.cuh"
 #include "bgzf_write.cuh"
 #include "genotype.cuh"
@@ -104,6 +105,8 @@ struct snfb_ctx {
     DevBuf b_comp, b_raw, b_ing, b_ing_work; HostBuf h_ing; uint64_t ing_sizes[8] = {0, 0, 0, 0, 0, 0, 0, 0}; bool from_bam = false;      // device BAM ingest: BGZF bytes, inflated stream, block / span tables, per-raw-record work arrays
     DevBuf b_zin, b_zslot, b_zout, b_zwork;          // BGZF compression: input bytes, 64 KiB member slots, packed members, sizes / offsets / candidate scratch
     DevBuf b_gt;                                     // force calling: candidate bin keys, sort scratch, targets and their results
+    // population table (snfb_population_load): sorted keys and columns, the ALT arena; b_popq: one batch of queries and their results
+    DevBuf b_pop, b_popq; population::P pop{}; bool have_pop = false;
     DevBuf b_ref, b_ref_work; std::vector<refseq::Contig> ref_ctg; bool have_ref = false;     // the unwrapped reference genome; tables / counters / N-run scratch
     HostBuf h_ref_runs, h_ref_coff, h_ref_out; uint64_t ref_n_runs = 0;                       // N runs and per-contig offsets; gather staging
     std::vector<snfb_task> tasks;
@@ -260,7 +263,8 @@ size_t snfb_sizeof(int which) {
                      case 4: return sizeof(snfb_config); case 5: return sizeof(snfb_lead); case 6: return sizeof(snfb_cand); case 7: return sizeof(snfb_gather_view);
                      case 8: return sizeof(snfb_gt_in); case 9: return sizeof(snfb_gt_out);
                      case 10: return sizeof(snfb_ref_contig); case 11: return sizeof(snfb_ref_input); case 12: return sizeof(snfb_ref_query); case 13: return sizeof(snfb_region);
-                     case 14: return sizeof(snfb_combine_plan_in); case 15: return sizeof(snfb_combine_plan_out); default: return 0; }
+                     case 14: return sizeof(snfb_combine_plan_in); case 15: return sizeof(snfb_combine_plan_out);
+                     case 16: return sizeof(snfb_pop_table); case 17: return sizeof(snfb_pop_query); default: return 0; }
 }
 
 uint64_t snfb_hash_name(const char* s, size_t n) {
@@ -1423,6 +1427,97 @@ int snfb_combine_plan(snfb_ctx* ctx, const snfb_combine_plan_in* in, snfb_combin
     CUDA_TRY(cudaMemcpyAsync(out->chunks, P.chunks, sizeof(snfb_combine_chunk) * n_chunk, cudaMemcpyDeviceToHost, st));
     if (combine_run_groups(ctx, &g, P, n_chain, n_chunk, n, use_alt, max_alt, b_state, b_out, &out->group, "snfb_combine_plan")) return 1;
     out->n_cand = n; out->n_chain = n_chain; out->n_chunk = n_chunk;
+    return 0;
+}
+
+// the population table (PopulationSNF.get_all_blocks, snfp.py:139-140): keyed on the device, sorted stably, kept on the context
+int snfb_population_load(snfb_ctx* ctx, const snfb_pop_table* in) {
+    if (!ctx || !in) return ctx ? fail(ctx, "snfb_population_load: null argument") : 1;
+    const uint32_t n = in->n;
+    if (n && (!in->contig || !in->block || !in->svtype || !in->pos || !in->svlen || !in->alt_off || !in->alt_len || (in->n_alt_bytes && !in->alt)))
+        return fail(ctx, "snfb_population_load: null array");
+    int32_t max_contig = -1; uint32_t max_alt = 16;
+    for (uint32_t i = 0; i < n; ++i) {
+        if (in->contig[i] < -1 || in->contig[i] >= (1 << 24) - 1 || in->svtype[i] < 0 || in->svtype[i] > 4)
+            return fail(ctx, "snfb_population_load: variant " + std::to_string(i) + " has a contig or svtype out of range");
+        if (in->alt_off[i] + in->alt_len[i] > in->n_alt_bytes) return fail(ctx, "snfb_population_load: ALT outside alt[]");
+        max_contig = std::max(max_contig, in->contig[i]); max_alt = std::max(max_alt, in->alt_len[i]);
+    }
+    cudaSetDevice(ctx->device);
+    cudaStream_t st = ctx->st;
+    ctx->have_pop = false; ctx->n_ev = 0;
+    population::P& P = ctx->pop;
+    P = population::P{};
+    int32_t *f_contig, *f_block, *f_svtype, *f_pos, *f_svlen; unsigned long long* f_alt_off; uint32_t* f_alt_len; unsigned long long* d_n;
+    uint64_t *k0, *k1; uint32_t *v0, *v1; prims::RadixTemp rt{};
+    auto lay = [&](Carver& c) {
+        f_contig = c.take<int32_t>(n + 1); f_block = c.take<int32_t>(n + 1); f_svtype = c.take<int32_t>(n + 1); f_pos = c.take<int32_t>(n + 1); f_svlen = c.take<int32_t>(n + 1);
+        f_alt_off = c.take<unsigned long long>(n + 1); f_alt_len = c.take<uint32_t>(n + 1); d_n = c.take<unsigned long long>(2);
+        k0 = c.take<uint64_t>(n + 1); k1 = c.take<uint64_t>(n + 1); v0 = c.take<uint32_t>(n + 1); v1 = c.take<uint32_t>(n + 1);
+        rt.hist = c.take<uint32_t>(prims::radix_hist_elems(n)); rt.scan_tmp = c.take<uint32_t>(prims::scan_tmp_elems(prims::radix_hist_elems(n)) + 16);
+        P.pos = c.take<int32_t>(n + 1); P.svlen = c.take<int32_t>(n + 1); P.alt_off = c.take<unsigned long long>(n + 1); P.alt_len = c.take<uint32_t>(n + 1);
+        P.alt = c.take<uint8_t>(in->n_alt_bytes + 16);
+    };
+    if (carve(ctx->b_pop, lay)) return fail(ctx, "snfb_population_load: out of device memory");
+    auto up = [&](const void* dst, const void* src, size_t bytes) { if (bytes && src) CUDA_TRY(cudaMemcpyAsync(const_cast<void*>(dst), src, bytes, cudaMemcpyHostToDevice, st)); return 0; };
+    const unsigned long long nn = n;
+    if (up(f_contig, in->contig, 4 * (size_t)n) || up(f_block, in->block, 4 * (size_t)n) || up(f_svtype, in->svtype, 4 * (size_t)n) || up(f_pos, in->pos, 4 * (size_t)n)
+        || up(f_svlen, in->svlen, 4 * (size_t)n) || up(f_alt_off, in->alt_off, 8 * (size_t)n) || up(f_alt_len, in->alt_len, 4 * (size_t)n)
+        || up(P.alt, in->alt, in->n_alt_bytes) || up(d_n, &nn, 8)) return 1;
+    const uint32_t absent = (uint32_t)(max_contig + 1);
+    mark(ctx, "population_load", 32ull * n + in->n_alt_bytes);
+    bool first = true;
+    if (n) {
+        launch(ctx->launches, population::k_pop_keys, grid_for(n, 256), 256, 0, st, f_contig, f_block, f_svtype, n, absent, k0, v0);
+        prims::radix_sort(ctx->launches, k0, v0, k1, v1, rt, d_n, n, 35 + bits_for(absent + 1), &first, st);
+        launch(ctx->launches, population::k_pop_gather, grid_for(n, 256), 256, 0, st, first ? v0 : v1, n, f_pos, f_svlen, f_alt_off, f_alt_len,
+               const_cast<int32_t*>(P.pos), const_cast<int32_t*>(P.svlen), const_cast<unsigned long long*>(P.alt_off), const_cast<uint32_t*>(P.alt_len));
+    }
+    mark(ctx, nullptr);
+    P.key = first ? k0 : k1; P.idx = first ? v0 : v1; P.n_var = n; P.n_contig = absent; P.max_alt = max_alt;
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, std::string("snfb_population_load: ") + cudaGetErrorString(e));
+    ctx->have_pop = true;
+    return 0;
+}
+
+// PopulationSNF.get_population_AF (snfp.py:131-155) for one batch of calls: one warp per call (population.cuh)
+int snfb_population_match(snfb_ctx* ctx, const snfb_pop_query* in, int32_t* best) {
+    if (!ctx || !in || !best) return ctx ? fail(ctx, "snfb_population_match: null argument") : 1;
+    if (!ctx->have_pop) return fail(ctx, "snfb_population_match: no population table (snfb_population_load)");
+    const uint32_t n = in->n;
+    if (n == 0) return 0;
+    if (!in->contig || !in->svtype || !in->pos || !in->svlen || !in->alt_off || !in->alt_len || (in->n_alt_bytes && !in->alt)) return fail(ctx, "snfb_population_match: null array");
+    if (in->block_size <= 0) return fail(ctx, "snfb_population_match: bad block size");
+    uint32_t max_alt = ctx->pop.max_alt;
+    for (uint32_t i = 0; i < n; ++i) {
+        if (in->svtype[i] < 0 || in->svtype[i] > 4 || in->contig[i] < -1 || in->contig[i] >= (1 << 24) - 1)
+            return fail(ctx, "snfb_population_match: query " + std::to_string(i) + " has a contig or svtype out of range");
+        if (in->alt_off[i] + in->alt_len[i] > in->n_alt_bytes) return fail(ctx, "snfb_population_match: ALT outside alt[]");
+        max_alt = std::max(max_alt, in->alt_len[i]);
+    }
+    max_alt = (max_alt + 15u) & ~15u;
+    cudaSetDevice(ctx->device);
+    cudaStream_t st = ctx->st;
+    ctx->n_ev = 0;
+    population::P P = ctx->pop;
+    const unsigned blocks = (unsigned)std::min<uint32_t>((n + 3) / 4, NUM_SMS * 8);
+    auto lay = [&](Carver& c) {
+        P.q_contig = c.take<int32_t>(n); P.q_svtype = c.take<int32_t>(n); P.q_pos = c.take<int32_t>(n); P.q_svlen = c.take<int32_t>(n);
+        P.q_alt_off = c.take<unsigned long long>(n); P.q_alt_len = c.take<uint32_t>(n); P.q_alt = c.take<uint8_t>(in->n_alt_bytes + 16);
+        P.best = c.take<int32_t>(n); P.hs = c.take<int8_t>((size_t)blocks * 4 * max_alt + 16);
+    };
+    if (carve(ctx->b_popq, lay)) return fail(ctx, "snfb_population_match: out of device memory");
+    auto up = [&](const void* dst, const void* src, size_t bytes) { if (bytes && src) CUDA_TRY(cudaMemcpyAsync(const_cast<void*>(dst), src, bytes, cudaMemcpyHostToDevice, st)); return 0; };
+    if (up(P.q_contig, in->contig, 4 * (size_t)n) || up(P.q_svtype, in->svtype, 4 * (size_t)n) || up(P.q_pos, in->pos, 4 * (size_t)n) || up(P.q_svlen, in->svlen, 4 * (size_t)n)
+        || up(P.q_alt_off, in->alt_off, 8 * (size_t)n) || up(P.q_alt_len, in->alt_len, 4 * (size_t)n) || up(P.q_alt, in->alt, in->n_alt_bytes)) return 1;
+    P.n_q = n; P.combine_match = in->combine_match; P.combine_match_max = in->combine_match_max; P.block_size = in->block_size; P.pctseq = in->combine_pctseq; P.max_alt = max_alt;
+    mark(ctx, "population_match");
+    launch(ctx->launches, population::k_pop_match, blocks, 128, 0, st, P);
+    mark(ctx, nullptr);
+    CUDA_TRY(cudaMemcpyAsync(best, P.best, 4 * (size_t)n, cudaMemcpyDeviceToHost, st));
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, std::string("snfb_population_match: ") + cudaGetErrorString(e));
     return 0;
 }
 

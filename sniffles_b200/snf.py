@@ -97,6 +97,37 @@ def compat_classes():
     return SVCall, SVCallBNDInfo, ForwardDifferenceWelford
 
 
+def population_class():
+    """sniffles.snfp.PopulationVariant (snfp.py:25-37), the class a population SNF's blocks pickle: the reference's own when it imports,
+    else a dataclass registered under that module path"""
+    compat_classes()
+    try:
+        m = importlib.import_module("sniffles.snfp")
+        return m.PopulationVariant
+    except Exception:
+        pass
+    mod = types.ModuleType("sniffles.snfp")
+
+    @dataclass
+    class PopulationVariant:                         # field set and order of snfp.py:25-37
+        contig: str
+        pos: int
+        id: str
+        alt: str
+        svtype: str
+        svlen: int
+        end: int
+        af: float
+        genotyped_sample_count: int
+        variant_sample_count: int
+
+    PopulationVariant.__module__, PopulationVariant.__qualname__ = "sniffles.snfp", "PopulationVariant"
+    mod.PopulationVariant = PopulationVariant
+    sys.modules["sniffles.snfp"] = mod
+    setattr(sys.modules["sniffles"], "snfp", mod)
+    return PopulationVariant
+
+
 def to_compat(call):
     """postprocess.SVCall -> the picklable candidate the reference expects (postprocessing info dropped as by SVCall.finalize)"""
     SVCall, BND, _ = compat_classes()
@@ -196,3 +227,22 @@ class SNFReader:
                     for t in TYPES:
                         for c in blk[t]:
                             yield contig, int(block), c
+
+
+class PopulationReader(SNFReader):
+    """a population SNF (--combine-population): an SNF whose header has a `population` record (snfp.py:110-115, 178-185) and whose blocks
+    hold PopulationVariant lists.  As PopulationSNF.get_all_blocks (snf.py:235-243) only the first part of a block is read."""
+
+    def __init__(self, path):
+        super().__init__(path)
+        self.population = self.header.get("population")
+        self.variant_class = population_class()
+
+    def blocks(self, contig):
+        """[(block start, {svtype: [PopulationVariant, ...]})] of the contig, in index order, each block's first part"""
+        out = []
+        for block in self.index.get(contig, {}):
+            start, length = self.index[contig][block][0]
+            self.f.seek(self.header_length + start)
+            out.append((int(block), pickle.loads(gzip.decompress(self.f.read(length)))))
+        return out

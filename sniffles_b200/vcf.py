@@ -14,9 +14,12 @@ reference's `VCF.write_header` / `VCF.write_call` (/root/reference/src/sniffles/
 The FASTA reader is any object with `fetch(contig, start, end) -> str` (pysam.FastaFile duck type); none is needed for
 symbolic / sequence-free output.  Genotype columns follow format_genotype (vcf.py:50-79)."""
 import io
+import logging
 from collections import Counter
 
 from . import bamio
+
+log = logging.getLogger("sniffles_b200.vcf")
 
 AMBIGUOUS = str.maketrans("RYSWKMBDHV", "N" * 10)          # util.py:169-170
 
@@ -136,6 +139,9 @@ class VCFWriter:
         if getattr(c, "combine_population", None):
             h.append('INFO=<ID=POPULATION_AF,Number=1,Type=Float,Description="Population Allele Frequency">')
             h.append('INFO=<ID=POPULATION_SIZE,Number=1,Type=Integer,Description="Size of genotyped population for this variant">')
+            if getattr(c, "mode", None) == "combine" and self.phased:        # vcf.py:201-204
+                log.warning("Sniffles does not provide population phasing, it just displays the phasing information from each independent "
+                            "sample. Multi-sample phased genotypes may be inconsistent with population phasing")
         for line in h:
             self._line("##" + line)
         self._line("#CHROM\tPOS\tID\tREF\tALT\tQUAL\tFILTER\tINFO\tFORMAT\t" + "\t".join(name for _, name in self.samples))
