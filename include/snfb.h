@@ -26,6 +26,7 @@
  *   snfb_load_reference / snfb_reference_runs / snfb_fetch_reference
  *                          <- pysam.FastaFile behind LeadProvider._mask_N_coverage (leadprov.py:420-443) and
  *                             VCF.open_reference / write_call (vcf.py:108-119, 299-342)
+ *   snfb_read_names        <- the query names behind SVCall.rnames (sv.py:520-525, 555), written as RNAMES by --output-rnames
  *   snfb_allgather_candidates <- the parent collecting every worker's finished task results before VCF
  *                             emission (sniffles:544-547, parallel.py:270-271), as one NCCL all-gather
  *
@@ -307,7 +308,7 @@ typedef struct snfb_ctx snfb_ctx;
 int         snfb_version(void);
 /* sizeof of the ABI structs, for binding self-checks: 0 rec, 1 task, 2 contig, 3 records, 4 config, 5 lead, 6 cand, 7 gather_view,
  * 8 gt_in, 9 gt_out, 10 ref_contig, 11 ref_input, 12 ref_query, 13 region, 14 combine_plan_in, 15 combine_plan_out, 16 pop_table,
- * 17 pop_query */
+ * 17 pop_query, 18 rnames_view */
 size_t      snfb_sizeof(int which);
 uint64_t    snfb_hash_name(const char* s, size_t n);
 int         snfb_ctx_create(int device, snfb_ctx** out);
@@ -552,6 +553,22 @@ typedef struct snfb_pop_query {
 } snfb_pop_query;
 int         snfb_population_load(snfb_ctx* ctx, const snfb_pop_table* in);
 int         snfb_population_match(snfb_ctx* ctx, const snfb_pop_query* in, int32_t* best);
+/* ---- read names (--output-rnames: the RNAMES of sv.py:520-525, 555) ----
+ * Runs after snfb_run (or snfb_cluster_call) on the same context, on the candidates and the record block it left there, and changes nothing
+ * that call produced.  Name k is the query name of snfb_cand_view.rnames[k]: for each candidate, each of its distinct qname hashes is
+ * resolved through the first of the candidate's leads (cand_leads[lead_off .. + lead_n + long_n)) that carries it, to that lead's record's
+ * var[var_off .. + l_qname).  Names come in the order of the hash list (per candidate ascending by hash), so candidate c owns names
+ * rnames_off[c] .. rnames_off[c + 1] and name k is text[off[k] .. off[k + 1]).  `collisions` counts the leads whose own name differs from
+ * the name kept for their hash (two reads with one 64-bit hash); a hash that none of the candidate's leads carries fails the call.  The view
+ * is library-owned pinned host memory, valid until the next call on the context.  Timing marks: rnames_resolve, rnames_copy. */
+typedef struct snfb_rnames_view {
+    uint64_t n_names;               /* = the run's snfb_cand_view rnames count */
+    uint64_t n_text;                /* bytes of text */
+    const uint8_t*  text;           /* the names back to back, as the records store them (no separator, no NUL) */
+    const uint32_t* off;            /* [n_names + 1] */
+    uint64_t collisions;
+} snfb_rnames_view;
+int         snfb_read_names(snfb_ctx* ctx, snfb_rnames_view* out);
 /* self-check of the exact statistics.stdev arithmetic (host build of the routine the kernels use): the correctly rounded sqrt(P / Q) for
  * P = p_hi * 2^64 + p_lo; slow != 0 selects the limb-by-limb restatement of CPython's _float_sqrt_of_frac, 0 the verified fast path */
 double      snfb_selftest_sqrt_frac(uint64_t p_hi, uint64_t p_lo, uint64_t q, int slow);

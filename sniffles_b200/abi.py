@@ -194,6 +194,10 @@ class GtOut(C.Structure):                                       # snfb_gt_out
     _fields_ = [("match", C.c_void_p), ("cov_start", C.c_void_p), ("cov_center", C.c_void_p), ("cov_end", C.c_void_p), ("bnd_no_prev", C.c_void_p)]
 
 
+class RnamesView(C.Structure):                                  # snfb_rnames_view
+    _fields_ = [("n_names", C.c_uint64), ("n_text", C.c_uint64), ("text", C.c_void_p), ("off", C.c_void_p), ("collisions", C.c_uint64)]
+
+
 REF_CONTIG_DTYPE = np.dtype([("offset", "<u8"), ("length", "<u8"), ("linebases", "<u4"), ("linewidth", "<u4")])       # snfb_ref_contig
 REF_QUERY_DTYPE = np.dtype([("contig", "<u4"), ("_pad", "<u4"), ("start", "<u8"), ("length", "<u8"), ("out_off", "<u8")])  # snfb_ref_query
 

@@ -19,7 +19,7 @@ EXPORTS = ["snfb_version", "snfb_sizeof", "snfb_hash_name", "snfb_ctx_create", "
            "snfb_nccl_unique_id", "snfb_comm_init", "snfb_allgather_candidates", "snfb_selftest_sqrt_frac", "snfb_poa", "snfb_combine_groups", "snfb_combine_plan", "snfb_selftest_edit_distance",
            "snfb_load_bam", "snfb_set_regions", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf", "snfb_deflate_bgzf",
            "snfb_genotype_targets", "snfb_load_reference", "snfb_reference_runs", "snfb_fetch_reference",
-           "snfb_population_load", "snfb_population_match"]
+           "snfb_population_load", "snfb_population_match", "snfb_read_names"]
 
 
 def lib():
@@ -65,6 +65,7 @@ def lib():
         L.snfb_allgather_candidates.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(abi.GatherView)]
         L.snfb_poa.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
         L.snfb_genotype_targets.argtypes = [C.c_void_p, C.POINTER(abi.GtIn), C.POINTER(abi.GtOut)]
+        L.snfb_read_names.argtypes = [C.c_void_p, C.POINTER(abi.RnamesView)]
         L.snfb_load_reference.argtypes = [C.c_void_p, C.POINTER(abi.RefInput)]
         L.snfb_reference_runs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
         L.snfb_fetch_reference.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
@@ -322,6 +323,15 @@ class Context:
         self._check(self._lib.snfb_genotype_targets(self._h, C.byref(I), C.byref(O)), "snfb_genotype_targets")
         return out
 
+    def read_names(self):
+        """The supporting reads' names of the last run's candidates (snfb_read_names), after `run` / `cluster_call` on this context and before
+        the next load.  Returns ReadNames: the names' bytes back to back (uint8) and their offsets (uint32, one per name of result.rnames
+        plus the end), so candidate i owns names rn_off[i] .. rn_off[i + 1], each in the order of its hash list."""
+        v = abi.RnamesView()
+        self._check(self._lib.snfb_read_names(self._h, C.byref(v)), "snfb_read_names")
+        return ReadNames(abi.view(v.text, "u1", v.n_text).copy(), abi.view(v.off, "<u4", v.n_names + 1).copy() if v.n_names else np.zeros(1, "<u4"),
+                         int(v.collisions))
+
     def load_reference(self, data, contigs, is_bgzf=False):
         """Reference FASTA -> the unwrapped genome resident on this context, and its 'N' runs (snfb_load_reference).  data: the file's bytes
         (whole BGZF members when is_bgzf); contigs: abi.REF_CONTIG_DTYPE rows (raw offset rebased to `data`'s inflated stream, length,
@@ -517,6 +527,23 @@ class Context:
         n = C.c_uint64()
         self._check(self._lib.snfb_device_candidates(self._h, C.byref(p), C.byref(n)), "snfb_device_candidates")
         return p.value, int(n.value)
+
+
+class ReadNames:
+    """The read names of a run's candidates (Context.read_names): text (uint8) and off (uint32, [n_names + 1]) with name k =
+    text[off[k]:off[k + 1]], in the order of the run's rnames hashes; collisions = leads whose name differs from the one kept for their hash."""
+
+    def __init__(self, text, off, collisions=0):
+        self.text, self.off, self.collisions = text, off, collisions
+        self._str = self._off = None
+
+    def per_candidate(self, rn_off, lo, hi):
+        """[list of str] for candidates lo .. hi - 1 (rn_off: the run's rnames offsets).  The text is decoded once, as ASCII (the SAM
+        specification's QNAME alphabet), and every name is a slice of that one string."""
+        if self._str is None:
+            self._str, self._off = self.text.tobytes().decode("ascii"), self.off.tolist()
+        s, off = self._str, self._off
+        return [[s[off[k]:off[k + 1]] for k in range(int(rn_off[i]), int(rn_off[i + 1]))] for i in range(lo, hi)]
 
 
 def alt_arena(alts):

@@ -128,11 +128,12 @@ def join_inputs(inputs, n_regions=None):
     return bgzf, np.concatenate(rows) if rows else np.zeros(0, abi.SPAN_DTYPE)
 
 
-def load_pass(ctx, bam, group, config, tr_all, contigs=None):
+def load_pass(ctx, bam, group, config, tr_all, contigs=None, read_names=False):
     """the device half of a pass over `group` (items of task_inputs): mask_block, set_config, set_regions, snfb_load_bam and snfb_run,
     the k-th task of the group being task index k of the block.  Returns the pass's tasks.BlockRun and its split {"load_bam_s", "run_s"};
     a load or run the library refuses raises CallSampleError naming the pass's contigs and inflated bytes.  contigs: the names
-    tasks.reference_for loads (None: all)."""
+    tasks.reference_for loads (None: all).  read_names: also gather the candidates' read names (snfb_read_names, before the next load
+    replaces the records) into BlockRun.read_names, timed as split["rnames_s"]."""
     tr = {k: [(int(a), int(b)) for a, b in tr_all[g[1]]] for k, g in enumerate(group) if g[1] in tr_all}
     # a task with regions: its records carry their region's window, its own bounds only clip the N mask (the host clips it to the regions)
     bounds = [(0, bam.get_reference_length(name)) if rg else (s, e) for _, name, s, e, _, _, _, rg in group]
@@ -152,19 +153,23 @@ def load_pass(ctx, bam, group, config, tr_all, contigs=None):
         t1 = time.perf_counter()
         res = ctx.run(want_leads=True, want_cands=True, want_seqs=True)
         t2 = time.perf_counter()
+        names = tasks.read_names(ctx) if read_names else None
+        t3 = time.perf_counter()
     except binding.SnfbError as e:
-        names = ", ".join(g[1] for g in group)
-        raise CallSampleError(f"the device pass over contig(s) {names} ({sum(g[6] for g in group)} inflated BAM bytes) failed: {e}") from e
+        contig_list = ", ".join(g[1] for g in group)
+        raise CallSampleError(f"the device pass over contig(s) {contig_list} ({sum(g[6] for g in group)} inflated BAM bytes) failed: {e}") from e
     split["load_bam_s"], split["run_s"] = t1 - t0, t2 - t1
+    if read_names:
+        split["rnames_s"] = t3 - t2
     rec_nm = abi.view(res._rec_nm_ptr, "<f8", n_rec).copy() if getattr(res, "_rec_nm_ptr", None) else None
-    return tasks.BlockRun(block, res, tasks.cand_ranges(res.cand, len(block.task)), rec_nm), split
+    return tasks.BlockRun(block, res, tasks.cand_ranges(res.cand, len(block.task)), rec_nm, read_names=names), split
 
 
 def run_pass(ctx, bam, group, config, tr_all, device=0, contigs=None, failed=None):
     """one device pass over `group` (items of task_inputs): load_pass, then every task as a CallTask on the pass's BlockRun.  Returns
-    [(CallTask, calls)] in task order and the pass's split {"load_bam_s", "run_s", "finalize_s"}.  contigs: the names
-    tasks.reference_for loads (None: all); failed: receives (task id, contig, error class name) of every task that fails."""
-    br, split = load_pass(ctx, bam, group, config, tr_all, contigs)
+    [(CallTask, calls)] in task order and the pass's split {"load_bam_s", "run_s", "finalize_s"}, with --output-rnames also "rnames_s".
+    contigs: the names tasks.reference_for loads (None: all); failed: receives (task id, contig, error class name) of every task that fails."""
+    br, split = load_pass(ctx, bam, group, config, tr_all, contigs, read_names=bool(getattr(config, "output_rnames", False)))
     t2 = time.perf_counter()
     done = []
     for k, (tid, name, s, e, *_) in enumerate(group):
@@ -237,7 +242,7 @@ def call_sample(config, device=0, budget=None, stats=None):
     reference = tasks.reference_for(ctx, config.reference) if getattr(config, "reference", None) else None
     if budget is None:
         budget = device_budget(device)
-    st.update(passes=0, pass_inflated_bytes=[], load_bam_s=[], run_s=[], finalize_s=0.0, vcf_write_s=0.0, snf_write_s=0.0, read_s=0.0)
+    st.update(passes=0, pass_inflated_bytes=[], load_bam_s=[], run_s=[], rnames_s=[], finalize_s=0.0, vcf_write_s=0.0, snf_write_s=0.0, read_s=0.0)
     st["index_s"] = time.perf_counter() - t0
     parts, written = [], 0
     with contextlib.ExitStack() as stack:
@@ -256,6 +261,8 @@ def call_sample(config, device=0, budget=None, stats=None):
             st["pass_inflated_bytes"].append(sum(g[6] for g in group))
             st["load_bam_s"].append(split["load_bam_s"])
             st["run_s"].append(split["run_s"])
+            if "rnames_s" in split:
+                st["rnames_s"].append(split["rnames_s"])
             st["finalize_s"] += split["finalize_s"]
             t1 = time.perf_counter()
             if writer is not None:
@@ -290,7 +297,7 @@ def run_rank_tasks(config, device, budget, rank, world):
     import io
     from . import dist
     t0 = time.perf_counter()
-    st = dict(passes=0, pass_inflated_bytes=[], load_bam_s=[], run_s=[], finalize_s=0.0, vcf_write_s=0.0, read_s=0.0)
+    st = dict(passes=0, pass_inflated_bytes=[], load_bam_s=[], run_s=[], rnames_s=[], finalize_s=0.0, vcf_write_s=0.0, read_s=0.0)
     bam, contig_lengths, planned, tr_all = plan_sample(config)
     weights = dist.task_weights(bam, planned, config.regions_by_contig)
     owner = dist.lpt_assign(weights, world)
@@ -310,6 +317,8 @@ def run_rank_tasks(config, device, budget, rank, world):
         st["pass_inflated_bytes"].append(sum(g[6] for g in group))
         st["load_bam_s"].append(split["load_bam_s"])
         st["run_s"].append(split["run_s"])
+        if "rnames_s" in split:
+            st["rnames_s"].append(split["rnames_s"])
         st["finalize_s"] += split["finalize_s"]
         t1 = time.perf_counter()
         if config.vcf is not None and reference is not None:

@@ -28,6 +28,7 @@
 #include "ingest.cuh"
 #include "bgzf_write.cuh"
 #include "genotype.cuh"
+#include "rnames.cuh"
 #include "reference.cuh"
 
 // one owning allocation of device memory, or of pinned host memory when Pinned; freed by the destructor
@@ -105,6 +106,7 @@ struct snfb_ctx {
     DevBuf b_comp, b_raw, b_ing, b_ing_work; HostBuf h_ing; uint64_t ing_sizes[8] = {0, 0, 0, 0, 0, 0, 0, 0}; bool from_bam = false;      // device BAM ingest: BGZF bytes, inflated stream, block / span tables, per-raw-record work arrays
     DevBuf b_zin, b_zslot, b_zout, b_zwork;          // BGZF compression: input bytes, 64 KiB member slots, packed members, sizes / offsets / candidate scratch
     DevBuf b_gt;                                     // force calling: candidate bin keys, sort scratch, targets and their results
+    DevBuf b_rn, b_rn_text; HostBuf h_rn_meta, h_rn_text;     // read names: per-name scratch and counters, the text; counters + offsets, text on the host
     // population table (snfb_population_load): sorted keys and columns, the ALT arena; b_popq: one batch of queries and their results
     DevBuf b_pop, b_popq; population::P pop{}; bool have_pop = false;
     DevBuf b_ref, b_ref_work; std::vector<refseq::Contig> ref_ctg; bool have_ref = false;     // the unwrapped reference genome; tables / counters / N-run scratch
@@ -264,7 +266,7 @@ size_t snfb_sizeof(int which) {
                      case 8: return sizeof(snfb_gt_in); case 9: return sizeof(snfb_gt_out);
                      case 10: return sizeof(snfb_ref_contig); case 11: return sizeof(snfb_ref_input); case 12: return sizeof(snfb_ref_query); case 13: return sizeof(snfb_region);
                      case 14: return sizeof(snfb_combine_plan_in); case 15: return sizeof(snfb_combine_plan_out);
-                     case 16: return sizeof(snfb_pop_table); case 17: return sizeof(snfb_pop_query); default: return 0; }
+                     case 16: return sizeof(snfb_pop_table); case 17: return sizeof(snfb_pop_query); case 18: return sizeof(snfb_rnames_view); default: return 0; }
 }
 
 uint64_t snfb_hash_name(const char* s, size_t n) {
@@ -1623,6 +1625,51 @@ int snfb_genotype_targets(snfb_ctx* ctx, const snfb_gt_in* in, snfb_gt_out* out)
     for (int k = 0; k < 4; ++k) CUDA_TRY(cudaMemcpyAsync(dst[k], G.cov_start + (size_t)k * n, 4 * n, cudaMemcpyDeviceToHost, st));
     const cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, std::string("snfb_genotype_targets: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+// read names (--output-rnames): the candidates' hash lists resolved to the resident records' names, gathered into one text
+int snfb_read_names(snfb_ctx* ctx, snfb_rnames_view* out) {
+    if (!ctx || !out) return ctx ? fail(ctx, "snfb_read_names: null argument") : 1;
+    if (!ctx->stage_b_done) return fail(ctx, "snfb_read_names: snfb_run or snfb_cluster_call must run first");
+    cudaSetDevice(ctx->device);
+    memset(out, 0, sizeof *out);
+    const unsigned long long nc = ctx->h_fin->n_cand, nn = ctx->h_fin->n_rnames;
+    rnames::P P{}; uint32_t* scan_tmp = nullptr;
+    auto lay = [&](Carver& c) {
+        P.first = c.take<uint32_t>(nn + 1); P.len = c.take<uint32_t>(nn + 1); P.off = c.take<uint32_t>(nn + 1); P.src = c.take<uint64_t>(nn + 1);
+        scan_tmp = c.take<uint32_t>(prims::scan_tmp_elems(nn) + 16); P.ctr = c.take<unsigned long long>(4);
+    };
+    if (carve(ctx->b_rn, lay)) return fail(ctx, "snfb_read_names: out of device memory");
+    if (ctx->h_rn_meta.ensure(32 + 4 * (nn + 1))) return fail(ctx, "snfb_read_names: out of pinned memory");
+    unsigned long long* h_ctr = ctx->h_rn_meta.as<unsigned long long>(); uint32_t* h_off = reinterpret_cast<uint32_t*>(h_ctr + 4);
+    P.cand = ctx->B.cand; P.n_cand = nc; P.leads = ctx->B.cand_leads; P.hash = ctx->B.rnames; P.rn_off = ctx->B.rn_off_out; P.n_names = nn;
+    P.rec = ctx->d_rec; P.var = ctx->d_var;
+    cudaStream_t st = ctx->st;
+    ctx->n_ev = 0;
+    mark(ctx, "rnames_resolve");
+    CUDA_TRY(cudaMemsetAsync(P.ctr, 0, 32, st));
+    if (nn) {
+        launch(ctx->launches, rnames::k_resolve, grid_for(nc * 32, 128), 128, 0, st, P);
+        prims::exclusive_scan(ctx->launches, P.len, P.off, scan_tmp, nullptr, nn, nullptr, st);
+    }
+    mark(ctx, nullptr);
+    CUDA_TRY(cudaMemcpyAsync(h_ctr, P.ctr, 32, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    const unsigned long long n_text = h_ctr[0];
+    if (h_ctr[2]) return fail(ctx, "snfb_read_names: " + std::to_string(h_ctr[2]) + " read name hash(es) carried by none of their candidate's leads");
+    if (n_text > 0xffffffffull) return fail(ctx, "snfb_read_names: the names of one pass exceed 4 GiB of text (32-bit offsets); use smaller passes");
+    if (ctx->b_rn_text.ensure(n_text + 16) || ctx->h_rn_text.ensure(n_text + 16)) return fail(ctx, "snfb_read_names: out of memory for the text");
+    P.text = ctx->b_rn_text.as<uint8_t>();
+    mark(ctx, "rnames_copy");
+    if (nn) launch(ctx->launches, rnames::k_copy, grid_for(nn * 32, 256), 256, 0, st, P);
+    mark(ctx, nullptr);
+    if (nn) CUDA_TRY(cudaMemcpyAsync(h_off, P.off, 4 * nn, cudaMemcpyDeviceToHost, st));
+    if (n_text) CUDA_TRY(cudaMemcpyAsync(ctx->h_rn_text.p, P.text, n_text, cudaMemcpyDeviceToHost, st));
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, std::string("snfb_read_names: ") + cudaGetErrorString(e));
+    h_off[nn] = (uint32_t)n_text;
+    out->n_names = nn; out->n_text = n_text; out->text = ctx->h_rn_text.as<uint8_t>(); out->off = h_off; out->collisions = h_ctr[1];
     return 0;
 }
 

@@ -93,9 +93,11 @@ class SVCall:                              # field surface of sv.SVCall (sv.py:8
         self.postprocess = None
 
 
-def calls_from_result(res, task_index, lo, hi, contig_names, task_contig, task_id, config, rec_nm=None, want_leads=False):
-    """snfb_cand[lo:hi] of one task -> SVCall objects as they leave Task.call_candidates (sv.py:561-598)."""
+def calls_from_result(res, task_index, lo, hi, contig_names, task_contig, task_id, config, rec_nm=None, want_leads=False, names=None):
+    """snfb_cand[lo:hi] of one task -> SVCall objects as they leave Task.call_candidates (sv.py:561-598).  names: the run's
+    binding.ReadNames (--output-rnames), which fill SVCall.rnames; without them rnames stays None."""
     out = []
+    rnames = names.per_candidate(res.rn_off, lo, hi) if names is not None else None
     for k, c in enumerate(res.cand[lo:hi]):
         svtype = abi.SVTYPE_NAMES[int(c["svtype"])]
         info = {}
@@ -131,7 +133,7 @@ def calls_from_result(res, task_index, lo, hi, contig_names, task_contig, task_i
                          ps_top=None if c["ps_top_null"] else int(c["ps_top"]), ps_support=int(c["ps_support"]), ps_other=int(c["ps_other"]))
         call = SVCall(contig=task_contig, pos=int(c["pos"]), id=f"{svtype}.{k:X}S{task_id:X}", ref="N", alt=alt, qual=int(c["qual"]), filter="PASS",
                       info=info, svtype=svtype, svlen=int(c["svlen"]), end=int(c["end"]), genotypes={}, precise=bool(c["precise"]),
-                      support=int(c["support"]), rnames=None, qc=True, nm=float(c["nm_mean"]), postprocess=cv, fwd=int(c["fwd"]), rev=int(c["rev"]),
+                      support=int(c["support"]), rnames=None if rnames is None else rnames[k], qc=True, nm=float(c["nm_mean"]), postprocess=cv, fwd=int(c["fwd"]), rev=int(c["rev"]),
                       coverage_upstream=int(c["cov_upstream"]), coverage_downstream=int(c["cov_downstream"]), coverage_start=int(c["cov_start"]),
                       coverage_center=int(c["cov_center"]), coverage_end=int(c["cov_end"]), bnd_info=bnd, cand_index=lo + k)
         if svtype == "INS" and int(c["alt_off"]) >= 0 and not config.symbolic:

@@ -79,6 +79,16 @@ class BlockRun:
     cand_range: list          # per task (lo, hi) into result.cand
     rec_nm: Optional[np.ndarray] = None
     genotype: Optional[dict] = None   # per task index: snfb_genotype_targets results of the task's targets (genotype.device_targets)
+    read_names: Optional[binding.ReadNames] = None    # with --output-rnames: the candidates' read names (read_names)
+
+
+def read_names(ctx):
+    """the read names of the run resident on `ctx` (snfb_read_names), a warning logged when two reads of a candidate share a 64-bit name hash"""
+    names = ctx.read_names()
+    if names.collisions:
+        logging.warning(f"{names.collisions} supporting read(s) share a 64-bit read name hash with another read of their SV candidate: "
+                        "RNAMES lists one name per hash")
+    return names
 
 
 def run_block(block, config, device: int = 0, ctx=None) -> BlockRun:
@@ -88,7 +98,8 @@ def run_block(block, config, device: int = 0, ctx=None) -> BlockRun:
     ctx.load(block)
     res = ctx.run(want_leads=True, want_cands=True, want_seqs=True)
     rec_nm = abi.view(res._rec_nm_ptr, "<f8", len(block.rec)).copy() if getattr(res, "_rec_nm_ptr", None) else None
-    return BlockRun(block, res, cand_ranges(res.cand, len(block.task)), rec_nm)
+    names = read_names(ctx) if getattr(config, "output_rnames", False) else None
+    return BlockRun(block, res, cand_ranges(res.cand, len(block.task)), rec_nm, read_names=names)
 
 
 def cand_ranges(cand, n_task):
@@ -263,11 +274,14 @@ class Task:
             r = br.result
             r.cand, r.cand_leads, r.rnames, r.rn_off, r.task_cov_mean, r.alt = cv.cand, cv.cand_leads, cv.rnames, cv.rn_off, cv.task_cov_mean, sv.alt
             br.cand_range = cand_ranges(r.cand, len(br.block.task))
+            if getattr(config, "output_rnames", False):
+                br.read_names = read_names(ctx)
             self._staged = False
         lo, hi = br.cand_range[self.task_index]
         need_leads = bool(config.mosaic) or bool(config.phase)
         calls = postprocess.calls_from_result(br.result, self.task_index, lo, hi, br.block.contig_names, self.contig, self.id, config,
-                                              rec_nm=br.rec_nm, want_leads=need_leads)
+                                              rec_nm=br.rec_nm, want_leads=need_leads,
+                                              names=br.read_names if getattr(config, "output_rnames", False) else None)
         self.sv_id += len(calls)
         self.coverage_average_total = float(br.result.task_cov_mean[self.task_index])
         return calls
