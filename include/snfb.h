@@ -397,6 +397,9 @@ int         snfb_device_alt(snfb_ctx* ctx, void** dptr, uint64_t* n_bytes);
 uint64_t    snfb_launch_count(snfb_ctx* ctx);
 /* number of times a run was repeated because a buffer capacity was too small or a chain cut had to be undone */
 uint64_t    snfb_rerun_count(snfb_ctx* ctx);
+/* the number of slices (1 to 8, default 2) stage C runs in: candidates cut to about equal consensus work, each slice's ALT bytes copied
+ * to the host while the next slice runs.  The results do not depend on it; it changes the launches and the copy schedule. */
+int         snfb_set_consensus_slices(snfb_ctx* ctx, int k);
 /* mean coverage of consecutive `binsize`-base bins over the whole contig of one task, as the SNF writer stores it
  * (snf.py:248-267: the coverage vector zero-padded to a multiple of binsize, row means; the writer rounds them).  With an N mask
  * loaded, positions inside the task's runs (clipped to the task region) count 0, as in the masked vector (leadprov.py:470).

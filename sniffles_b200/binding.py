@@ -19,7 +19,7 @@ EXPORTS = ["snfb_version", "snfb_sizeof", "snfb_hash_name", "snfb_ctx_create", "
            "snfb_nccl_unique_id", "snfb_comm_init", "snfb_allgather_candidates", "snfb_selftest_sqrt_frac", "snfb_poa", "snfb_combine_groups", "snfb_combine_plan", "snfb_selftest_edit_distance",
            "snfb_load_bam", "snfb_set_regions", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf", "snfb_deflate_bgzf",
            "snfb_genotype_targets", "snfb_load_reference", "snfb_reference_runs", "snfb_fetch_reference",
-           "snfb_population_load", "snfb_population_match", "snfb_read_names"]
+           "snfb_population_load", "snfb_population_match", "snfb_read_names", "snfb_set_consensus_slices"]
 
 
 def lib():
@@ -59,6 +59,7 @@ def lib():
         L.snfb_unpin_host.argtypes = [C.c_void_p]
         L.snfb_rerun_count.restype = C.c_uint64
         L.snfb_rerun_count.argtypes = [C.c_void_p]
+        L.snfb_set_consensus_slices.argtypes = [C.c_void_p, C.c_int]
         L.snfb_coverage_bins.argtypes = [C.c_void_p, C.c_uint32, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
         L.snfb_nccl_unique_id.argtypes = [C.c_void_p]
         L.snfb_comm_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
@@ -298,6 +299,10 @@ class Context:
 
     def rerun_count(self):
         return int(self._lib.snfb_rerun_count(self._h))
+
+    def set_consensus_slices(self, k: int):
+        """snfb_set_consensus_slices: run stage C in k slices (1 to 8); the results are the same for every k"""
+        self._check(self._lib.snfb_set_consensus_slices(self._h, int(k)), "snfb_set_consensus_slices")
 
     def coverage_bins(self, task: int, binsize: int) -> np.ndarray:
         """Mean coverage per `binsize` bases over the task's contig (snf.py:248-267); the SNF writer rounds them."""

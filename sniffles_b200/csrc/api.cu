@@ -96,6 +96,8 @@ struct Caps { unsigned long long lead = 0, cand = 0, cand_lead = 0, rn = 0, alt 
 
 struct snfb_ctx {
     int device = 0; cudaStream_t st = nullptr, st_copy = nullptr, st_side = nullptr; cudaEvent_t ev_b = nullptr, ev_mid = nullptr, ev_fork = nullptr, ev_join = nullptr; std::string err;
+    // stage C slices: each one's k_align / k_vote has ended
+    cudaEvent_t ev_aligned[consensus::MAX_SLICES] = {}, ev_slice[consensus::MAX_SLICES] = {}; int n_slices = consensus::DEFAULT_SLICES;
     snfb_config cfg{}; bool have_cfg = false;
     // records
     bool loaded = false, on_device = false, seq_on_demand = false; const uint8_t* h_seq = nullptr; uint32_t evt_min = 0;     // E-bit threshold of the loaded CIGAR16 arena
@@ -127,11 +129,11 @@ struct snfb_ctx {
     snfb_lead* leads; extract::Event* ev_buf; snfb_lead* sorted_leads; uint32_t* radix_hist;
     cluster::B B{};
     // stage C (arena_c)
-    consensus::C Cc{}; consensus::SeqReq* seq_req; uint32_t* arena_off; uint8_t* seq_arena;
+    consensus::C Cc{}; consensus::SeqReq* seq_req; uint32_t* arena_off; uint8_t* seq_arena; uint32_t* q_scan_tmp;
     HostBuf h_seq_req, h_seq_arena; uint64_t seq_h2d_bytes = 0;
     bool stage_a_done = false, stage_b_done = false, stage_c_done = false;
     // host staging
-    HostBuf h_ctr_buf; DevCounters* h_mid = nullptr; DevCounters* h_fin = nullptr; uint32_t* h_work = nullptr;
+    HostBuf h_ctr_buf; DevCounters* h_mid = nullptr; DevCounters* h_fin = nullptr; consensus::Work* h_work = nullptr;      // h_work[0] read with h_mid, h_work[1] with h_fin
     HostBuf h_leads, h_task_reads, h_task_nm, h_rec_nm, h_cand, h_cand_leads, h_rnames, h_rn_off, h_task_cov, h_task_cov_raw, h_alt, h_cov_bins;
     // gather
     void* comm = nullptr; int rank = 0, nranks = 1; DevBuf b_gsend, b_grecv; HostBuf h_gather, h_gather_out; unsigned long long gather_cap = 0;     // h_gather: layout words, header table, rank_n_cand; h_gather_out: the merged arrays
@@ -285,10 +287,12 @@ int snfb_ctx_create(int device, snfb_ctx** out) {
         || cudaStreamCreateWithFlags(&ctx->st_side, cudaStreamNonBlocking) != cudaSuccess) { delete ctx; return 4; }
     cudaEventCreateWithFlags(&ctx->ev_b, cudaEventDisableTiming); cudaEventCreateWithFlags(&ctx->ev_mid, cudaEventDisableTiming);
     cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming); cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming);
+    for (int i = 0; i < consensus::MAX_SLICES; ++i) { cudaEventCreateWithFlags(&ctx->ev_aligned[i], cudaEventDisableTiming); cudaEventCreateWithFlags(&ctx->ev_slice[i], cudaEventDisableTiming); }
     for (int i = 0; i <= MAX_TIMINGS; ++i) cudaEventCreate(&ctx->ev[i]);
-    if (ctx->h_ctr_buf.ensure(2 * sizeof(DevCounters) + 256) || ctx->b_ctr.ensure(sizeof(DevCounters) + 64)) { delete ctx; return 5; }
-    ctx->h_mid = ctx->h_ctr_buf.as<DevCounters>(); ctx->h_fin = ctx->h_mid + 1; ctx->h_work = reinterpret_cast<uint32_t*>(ctx->h_fin + 1);
-    memset(ctx->h_ctr_buf.p, 0, 2 * sizeof(DevCounters) + 256);
+    const size_t ctr_bytes = 2 * sizeof(DevCounters) + 2 * sizeof(consensus::Work);
+    if (ctx->h_ctr_buf.ensure(ctr_bytes) || ctx->b_ctr.ensure(sizeof(DevCounters) + 64)) { delete ctx; return 5; }
+    ctx->h_mid = ctx->h_ctr_buf.as<DevCounters>(); ctx->h_fin = ctx->h_mid + 1; ctx->h_work = reinterpret_cast<consensus::Work*>(ctx->h_fin + 1);
+    memset(ctx->h_ctr_buf.p, 0, ctr_bytes);
     cudaFuncSetAttribute(cluster::k_cluster_warp<cluster::SMALL_CAP, cluster::CWS_WARPS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cluster::CwCfg<cluster::SMALL_CAP, cluster::CWS_WARPS>::smem);
     cudaFuncSetAttribute(cluster::k_cluster_warp<cluster::WARP_CAP, cluster::CWM_WARPS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cluster::CwCfg<cluster::WARP_CAP, cluster::CWM_WARPS>::smem);
     cudaFuncSetAttribute(cluster::k_cluster_block, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cluster::CB_SMEM);
@@ -303,6 +307,7 @@ void snfb_ctx_destroy(snfb_ctx* ctx) {
     if (ctx->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(ctx->comm);
     for (int i = 0; i <= MAX_TIMINGS; ++i) cudaEventDestroy(ctx->ev[i]);
     cudaEventDestroy(ctx->ev_b); cudaEventDestroy(ctx->ev_mid); cudaEventDestroy(ctx->ev_fork); cudaEventDestroy(ctx->ev_join);
+    for (int i = 0; i < consensus::MAX_SLICES; ++i) { cudaEventDestroy(ctx->ev_aligned[i]); cudaEventDestroy(ctx->ev_slice[i]); }
     cudaStreamDestroy(ctx->st_side); cudaStreamDestroy(ctx->st_copy); cudaStreamDestroy(ctx->st);
     delete ctx;      // frees every buffer
 }
@@ -755,7 +760,8 @@ static void carve_c(snfb_ctx* ctx, Carver& c) {
     b.cand = c.take<snfb_cand>(k.cand + 1); b.cand_leads = c.take<snfb_lead>(k.cand_lead + 1); b.out_plo = c.take<uint32_t>(k.cand_lead + 1); b.out_pn = c.take<uint32_t>(k.cand_lead + 1);
     b.rnames = c.take<uint64_t>(k.rn + 1); b.rn_off_out = c.take<uint32_t>(k.cand + 2);
     cc.plan_best = c.take<uint32_t>(k.cand + 1); cc.plan_nother = c.take<uint32_t>(k.cand + 1); cc.plan_otot = c.take<uint32_t>(k.cand + 1); cc.alt_len = c.take<uint32_t>(k.cand + 1); cc.scr_len = c.take<uint32_t>(k.cand + 1);
-    cc.alt_off = c.take<uint32_t>(k.cand + 1); cc.scr_off = c.take<uint32_t>(k.cand + 1); cc.work_big = c.take<uint32_t>(k.cand + 1); cc.work_small = c.take<uint32_t>(k.cand + 1); cc.work_ctr = c.take<uint32_t>(64);
+    cc.alt_off = c.take<uint32_t>(k.cand + 1); cc.scr_off = c.take<uint32_t>(k.cand + 1); cc.work_big = c.take<uint32_t>(k.cand + 1); cc.work_small = c.take<uint32_t>(k.cand + 1); cc.work = c.take<consensus::Work>(1);
+    cc.q_cnt = c.take<uint32_t>(consensus::NQ * (k.cand + 1)); cc.q_off = c.take<uint32_t>(consensus::NQ * (k.cand + 1)); ctx->q_scan_tmp = c.take<uint32_t>(consensus::NQ * prims::scan_tmp_elems(k.cand));
     cc.items_big = c.take<consensus::C::Item>(k.item + 1); cc.items_small = c.take<consensus::C::Item>(k.item + 1); cc.tiles = c.take<uint2>(k.tile + 1);
     cc.alt = c.take<uint8_t>(k.alt + 64); cc.scr = c.take<uint8_t>(k.scr16 * 16 + 64);
     ctx->seq_req = c.take<consensus::SeqReq>(k.req + 1); ctx->seq_arena = c.take<uint8_t>(k.req16 * 16 + 64);
@@ -900,12 +906,14 @@ static int enqueue_stage_b(snfb_ctx* ctx) {
     launch(ctx->launches, cluster::k_coverage, NUM_SMS * 32, 128, 0, st, b);
     // consensus plan: best read per INS candidate, sizes and offsets of the ALT bytes and of the scratch; the candidate records are final after this
     consensus::C& c = ctx->Cc;
-    CUDA_TRY(cudaMemsetAsync(c.work_ctr, 0, 64, st));
+    CUDA_TRY(cudaMemsetAsync(c.work, 0, sizeof(consensus::Work), st));
     mark(ctx, "consensus_plan");
     launch(ctx->launches, consensus::k_plan, grid_for(ctx->cap.cand, 128), 128, 0, st, c);
     prims::exclusive_scan(ctx->launches, c.alt_len, c.alt_off, b.scan_tmp, &ctr->n_cand, ctx->cap.cand, &ctr->n_alt_bytes, st);
     prims::exclusive_scan(ctx->launches, c.scr_len, c.scr_off, b.scan_tmp, &ctr->n_cand, ctx->cap.cand, &ctr->n_seq_bytes, st);
+    prims::exclusive_scan_cols(ctx->launches, c.q_cnt, c.q_off, ctx->cap.cand + 1, consensus::NQ, ctx->q_scan_tmp, &ctr->n_cand, ctx->cap.cand, c.work->n, st);
     launch(ctx->launches, consensus::k_plan_finish, grid_for(ctx->cap.cand, 128), 128, 0, st, c);
+    launch(ctx->launches, consensus::k_plan_slices, 1, 32, 0, st, c, ctx->n_slices);
     mark(ctx, nullptr);
     CUDA_TRY(cudaGetLastError());
     return 0;
@@ -941,12 +949,25 @@ static int enqueue_stage_c(snfb_ctx* ctx) {
         }
         c.seq = ctx->seq_arena; c.arena_off = ctx->arena_off;
     }
-    mark(ctx, "consensus");
-    launch(ctx->launches, consensus::k_prep, NUM_SMS * 8, 128, 0, st, c);
-    mark(ctx, "consensus_align");
-    launch(ctx->launches, consensus::k_align, NUM_SMS * 7, consensus::ALIGN_WARPS * 32, 0, st, c);
-    mark(ctx, "consensus_vote");
-    launch(ctx->launches, consensus::k_vote, NUM_SMS * 16, consensus::VOTE_THREADS, 0, st, c);
+    // Slice by slice, the slices alternating between the main and the side stream.  The slices share no candidate, scratch or ALT byte, so
+    // a slice's k_prep and k_align only wait for the previous slice's k_align: they fill the SMs while it votes, and the slices still end
+    // in order.  The event after a slice's vote lets the copy stream take its ALT bytes while the next slice runs.  The marks are on the
+    // main stream: together they span the whole stage (the interval of a vote there runs until the next slice on the main stream starts,
+    // or until the side stream has finished).
+    CUDA_TRY(cudaEventRecord(ctx->ev_fork, st)); CUDA_TRY(cudaStreamWaitEvent(ctx->st_side, ctx->ev_fork, 0));
+    for (int s = 0; s < ctx->n_slices; ++s) {
+        cudaStream_t ss = (s & 1) ? ctx->st_side : st; const bool on_main = ss == st;
+        if (s) CUDA_TRY(cudaStreamWaitEvent(ss, ctx->ev_aligned[s - 1], 0));
+        if (on_main) mark(ctx, "consensus");
+        launch(ctx->launches, consensus::k_prep, NUM_SMS * 8, 128, 0, ss, c, s);
+        if (on_main) mark(ctx, "consensus_align");
+        launch(ctx->launches, consensus::k_align, NUM_SMS * 7, consensus::ALIGN_WARPS * 32, 0, ss, c, s);
+        CUDA_TRY(cudaEventRecord(ctx->ev_aligned[s], ss));
+        if (on_main) mark(ctx, "consensus_vote");
+        launch(ctx->launches, consensus::k_vote, NUM_SMS * 16, consensus::VOTE_THREADS, 0, ss, c, s);
+        CUDA_TRY(cudaEventRecord(ctx->ev_slice[s], ss));
+    }
+    CUDA_TRY(cudaEventRecord(ctx->ev_join, ctx->st_side)); CUDA_TRY(cudaStreamWaitEvent(st, ctx->ev_join, 0));
     mark(ctx, nullptr);
     CUDA_TRY(cudaGetLastError());
     return 0;
@@ -972,7 +993,7 @@ static void initial_caps(snfb_ctx* ctx) {
 }
 static unsigned long long grown(unsigned long long need) { return need + need / 4 + 1024; }
 // does everything the counters report fit the capacities the run used?  If not, raise them (what was needed + 25 %).
-static bool caps_fit(snfb_ctx* ctx, const DevCounters& c, const uint32_t* work, int upto) {
+static bool caps_fit(snfb_ctx* ctx, const DevCounters& c, const consensus::Work& work, int upto) {
     Caps& k = ctx->cap; bool ok = true;
     const unsigned long long need_lead = std::max(c.n_slots, c.n_leads);
     if (need_lead > k.lead || c.lead_overflow) { k.lead = std::max(grown(need_lead), k.lead + k.lead / 2); ok = false; }
@@ -982,9 +1003,9 @@ static bool caps_fit(snfb_ctx* ctx, const DevCounters& c, const uint32_t* work, 
         if (c.n_rnames > k.rn) { k.rn = grown(c.n_rnames); ok = false; }
         if (c.n_alt_bytes > k.alt) { k.alt = grown(c.n_alt_bytes); ok = false; }
         if (c.n_seq_bytes > k.scr16) { k.scr16 = grown(c.n_seq_bytes); ok = false; }
-        const unsigned long long items = std::max(work[4], work[5]);
+        const unsigned long long items = std::max(work.n[consensus::Q_HEAVY], work.n[consensus::Q_LIGHT]);
         if (items > k.item) { k.item = grown(items); ok = false; }
-        if (work[8] > k.tile) { k.tile = grown(work[8]); ok = false; }
+        if (work.n[consensus::Q_TILE] > k.tile) { k.tile = grown(work.n[consensus::Q_TILE]); ok = false; }
     }
     if (upto >= 3) {
         if (c.n_req > k.req) { k.req = grown(c.n_req); ok = false; }
@@ -1042,6 +1063,56 @@ static const char* fatal_counter(const DevCounters& c) {
     if (c.ordinal_overflow) return "a read carries more than 65535 SV signatures (16-bit lead ordinal)";
     return nullptr;
 }
+// every copy and kernel of the context has ended: before buffers they use may be reallocated, and before an error return
+static void drain(snfb_ctx* ctx) { cudaStreamSynchronize(ctx->st); cudaStreamSynchronize(ctx->st_side); cudaStreamSynchronize(ctx->st_copy); }
+static int run_attempts(snfb_ctx* ctx, int upto, snfb_cand_view* cands, snfb_seq_view* seqs) {
+    for (int attempt = 0; ; ++attempt) {
+        if (attempt == 6) return fail(ctx, "buffer capacities did not converge");
+        if (ensure_arenas(ctx)) return 1;
+        bind_inputs(ctx);
+        ctx->n_ev = ctx->n_ev_load;
+        cudaStream_t st = ctx->st; DevCounters* ctr = ctx->B.ctr;
+        if (enqueue_stage_a(ctx)) return 1;
+        bool mid = false;
+        if (upto >= 2) {
+            if (enqueue_stage_b(ctx)) return 1;
+            // the host reads the counters and the slice table on the copy stream while the consensus kernels run
+            CUDA_TRY(cudaEventRecord(ctx->ev_b, st)); CUDA_TRY(cudaStreamWaitEvent(ctx->st_copy, ctx->ev_b, 0));
+            CUDA_TRY(cudaMemcpyAsync(ctx->h_mid, ctr, sizeof(DevCounters), cudaMemcpyDeviceToHost, ctx->st_copy));
+            CUDA_TRY(cudaMemcpyAsync(&ctx->h_work[0], ctx->Cc.work, sizeof(consensus::Work), cudaMemcpyDeviceToHost, ctx->st_copy));
+            CUDA_TRY(cudaEventRecord(ctx->ev_mid, ctx->st_copy));
+            mid = true;
+        }
+        if (upto >= 3 && !ctx->seq_on_demand) { if (enqueue_stage_c(ctx)) return 1; }
+        if (mid) {
+            CUDA_TRY(cudaEventSynchronize(ctx->ev_mid));
+            if (const char* m = fatal_counter(*ctx->h_mid)) return fail(ctx, m);
+            if (!caps_fit(ctx, *ctx->h_mid, ctx->h_work[0], 2)) { drain(ctx); ++ctx->reruns; continue; }
+            if (ctx->h_mid->unverified_breaks && !ctx->force_no_cuts) { drain(ctx); ctx->force_no_cuts = true; ++ctx->reruns; continue; }   // a chain cut was wrong: redo with whole chains
+            if (cands) { if (enqueue_cand_copies(ctx, *ctx->h_mid, ctx->st_copy)) return 1; }
+            if (upto >= 3 && ctx->seq_on_demand) { if (enqueue_stage_c(ctx)) return 1; }
+        }
+        if (upto >= 3 && seqs) {
+            // each slice's ALT bytes, behind the candidate copies, as soon as its vote has ended
+            const unsigned long long na = ctx->h_mid->n_alt_bytes;
+            if (ctx->h_alt.ensure(na + 16)) return fail(ctx, "out of pinned memory for the ALT arena");
+            for (int s = 0; s < ctx->n_slices; ++s) {
+                const consensus::Slice& sl = ctx->h_work[0].slice[s];
+                if (sl.alt_hi <= sl.alt_lo) continue;
+                CUDA_TRY(cudaStreamWaitEvent(ctx->st_copy, ctx->ev_slice[s], 0));
+                CUDA_TRY(cudaMemcpyAsync(ctx->h_alt.as<uint8_t>() + sl.alt_lo, ctx->Cc.alt + sl.alt_lo, sl.alt_hi - sl.alt_lo, cudaMemcpyDeviceToHost, ctx->st_copy));
+            }
+        }
+        CUDA_TRY(cudaMemcpyAsync(ctx->h_fin, ctr, sizeof(DevCounters), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(&ctx->h_work[1], ctx->Cc.work, sizeof(consensus::Work), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        CUDA_TRY(cudaStreamSynchronize(ctx->st_copy));
+        CUDA_TRY(cudaGetLastError());
+        if (const char* m = fatal_counter(*ctx->h_fin)) return fail(ctx, m);
+        if (!caps_fit(ctx, *ctx->h_fin, ctx->h_work[upto >= 2 ? 1 : 0], upto)) { ++ctx->reruns; continue; }
+        return 0;
+    }
+}
 // upto: 1 = stage A (+ sort and bins), 2 = + stage B and the consensus plan, 3 = + consensus.
 static int run_pipeline(snfb_ctx* ctx, int upto, snfb_lead_view* leads, snfb_cand_view* cands, snfb_seq_view* seqs) {
     if (!ctx->loaded) return fail(ctx, "no records loaded");
@@ -1050,46 +1121,7 @@ static int run_pipeline(snfb_ctx* ctx, int upto, snfb_lead_view* leads, snfb_can
     for (uint32_t t = 0; t < ctx->n_task; ++t) if ((long long)ctx->tasks[t].contig_len / ctx->cfg.cluster_binsize >= (1ll << 26)) return fail(ctx, "contig_len / cluster_binsize must stay below 2^26 (bin field of the sort key)");
     initial_caps(ctx);
     ctx->stage_a_done = ctx->stage_b_done = ctx->stage_c_done = false;
-    for (int attempt = 0; ; ++attempt) {
-        if (attempt == 6) return fail(ctx, "buffer capacities did not converge");
-        if (ensure_arenas(ctx)) return 1;
-        bind_inputs(ctx);
-        ctx->n_ev = ctx->n_ev_load;
-        cudaStream_t st = ctx->st; DevCounters* ctr = ctx->B.ctr;
-        if (enqueue_stage_a(ctx)) return 1;
-        bool mid = false, copies = false;
-        if (upto >= 2) {
-            if (enqueue_stage_b(ctx)) return 1;
-            // the host reads the counters on the copy stream while the consensus kernels run
-            CUDA_TRY(cudaEventRecord(ctx->ev_b, st)); CUDA_TRY(cudaStreamWaitEvent(ctx->st_copy, ctx->ev_b, 0));
-            CUDA_TRY(cudaMemcpyAsync(ctx->h_mid, ctr, sizeof(DevCounters), cudaMemcpyDeviceToHost, ctx->st_copy));
-            CUDA_TRY(cudaMemcpyAsync(ctx->h_work, ctx->Cc.work_ctr, 64, cudaMemcpyDeviceToHost, ctx->st_copy));
-            CUDA_TRY(cudaEventRecord(ctx->ev_mid, ctx->st_copy));
-            mid = true;
-        }
-        if (upto >= 3 && !ctx->seq_on_demand) { if (enqueue_stage_c(ctx)) return 1; }
-        if (mid) {
-            CUDA_TRY(cudaEventSynchronize(ctx->ev_mid));
-            if (const char* m = fatal_counter(*ctx->h_mid)) { cudaStreamSynchronize(st); return fail(ctx, m); }
-            if (!caps_fit(ctx, *ctx->h_mid, ctx->h_work, 2)) { CUDA_TRY(cudaStreamSynchronize(st)); ++ctx->reruns; continue; }
-            if (ctx->h_mid->unverified_breaks && !ctx->force_no_cuts) { CUDA_TRY(cudaStreamSynchronize(st)); ctx->force_no_cuts = true; ++ctx->reruns; continue; }   // a chain cut was wrong: redo with whole chains
-            if (cands) { if (enqueue_cand_copies(ctx, *ctx->h_mid, ctx->st_copy)) return 1; copies = true; }
-            if (upto >= 3 && ctx->seq_on_demand) { if (enqueue_stage_c(ctx)) return 1; }
-        }
-        if (upto >= 3 && seqs) {
-            const unsigned long long na = ctx->h_mid->n_alt_bytes;
-            if (ctx->h_alt.ensure(na + 16)) return fail(ctx, "out of pinned memory for the ALT arena");
-            if (na) CUDA_TRY(cudaMemcpyAsync(ctx->h_alt.p, ctx->Cc.alt, na, cudaMemcpyDeviceToHost, st));
-        }
-        CUDA_TRY(cudaMemcpyAsync(ctx->h_fin, ctr, sizeof(DevCounters), cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaMemcpyAsync(ctx->h_work + 16, ctx->Cc.work_ctr, 64, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        if (copies) CUDA_TRY(cudaStreamSynchronize(ctx->st_copy));
-        CUDA_TRY(cudaGetLastError());
-        if (const char* m = fatal_counter(*ctx->h_fin)) return fail(ctx, m);
-        if (!caps_fit(ctx, *ctx->h_fin, upto >= 2 ? ctx->h_work + 16 : ctx->h_work, upto)) { ++ctx->reruns; continue; }
-        break;
-    }
+    if (run_attempts(ctx, upto, cands, seqs)) { drain(ctx); return 1; }
     ctx->stage_a_done = true; ctx->stage_b_done = upto >= 2; ctx->stage_c_done = upto >= 3;
     if (leads) { memset(leads, 0, sizeof *leads); if (fill_lead_view(ctx, leads)) return 1; }
     if (cands) { memset(cands, 0, sizeof *cands); finish_cand_view(ctx, *ctx->h_fin, cands); }
@@ -1146,6 +1178,11 @@ int snfb_device_alt(snfb_ctx* ctx, void** dptr, uint64_t* n_bytes) {
 uint64_t snfb_launch_count(snfb_ctx* ctx) { return ctx ? ctx->launches : 0; }
 double snfb_selftest_sqrt_frac(uint64_t p_hi, uint64_t p_lo, uint64_t q, int slow) { const u128 P = ((u128)p_hi << 64) | p_lo; return slow ? sqrt_frac_rn_slow(P, q) : sqrt_frac_rn(P, q); }
 uint64_t snfb_rerun_count(snfb_ctx* ctx) { return ctx ? ctx->reruns : 0; }
+int snfb_set_consensus_slices(snfb_ctx* ctx, int k) {
+    if (!ctx) return 1;
+    if (k < 1 || k > consensus::MAX_SLICES) return fail(ctx, "snfb_set_consensus_slices: k must be 1 to 8");
+    ctx->n_slices = k; return 0;
+}
 int snfb_pin_host(void* p, size_t bytes) { return cudaHostRegister(p, bytes, cudaHostRegisterDefault) == cudaSuccess ? 0 : 1; }
 int snfb_unpin_host(void* p) { return cudaHostUnregister(p) == cudaSuccess ? 0 : 1; }
 

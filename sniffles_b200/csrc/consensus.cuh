@@ -15,6 +15,19 @@ constexpr uint8_t DASH = 0xff;
 // The light items run with the smaller per-warp hit arrays, i.e. with more warps per SM (they are latency bound).
 constexpr int MAXHIT = 512, MAXHIT_LIGHT = 384; constexpr uint32_t HEAVY_L = 3000;
 
+// The five work queues are written in candidate order, each candidate's entries at the exclusive scan of what the candidates before it
+// put there, so the entries of candidates [c_lo, c_hi) are one range of every queue.  Stage C runs in slices of candidates cut to about
+// equal scratch (rows x length, i.e. work): the kernels of a slice take only its ranges, and its ALT bytes [alt_lo, alt_hi) are final
+// when its k_vote ends, so they can go to the host while the next slice runs.
+enum { Q_BIG, Q_SMALL, Q_HEAVY, Q_LIGHT, Q_TILE, NQ };      // prep queues (candidates), align queues (items), vote queue (tiles)
+constexpr int MAX_SLICES = 8, DEFAULT_SLICES = 2;
+struct Slice { uint32_t c_lo, c_hi; uint32_t lo[NQ], hi[NQ]; unsigned long long alt_lo, alt_hi; };
+struct Work {
+    unsigned long long n[NQ];                 // queue lengths (the scans' totals; may exceed the capacities: the run is redone)
+    uint32_t pos[MAX_SLICES][4];              // per slice: next prep candidate, heavy item, light item, vote tile
+    Slice slice[MAX_SLICES];
+};
+
 struct C {
     const snfb_cand* cand; snfb_cand* cand_rw; const snfb_lead* cand_leads;
     const uint32_t* out_plo; const uint32_t* out_pn;     // per candidate lead: the run of `ord` entries (merge_inner parts) it was folded from
@@ -23,7 +36,8 @@ struct C {
     const uint32_t* arena_off;       // seq on demand: per kept lead, 16-byte unit offset of its bytes in `seq` (which then is the compact arena); nullptr = full arena
     uint32_t* plan_best; uint32_t* plan_nother; uint32_t* plan_otot; uint32_t* alt_len; uint32_t* scr_len; uint32_t* alt_off; uint32_t* scr_off;   // scr in units of 16 bytes
     uint8_t* alt; uint8_t* scr; unsigned long long alt_cap, scr_cap16, cand_cap;
-    uint32_t* work_big; uint32_t* work_small; uint32_t* work_ctr;      // work_ctr: [0] n_big, [1] n_small, [2],[3] queue positions, [4] n_items_big, [5] n_items_small, [6],[7] item queue positions, [8] n_tiles, [9] tile queue position
+    uint32_t* work_big; uint32_t* work_small; Work* work;
+    uint32_t* q_cnt; uint32_t* q_off;     // per queue (Q_*) one column of cand_cap + 1 entries: what each candidate puts in the queue, its scanned position
     // item pipeline: one (candidate, supporting read) pair per warp, one (candidate, column tile) per block
     struct Item { uint32_t cand; uint32_t k; uint32_t row; uint32_t rd_off; };
     Item* items_big; Item* items_small; uint2* tiles; unsigned long long item_cap, tile_cap;
@@ -36,7 +50,7 @@ __device__ __forceinline__ uint8_t seq_code(const uint8_t* sq, long long q) { co
 __global__ void k_plan(C c) {
     const unsigned long long nc = c.ctr->n_cand < c.cand_cap ? c.ctr->n_cand : c.cand_cap;
     for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < nc; i += (unsigned long long)gridDim.x * blockDim.x) {
-        uint32_t al = 0, sl = 0;
+        uint32_t al = 0, sl = 0, heavy_n = 0, light_n = 0, tiles = 0; bool big = false;
         if (c.cand[i].svtype == SNFB_INS && !c.cfg.symbolic) {
             const snfb_cand* cd = &c.cand[i]; long nm = 0, bi = -1; long long bd = 0; long long tot = 0;
             for (int k = 0; k < cd->lead_n; ++k) { const snfb_lead* l = &c.cand_leads[cd->lead_off + k]; if (!(l->flags & SNFB_LF_HAS_SEQ)) continue;
@@ -51,31 +65,55 @@ __global__ void k_plan(C c) {
                 const unsigned long long bytes = cons ? (unsigned long long)tot + 8 + (unsigned long long)(nm - 1) * ((L + 3u) & ~3u) + (unsigned long long)(nm - 1) * 16 + 64 + 16 + TAB * 8 : (unsigned long long)L + 24;
                 sl = (uint32_t)((bytes + 15) / 16);
                 c.cand_rw[i].alt_len = (int)L;
-                // work queue: the heavy tail (long insertions with many reads) is scheduled first
-                const unsigned long long work = (unsigned long long)L * (unsigned long long)nm;
-                if (work > 60000ull) c.work_big[atomicAdd(&c.work_ctr[0], 1u)] = (uint32_t)i; else c.work_small[atomicAdd(&c.work_ctr[1], 1u)] = (uint32_t)i;
-                if (cons) {
-                    // one work item per supporting read (heavy rows first) and one per 4096-column tile of the vote
-                    const bool heavy = L > HEAVY_L; C::Item* dst = heavy ? c.items_big : c.items_small;
-                    const uint32_t base = atomicAdd(&c.work_ctr[heavy ? 4 : 5], (uint32_t)(nm - 1));
-                    uint32_t row = 0, ro = 0;
-                    for (int k = 0; k < cd->lead_n; ++k) { const snfb_lead* l = &c.cand_leads[cd->lead_off + k]; if (!(l->flags & SNFB_LF_HAS_SEQ) || k == bi) continue;
-                        if ((unsigned long long)base + row < c.item_cap) { C::Item it; it.cand = (uint32_t)i; it.k = (uint32_t)k; it.row = row; it.rd_off = ro; dst[base + row] = it; }
-                        ++row; ro += ((uint32_t)l->seq_len + 7u) & ~7u; }
-                    const uint32_t nt = (L + 4095u) / 4096u; const uint32_t tb = atomicAdd(&c.work_ctr[8], nt);
-                    for (uint32_t t = 0; t < nt; ++t) if ((unsigned long long)tb + t < c.tile_cap) c.tiles[tb + t] = make_uint2((uint32_t)i, t);
-                }
+                // prep queue: the heavy tail (long insertions with many reads) is scheduled first; one align item per supporting read
+                // (heavy rows first) and one vote item per 4096-column tile
+                big = (unsigned long long)L * (unsigned long long)nm > 60000ull;
+                if (cons) { const bool heavy = L > HEAVY_L; heavy_n = heavy ? (uint32_t)(nm - 1) : 0u; light_n = heavy ? 0u : (uint32_t)(nm - 1); tiles = (L + 4095u) / 4096u; }
             }
         }
         c.alt_len[i] = al; c.scr_len[i] = sl;
+        const size_t col = c.cand_cap + 1;
+        c.q_cnt[Q_BIG * col + i] = sl && big; c.q_cnt[Q_SMALL * col + i] = sl && !big; c.q_cnt[Q_HEAVY * col + i] = heavy_n; c.q_cnt[Q_LIGHT * col + i] = light_n; c.q_cnt[Q_TILE * col + i] = tiles;
     }
 }
 
-// the candidate records are final once the ALT offsets are known (stage C only fills the ALT bytes)
+// the candidate records are final once the ALT offsets are known (stage C only fills the ALT bytes); every queue entry goes to its
+// scanned position
 __global__ void k_plan_finish(C c) {
-    const unsigned long long nc = c.ctr->n_cand < c.cand_cap ? c.ctr->n_cand : c.cand_cap;
-    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < nc; i += (unsigned long long)gridDim.x * blockDim.x)
-        if (c.scr_len[i]) c.cand_rw[i].alt_off = (int)c.alt_off[i];
+    const unsigned long long nc = c.ctr->n_cand < c.cand_cap ? c.ctr->n_cand : c.cand_cap; const size_t col = c.cand_cap + 1;
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < nc; i += (unsigned long long)gridDim.x * blockDim.x) {
+        if (!c.scr_len[i]) continue;
+        c.cand_rw[i].alt_off = (int)c.alt_off[i];
+        if (c.q_cnt[Q_BIG * col + i]) c.work_big[c.q_off[Q_BIG * col + i]] = (uint32_t)i; else c.work_small[c.q_off[Q_SMALL * col + i]] = (uint32_t)i;
+        const uint32_t nh = c.q_cnt[Q_HEAVY * col + i], no = nh + c.q_cnt[Q_LIGHT * col + i];
+        C::Item* dst = nh ? c.items_big : c.items_small; const uint32_t base = c.q_off[(nh ? Q_HEAVY : Q_LIGHT) * col + i];
+        const snfb_cand* cd = &c.cand[i]; const uint32_t bi = c.plan_best[i];
+        uint32_t row = 0, ro = 0;
+        for (int k = 0; no && k < cd->lead_n; ++k) { const snfb_lead* l = &c.cand_leads[cd->lead_off + k]; if (!(l->flags & SNFB_LF_HAS_SEQ) || (uint32_t)k == bi) continue;
+            if ((unsigned long long)base + row < c.item_cap) { C::Item it; it.cand = (uint32_t)i; it.k = (uint32_t)k; it.row = row; it.rd_off = ro; dst[base + row] = it; }
+            ++row; ro += ((uint32_t)l->seq_len + 7u) & ~7u; }
+        const uint32_t nt = c.q_cnt[Q_TILE * col + i], tb = c.q_off[Q_TILE * col + i];
+        for (uint32_t t = 0; t < nt; ++t) if ((unsigned long long)tb + t < c.tile_cap) c.tiles[tb + t] = make_uint2((uint32_t)i, t);
+    }
+}
+
+// the slices: thread s cuts at the first candidate whose scratch starts at or after s / k of the total, and reads every queue's and
+// the ALT arena's position there (the totals past the last candidate).  Slices may be empty.
+__global__ void k_plan_slices(C c, int k) {
+    const int s = threadIdx.x; if (s >= k) return;
+    const unsigned long long nc = c.ctr->n_cand < c.cand_cap ? c.ctr->n_cand : c.cand_cap; const size_t col = c.cand_cap + 1;
+    const unsigned long long tot = c.ctr->n_seq_bytes;
+    auto cut = [&](int j) -> uint32_t {
+        if (j <= 0) return 0; if (j >= k) return (uint32_t)nc;
+        const unsigned long long want = (tot * (unsigned long long)j + k - 1) / (unsigned long long)k;
+        uint32_t lo = 0, hi = (uint32_t)nc;
+        while (lo < hi) { const uint32_t m = (lo + hi) / 2; if (c.scr_off[m] < want) lo = m + 1; else hi = m; }
+        return lo;
+    };
+    Slice sl; sl.c_lo = cut(s); sl.c_hi = cut(s + 1);
+    for (int q = 0; q < NQ; ++q) { sl.lo[q] = sl.c_lo < nc ? c.q_off[q * col + sl.c_lo] : (uint32_t)c.work->n[q]; sl.hi[q] = sl.c_hi < nc ? c.q_off[q * col + sl.c_hi] : (uint32_t)c.work->n[q]; }
+    sl.alt_lo = sl.c_lo < nc ? c.alt_off[sl.c_lo] : c.ctr->n_alt_bytes; sl.alt_hi = sl.c_hi < nc ? c.alt_off[sl.c_hi] : c.ctr->n_alt_bytes;
+    c.work->slice[s] = sl;
 }
 
 // unpack `len` bases starting at nibble `off` of sq into dst (one code per byte); `tid`/`nthr` = cooperating threads.
@@ -323,13 +361,15 @@ __device__ __forceinline__ uint8_t* cand_table(const C& c, uint32_t ci, uint32_t
     return scr;
 }
 
-__global__ void __launch_bounds__(128) k_prep(C c) {
+// the kernels of stage C take slice `s` of every queue
+__global__ void __launch_bounds__(128) k_prep(C c, int s) {
     __shared__ uint32_t s_cand;
     static const char CODE[17] = "=ACMGRSVTWYHKDBN";
+    const Slice& sl = c.work->slice[s];
     for (;;) {
         __syncthreads();
-        if (threadIdx.x == 0) { const uint32_t q = atomicAdd(&c.work_ctr[2], 1u); const uint32_t nb = c.work_ctr[0], ns = c.work_ctr[1];
-            s_cand = q < nb ? c.work_big[q] : (q < nb + ns ? c.work_small[q - nb] : 0xffffffffu); }
+        if (threadIdx.x == 0) { const uint32_t q = atomicAdd(&c.work->pos[s][0], 1u); const uint32_t nb = sl.hi[Q_BIG] - sl.lo[Q_BIG], ns = sl.hi[Q_SMALL] - sl.lo[Q_SMALL];
+            s_cand = q < nb ? c.work_big[sl.lo[Q_BIG] + q] : (q < nb + ns ? c.work_small[sl.lo[Q_SMALL] + q - nb] : 0xffffffffu); }
         __syncthreads();
         const uint32_t ci = s_cand; if (ci == 0xffffffffu) break;
         const uint32_t L = c.alt_len[ci];
@@ -466,14 +506,15 @@ __device__ __forceinline__ void align_item(const C& c, const C::Item it, const G
 // Heavy items (long insertions) first, the whole block on one item (the longest insertion's reads are the tail of the step);
 // then the light items, one per warp.  Per-warp hit arrays of MAXHIT_LIGHT entries; a block item uses all of them as one array.
 constexpr int ALIGN_WARPS = 4;
-__global__ void __launch_bounds__(ALIGN_WARPS * 32, 7) k_align(C c) {
+__global__ void __launch_bounds__(ALIGN_WARPS * 32, 7) k_align(C c, int s) {
     __shared__ int sm[5][ALIGN_WARPS * MAXHIT_LIGHT]; __shared__ int s_red[2 * ALIGN_WARPS]; __shared__ uint32_t s_q;
     static_assert(ALIGN_WARPS * MAXHIT_LIGHT >= MAXHIT, "a block item needs MAXHIT entries");
     const int lane = lane_id(), warp = threadIdx.x >> 5;
-    const uint32_t nb = (uint32_t)min((unsigned long long)c.work_ctr[4], c.item_cap), ns = (uint32_t)min((unsigned long long)c.work_ctr[5], c.item_cap);
+    const Slice& sl = c.work->slice[s];
+    const uint32_t b0 = sl.lo[Q_HEAVY], nb = (uint32_t)min((unsigned long long)sl.hi[Q_HEAVY], c.item_cap), s0 = sl.lo[Q_LIGHT], ns = (uint32_t)min((unsigned long long)sl.hi[Q_LIGHT], c.item_cap);
     for (;;) {
         __syncthreads();
-        if (threadIdx.x == 0) s_q = atomicAdd(&c.work_ctr[6], 1u);
+        if (threadIdx.x == 0) s_q = b0 + atomicAdd(&c.work->pos[s][1], 1u);
         __syncthreads();
         const uint32_t q = s_q; if (q >= nb) break;
         BlockGrp<ALIGN_WARPS> g; g.tid = threadIdx.x; g.red = s_red;
@@ -481,7 +522,7 @@ __global__ void __launch_bounds__(ALIGN_WARPS * 32, 7) k_align(C c) {
     }
     __syncthreads();
     for (;;) {
-        uint32_t q = 0; if (lane == 0) q = atomicAdd(&c.work_ctr[7], 1u);
+        uint32_t q = 0; if (lane == 0) q = s0 + atomicAdd(&c.work->pos[s][2], 1u);
         q = __shfl_sync(FULL, q, 0);
         if (q >= ns) break;
         WarpGrp g; g.tid = lane; const int o = warp * MAXHIT_LIGHT;
@@ -499,12 +540,13 @@ __device__ __forceinline__ void vote_add(unsigned long long (&cnt)[4], uint32_t 
     for (int k = 0; k < 4; ++k) cnt[k] += sel == (uint32_t)k ? inc : 0ull;
 }
 constexpr int VOTE_THREADS = 64;      // most candidates are a few hundred columns: small blocks, many of them
-__global__ void __launch_bounds__(VOTE_THREADS) k_vote(C c) {
+__global__ void __launch_bounds__(VOTE_THREADS) k_vote(C c, int s) {
     __shared__ uint2 s_tile; __shared__ int s_nacc, s_nlist; __shared__ uint16_t s_rows[VOTE_LIST];
     static const char CODE[17] = "=ACMGRSVTWYHKDBN";
+    const Slice& sl = c.work->slice[s];
     for (;;) {
         __syncthreads();
-        if (threadIdx.x == 0) { const uint32_t q = atomicAdd(&c.work_ctr[9], 1u); s_tile = q < c.work_ctr[8] && q < c.tile_cap ? c.tiles[q] : make_uint2(0xffffffffu, 0); }
+        if (threadIdx.x == 0) { const uint32_t q = sl.lo[Q_TILE] + atomicAdd(&c.work->pos[s][3], 1u); s_tile = q < sl.hi[Q_TILE] && q < c.tile_cap ? c.tiles[q] : make_uint2(0xffffffffu, 0); }
         __syncthreads();
         const uint32_t ci = s_tile.x; if (ci == 0xffffffffu) break;
         const uint32_t L = c.alt_len[ci], no = c.plan_nother[ci];

@@ -37,10 +37,12 @@ __device__ inline uint32_t block_excl_scan(uint32_t v, uint32_t* total) {
     return r;
 }
 
+// The scans take blockIdx.y as a column: column y is in / out + y * stride, its tile sums tile_sum + y * gridDim.x, its total total_out[y].
 // pass 1: per-tile sums
 __global__ void __launch_bounds__(SCAN_THREADS) k_scan_reduce(const uint32_t* __restrict__ in, uint32_t* __restrict__ tile_sum,
-                                                              const unsigned long long* __restrict__ n_ptr, unsigned long long n_bound) {
+                                                              const unsigned long long* __restrict__ n_ptr, unsigned long long n_bound, size_t stride) {
     unsigned long long n = n_ptr ? *n_ptr : n_bound; if (n > n_bound) n = n_bound;
+    in += blockIdx.y * stride; tile_sum += (size_t)blockIdx.y * gridDim.x;
     unsigned long long base = (unsigned long long)blockIdx.x * SCAN_TILE;
     uint32_t s = 0;
     #pragma unroll
@@ -50,19 +52,20 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_scan_reduce(const uint32_t* __
 }
 // pass 2: exclusive scan of the tile sums by one block; writes the grand total to *total_out (64-bit)
 __global__ void __launch_bounds__(SCAN_THREADS) k_scan_tiles(uint32_t* __restrict__ tile_sum, int ntiles, unsigned long long* total_out) {
-    uint32_t carry = 0;
+    uint32_t carry = 0; tile_sum += (size_t)blockIdx.x * ntiles;
     for (int b = 0; b < ntiles; b += SCAN_THREADS) {
         int j = b + threadIdx.x; uint32_t v = j < ntiles ? tile_sum[j] : 0; uint32_t tot;
         uint32_t e = block_excl_scan(v, &tot);
         if (j < ntiles) tile_sum[j] = e + carry;
         carry += tot;
     }
-    if (threadIdx.x == 0 && total_out) *total_out = carry;
+    if (threadIdx.x == 0 && total_out) total_out[blockIdx.x] = carry;
 }
 // pass 3: per-tile exclusive scan plus tile offset.  Thread t owns SCAN_ITEMS consecutive elements.
 __global__ void __launch_bounds__(SCAN_THREADS) k_scan_down(const uint32_t* __restrict__ in, uint32_t* __restrict__ out, const uint32_t* __restrict__ tile_sum,
-                                                            const unsigned long long* __restrict__ n_ptr, unsigned long long n_bound) {
+                                                            const unsigned long long* __restrict__ n_ptr, unsigned long long n_bound, size_t stride) {
     unsigned long long n = n_ptr ? *n_ptr : n_bound; if (n > n_bound) n = n_bound;
+    in += blockIdx.y * stride; out += blockIdx.y * stride; tile_sum += (size_t)blockIdx.y * gridDim.x;
     unsigned long long base = (unsigned long long)blockIdx.x * SCAN_TILE + (unsigned long long)threadIdx.x * SCAN_ITEMS;
     uint32_t v[SCAN_ITEMS]; uint32_t s = 0;
     #pragma unroll
@@ -72,15 +75,19 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_scan_down(const uint32_t* __re
     for (int i = 0; i < SCAN_ITEMS; ++i) { if (base + i < n) out[base + i] = e; e += v[i]; }
 }
 
-// exclusive scan of in[0..n) into out (may alias in); total (u64) to *total_out if not null.
-// tmp must hold ceil(n_bound / SCAN_TILE) u32.  Launches are counted in `launches`.
+// exclusive scans of `cols` columns in[y * stride + 0..n) into out (may alias in), in the same three launches; the totals (u64) to
+// total_out[0..cols) if not null.  tmp must hold cols * ceil(n_bound / SCAN_TILE) u32.  Launches are counted in `launches`.
+inline void exclusive_scan_cols(uint64_t& launches, const uint32_t* in, uint32_t* out, size_t stride, int cols, uint32_t* tmp, const unsigned long long* n_ptr,
+                                unsigned long long n_bound, unsigned long long* total_out, cudaStream_t st) {
+    if (n_bound == 0) { if (total_out) cudaMemsetAsync(total_out, 0, 8 * cols, st); return; }
+    int ntiles = (int)((n_bound + SCAN_TILE - 1) / SCAN_TILE);
+    launch(launches, k_scan_reduce, dim3(ntiles, cols), SCAN_THREADS, 0, st, in, tmp, n_ptr, n_bound, stride);
+    launch(launches, k_scan_tiles, cols, SCAN_THREADS, 0, st, tmp, ntiles, total_out);
+    launch(launches, k_scan_down, dim3(ntiles, cols), SCAN_THREADS, 0, st, in, out, tmp, n_ptr, n_bound, stride);
+}
 inline void exclusive_scan(uint64_t& launches, const uint32_t* in, uint32_t* out, uint32_t* tmp, const unsigned long long* n_ptr, unsigned long long n_bound,
                            unsigned long long* total_out, cudaStream_t st) {
-    if (n_bound == 0) { if (total_out) cudaMemsetAsync(total_out, 0, 8, st); return; }
-    int ntiles = (int)((n_bound + SCAN_TILE - 1) / SCAN_TILE);
-    launch(launches, k_scan_reduce, ntiles, SCAN_THREADS, 0, st, in, tmp, n_ptr, n_bound);
-    launch(launches, k_scan_tiles, 1, SCAN_THREADS, 0, st, tmp, ntiles, total_out);
-    launch(launches, k_scan_down, ntiles, SCAN_THREADS, 0, st, in, out, tmp, n_ptr, n_bound);
+    exclusive_scan_cols(launches, in, out, 0, 1, tmp, n_ptr, n_bound, total_out, st);
 }
 inline size_t scan_tmp_elems(unsigned long long n_bound) { return (size_t)((n_bound + SCAN_TILE - 1) / SCAN_TILE) + 1; }
 
