@@ -250,6 +250,7 @@ __global__ void k_verify_cuts(B b) {
 }
 __global__ void k_cluster_build(B b) {
     const unsigned long long nk = b.ctr->n_kbins;
+    if (blockIdx.x == 0 && threadIdx.x == 0) b.ctr->n_small_taken = 0;        // the work queue of k_cluster_warp<SMALL_CAP>
     for (unsigned long long k = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; k < nk; k += (unsigned long long)gridDim.x * blockDim.x)
         if (b.flag[k]) {
             const uint32_t c = b.scan[k], kl_ = b.c_last[k]; b.cl_first[c] = (uint32_t)k; b.cl_last[c] = kl_; b.cl_rep[c] = b.c_rep[k];
@@ -595,9 +596,10 @@ __device__ void process_cluster(const G& g, const B& b, const uint32_t c, const 
         if (tid == 0) b.sub_valid[sidx] = 0;
         if (ns == 0) continue;
         #define SUB_ML(i) (subl[slo + (i)])
-        #define SUB_LEAD(i) (ML_LEAD(SUB_ML(i)))
-        // svlen = center(svlens)
-        for (int i = tid; i < ns; i += nthr) w[i] = bias64(ml_svlen[SUB_ML(i)]);
+        #define SUB_LEAD(i) (L[sl[(i)]])
+        // svlen = center(svlens); each lead's place in L is resolved here once (sl), so the loops below read a lead through one index
+        uint32_t* sl = sC;
+        for (int i = tid; i < ns; i += nthr) { const uint32_t mi = SUB_ML(i); sl[i] = ordv[ml_plo[mi]]; w[i] = bias64(ml_svlen[mi]); }
         g.sync();
         sort1(g, w, ns);
         const long long svlen = center_sorted(g, w, ns, sA, sB);
@@ -660,9 +662,9 @@ __device__ void process_cluster(const G& g, const B& b, const uint32_t c, const 
             best = (int)bcast_ll(g, best);
             // stable filter of the sub-cluster's order
             const int m = compact(g, ns, sA, [&](int i) { return SUB_LEAD(i).mate_contig == best; });
-            for (int i = tid; i < m; i += nthr) sB[i] = SUB_ML(sA[i]);
+            for (int i = tid; i < m; i += nthr) { sB[i] = SUB_ML(sA[i]); sD[i] = sl[sA[i]]; }
             g.sync();
-            for (int i = tid; i < m; i += nthr) subl[slo + i] = sB[i];
+            for (int i = tid; i < m; i += nthr) { subl[slo + i] = sB[i]; sl[i] = sD[i]; }
             g.sync();
             long long nf = 0, nr = 0;
             for (int i = tid; i < m; i += nthr) { const snfb_lead* l = &SUB_LEAD(i); w[i] = bias64(l->mate_pos); w2[i] = l->qname_hash; nf += (l->flags & SNFB_LF_BND_FIRST) != 0; nr += (l->flags & SNFB_LF_BND_REVERSE) != 0; }
@@ -683,7 +685,7 @@ __device__ void process_cluster(const G& g, const B& b, const uint32_t c, const 
         const uint32_t st0 = lo + (uint32_t)slo;          // staging offset of this sub-cluster's leads and names
         int nstr_f = 0, nstr_r = 0; long long ninl = 0;
         for (int i = tid; i < nfinal; i += nthr) {
-            const uint32_t mi = SUB_ML(i); snfb_lead X = ML_LEAD(mi);
+            const uint32_t mi = SUB_ML(i); snfb_lead X = L[sl[i]];
             X.svlen = ml_svlen[mi];
             if (ml_has[mi]) { X.flags |= SNFB_LF_HAS_SEQ; X.seq_len = ml_seqlen[mi]; } else { X.flags &= ~SNFB_LF_HAS_SEQ; X.seq_len = 0; X.seq_off = -1; }
             extract::store_lead(b.st_leads + st0 + i, X);
@@ -773,18 +775,24 @@ __global__ void __launch_bounds__(WARPS * 32, LIST ? 1 : 4) k_cluster_warp(const
     const unsigned long long n_items = LIST ? b.ctr->n_mid : b.ctr->n_clusters;
     const unsigned long long nw = (unsigned long long)gridDim.x * WARPS;
     coop::WarpG g;
-    for (unsigned long long q = (unsigned long long)blockIdx.x * WARPS + warp; q < n_items; q += nw) {
+    // the dense kernel takes clusters from a queue (their cost varies with their size), asking for the next one before working on this one
+    unsigned long long q = LIST ? (unsigned long long)blockIdx.x * WARPS + warp : __shfl_sync(FULL, lane == 0 ? atomicAdd(&b.ctr->n_small_taken, 1ULL) : 0ULL, 0);
+    for (; q < n_items; ) {
+        unsigned long long next = 0;
+        if (LIST) next = q + nw; else if (lane == 0) next = atomicAdd(&b.ctr->n_small_taken, 1ULL);
         const uint32_t c = LIST ? b.mid_list[q] : (uint32_t)q;
         const uint32_t kf = b.cl_first[c], kl_ = b.cl_last[c];
         const uint32_t lo = b.kb_lead_off[kf], n = b.kb_lead_off[kl_] + b.kb_lead_n[kl_] - lo;
-        if (!LIST && n > (uint32_t)CAP) continue;             // the list kernels take it
-        __syncwarp();                                         // the previous cluster's reads of the staged leads are done
-        if (lane == 0) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            coop::mbar_expect_tx(bar, n * 64u); coop::bulk_g2s(base, b.kleads + lo, n * 64u, bar);
+        if (LIST || n <= (uint32_t)CAP) {                     // larger ones: the list kernels take them
+            __syncwarp();                                     // the previous cluster's reads of the staged leads are done
+            if (lane == 0) {
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                coop::mbar_expect_tx(bar, n * 64u); coop::bulk_g2s(base, b.kleads + lo, n * 64u, bar);
+            }
+            coop::mbar_wait(bar, phase); phase ^= 1u;
+            process_cluster(g, b, c, ws);
         }
-        coop::mbar_wait(bar, phase); phase ^= 1u;
-        process_cluster(g, b, c, ws);
+        q = LIST ? next : __shfl_sync(FULL, next, 0);
     }
 }
 constexpr int CWS_WARPS = 8, CWM_WARPS = 4;

@@ -36,6 +36,7 @@ struct DevCounters {
     unsigned long long ordinal_overflow;   // reads with more than 65535 leads (the ordinal is a 16-bit field)
     unsigned long long bad_records;    // records whose offsets point outside the block's arenas or tables (snfb_load_records fails)
     unsigned long long n_items, n_tiles, n_req, n_req_units;   // consensus work items / vote tiles / seq-on-demand requests
+    unsigned long long n_small_taken;  // clusters handed out by the dense warp-per-cluster kernel's work queue (reset by k_cluster_build)
 };
 
 // ---------------------------------------------------------------- small utilities
