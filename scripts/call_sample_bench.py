@@ -67,8 +67,8 @@ def peak_per_inflated_byte(path):
     bam = bamio.BamFile(path)
     planned = tasks.plan(bam.contigs, cfg)[1]
     items = list(call.task_inputs(bam, planned))
-    z, spans = call.join_inputs([(it[4], it[5]) for it in items])
-    block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[n], s, e, tid) for tid, n, s, e, *_ in items])
+    z, spans = call.join_inputs([(it.bgzf, it.spans) for it in items])
+    block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[it.contig], it.start, it.end, it.id) for it in items])
     ctx = binding.Context(0)
     ctx.set_config(abi.Config.from_sniffles(cfg))
     with MemPoll() as m:
@@ -76,7 +76,7 @@ def peak_per_inflated_byte(path):
         ctx.run()
     ctx.close()
     bam.close()
-    return sum(it[6] for it in items), m.start - m.low
+    return sum(it.inflated for it in items), m.start - m.low
 
 
 def run_call(path, tmp, budget, tag):

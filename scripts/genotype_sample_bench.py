@@ -33,8 +33,8 @@ def _device_pass(path, cfg, cols=None):
     from sniffles_b200 import abi, bamio, binding, call, tasks
     bam = bamio.BamFile(path)
     items = list(call.task_inputs(bam, tasks.plan(bam.contigs, cfg)[1]))
-    z, spans = call.join_inputs([(it[4], it[5]) for it in items])
-    block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[n], s, e, tid) for tid, n, s, e, *_ in items])
+    z, spans = call.join_inputs([(it.bgzf, it.spans) for it in items])
+    block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[it.contig], it.start, it.end, it.id) for it in items])
     ctx = binding.Context(0)
     ctx.set_config(abi.Config.from_sniffles(cfg))
     with csb.MemPoll() as m:
@@ -45,7 +45,7 @@ def _device_pass(path, cfg, cols=None):
             ctx.genotype_targets(*cols, cfg.combine_match, cfg.combine_match_max)
     ctx.close()
     bam.close()
-    return sum(it[6] for it in items), res.cand.copy(), [it[1] for it in items], m.start - run_low, m.start - m.low
+    return sum(it.inflated for it in items), res.cand.copy(), [it.contig for it in items], m.start - run_low, m.start - m.low
 
 
 def write_targets(cand, names, lengths, n, path):

@@ -42,8 +42,8 @@ def names_step(path, reps, warmup):
     cfg = sconfig.default_config("--all-contigs")
     bam = bamio.BamFile(path)
     items = list(call.task_inputs(bam, tasks.plan(bam.contigs, cfg)[1]))
-    z, spans = call.join_inputs([(it[4], it[5]) for it in items])
-    block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[n], s, e, tid) for tid, n, s, e, *_ in items])
+    z, spans = call.join_inputs([(it.bgzf, it.spans) for it in items])
+    block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[it.contig], it.start, it.end, it.id) for it in items])
     bam.close()
     ctx = binding.Context(0)
     ctx.set_config(abi.Config.from_sniffles(cfg))
@@ -70,7 +70,7 @@ def names_step(path, reps, warmup):
             "device_ms_median": statistics.median(dev_ms), "device_ms_min": min(dev_ms), "device_ms_max": max(dev_ms),
             "host_decode_ms_median": 1e3 * statistics.median(decode_s),
             "device_bytes_added": int(free0 - free1), "device_bytes_per_name": (free0 - free1) / n if n else None,
-            "inflated_bytes": sum(it[6] for it in items)}
+            "inflated_bytes": sum(it.inflated for it in items)}
 
 
 def main():

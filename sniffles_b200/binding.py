@@ -250,16 +250,6 @@ class Context:
         self._check(self._lib.snfb_extract_leads(self._h, C.byref(lv) if want else None), "snfb_extract_leads")
         return self._collect(lv if want else None, None, None, True)
 
-    def cluster_call(self, want=True):
-        cv = abi.CandView()
-        self._check(self._lib.snfb_cluster_call(self._h, C.byref(cv) if want else None), "snfb_cluster_call")
-        return self._collect(None, cv if want else None, None, True)
-
-    def consensus(self, want=True):
-        sv = abi.SeqView()
-        self._check(self._lib.snfb_consensus(self._h, C.byref(sv) if want else None), "snfb_consensus")
-        return self._collect(None, None, sv if want else None, True)
-
     def _collect(self, lv, cv, sv, copy) -> Result:
         r = Result()
         cp = (lambda a: a.copy()) if copy else (lambda a: a)
@@ -312,7 +302,7 @@ class Context:
         return abi.view(p.value, "<f8", n.value).copy()
 
     def genotype_targets(self, task, svtype, pos, svlen, bnd_is_first, mate_contig, combine_match, combine_match_max):
-        """Force calling on the device (snfb_genotype_targets) after `run` / `cluster_call` on this context.  Targets as int32 arrays,
+        """Force calling on the device (snfb_genotype_targets) after `run` on this context.  Targets as int32 arrays,
         ordered by task then input order.  Returns (match, cov_start, cov_center, cov_end, bnd_no_prev): match = the candidate's index
         in the run's emission order (int64, -1 none); bnd_no_prev = 1 for a BND with no earlier non-BND target in its task."""
         cols = [np.ascontiguousarray(a, dtype="<i4") for a in (task, svtype, pos, svlen, bnd_is_first, mate_contig)]
@@ -329,7 +319,7 @@ class Context:
         return out
 
     def read_names(self):
-        """The supporting reads' names of the last run's candidates (snfb_read_names), after `run` / `cluster_call` on this context and before
+        """The supporting reads' names of the last run's candidates (snfb_read_names), after `run` on this context and before
         the next load.  Returns ReadNames: the names' bytes back to back (uint8) and their offsets (uint32, one per name of result.rnames
         plus the end), so candidate i owns names rn_off[i] .. rn_off[i + 1], each in the order of its hash list."""
         v = abi.RnamesView()

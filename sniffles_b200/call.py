@@ -2,10 +2,11 @@
 
   * planning is tasks.plan, shared with --genotype-vcf: one task per processed contig, [0, length - 1], task ids counted as the
     reference counts them; config.task_read_id_offset_mult follows sniffles:304-309 from the index's mapped-read counts;
-  * the genome streams through the device in passes: consecutive tasks, in task-id order, whose inflated BAM bytes (the ISIZE of every
-    BGZF block bamio.BamFile.device_input selects for them) fit a budget.  A pass is one mask_block, one snfb_load_bam and one snfb_run;
-    its tasks then run as tasks.CallTask on the pass's BlockRun, and their VCF records and SNF parts are written before the next pass
-    loads (host memory stays bounded, and snfb_coverage_bins reads the block loaded on the context);
+  * the genome streams through the device in passes (device_passes, shared with --genotype-vcf): consecutive tasks, in task-id order,
+    whose inflated BAM bytes (the ISIZE of every BGZF block bamio.BamFile.device_input selects for them) fit a budget.  A pass is
+    tasks.pass_block (tables and N mask) and tasks.load_and_run (one snfb_load_bam and one snfb_run); its tasks then run as tasks.CallTask
+    on the pass's BlockRun (run_pass), and their VCF records and SNF parts are written before the next pass loads (host memory stays
+    bounded, and snfb_coverage_bins reads the block loaded on the context);
   * the VCF goes through vcf.open_output (a .vcf.gz gets BGZF compressed on the GPU and a .tbi), the SNF through snf.write_results;
   * with --gpus N > 1, under torchrun, every rank runs its share of the tasks and rank 0 writes the files (call_sample_ranks)."""
 import contextlib
@@ -88,25 +89,23 @@ def group_passes(items, budget, size=lambda item: item[-1]):
 
 
 def task_inputs(bam, planned, stats=None, regions_by_contig=None, failed=None):
-    """per planned task, in task order: (task id, contig, start, end, BGZF bytes, spans, inflated bytes, regions) of
-    bamio.BamFile.device_input over the task's fetch windows (tasks.fetch_windows; regions: those windows when the contig has regions, else
-    None).  A task whose regions pysam would refuse is logged and left out, as the reference's worker fails it (and listed in `failed` as
-    (task id, contig, error class name)).  The time spent reading is added to stats["read_s"]"""
+    """per planned task, in task order, its tasks.TaskInput: bamio.BamFile.device_input over the task's fetch windows
+    (tasks.fetch_windows), their inflated bytes, and the windows when the contig has regions.  A task whose regions pysam would refuse is
+    logged and left out, as the reference's worker fails it (and listed in `failed`).  The time spent reading is added to
+    stats["read_s"]"""
     for tid, name, s, e in planned:
         t0 = time.perf_counter()
         rg = (regions_by_contig or {}).get(name)
         try:
             windows = tasks.fetch_windows(name, s, e, rg)
         except ValueError as err:
-            log.error(f"Error in worker process while executing CallTask(id={tid}, contig={name}, start={s}, end={e}): {err}")
-            if failed is not None:
-                failed.append((tid, name, type(err).__name__))
+            tasks.CallTask(tid, 0, name, s, e, None).log_failure(log, err, failed)
             continue
         z, spans = bam.device_input([(name, a, b) for a, b in windows], tags=[(0, g) for g in range(len(windows))])
         n = inflated_bytes(z)
         if stats is not None:
             stats["read_s"] += time.perf_counter() - t0
-        yield tid, name, s, e, z, spans, n, (windows if rg else None)
+        yield tasks.TaskInput(tid, name, s, e, z, spans, n, windows if rg else None)
 
 
 def join_inputs(inputs, n_regions=None):
@@ -128,62 +127,51 @@ def join_inputs(inputs, n_regions=None):
     return bgzf, np.concatenate(rows) if rows else np.zeros(0, abi.SPAN_DTYPE)
 
 
-def load_pass(ctx, bam, group, config, tr_all, contigs=None, read_names=False):
-    """the device half of a pass over `group` (items of task_inputs): mask_block, set_config, set_regions, snfb_load_bam and snfb_run,
-    the k-th task of the group being task index k of the block.  Returns the pass's tasks.BlockRun and its split {"load_bam_s", "run_s"};
-    a load or run the library refuses raises CallSampleError naming the pass's contigs and inflated bytes.  contigs: the names
-    tasks.reference_for loads (None: all).  read_names: also gather the candidates' read names (snfb_read_names, before the next load
-    replaces the records) into BlockRun.read_names, timed as split["rnames_s"]."""
-    tr = {k: [(int(a), int(b)) for a, b in tr_all[g[1]]] for k, g in enumerate(group) if g[1] in tr_all}
-    # a task with regions: its records carry their region's window, its own bounds only clip the N mask (the host clips it to the regions)
-    bounds = [(0, bam.get_reference_length(name)) if rg else (s, e) for _, name, s, e, _, _, _, rg in group]
-    block = bamio.pack_records(bam.contigs, [], [(bam.name_to_id[g[1]], a, b, g[0]) for g, (a, b) in zip(group, bounds)], tandem_repeats=tr or None)
-    by_task = [(k, g[7] or [(g[2], g[3])]) for k, g in enumerate(group)]
-    has_regions = any(g[7] for g in group)
-    mask_regions = {k: g[7] for k, g in enumerate(group) if g[7]}
-    # without regions or a contig subset the N mask is the plain mask_block(block, config, ctx), as --genotype-vcf has always called it
-    tasks.mask_block(block, config, ctx, *((mask_regions or None, contigs) if mask_regions or contigs is not None else ()))
-    ctx.set_config(abi.Config.from_sniffles(config))
-    bgzf, spans = join_inputs([(g[4], g[5]) for g in group], [len(w) for _, w in by_task] if has_regions else None)
-    split = {}
+def load_pass(ctx, bam, group, config, tr_all, contigs=None):
+    """the device half of a pass over `group` (TaskInputs of task_inputs, the k-th being task index k of the block): tasks.pass_block,
+    then tasks.load_and_run over the tasks' joined BGZF bytes.  Returns the pass's tasks.BlockRun and its split; a load or run the library
+    refuses raises CallSampleError naming the pass's contigs and inflated bytes.  contigs: the names tasks.reference_for loads (None: all)."""
+    block = tasks.pass_block(ctx, bam, group, config, tr_all, contigs)
+    has_regions = any(it.regions for it in group)
+    windows = [(k, it.regions or [(it.start, it.end)]) for k, it in enumerate(group)] if has_regions else None
+    bgzf, spans = join_inputs([(it.bgzf, it.spans) for it in group], [len(w) for _, w in windows] if has_regions else None)
     try:
-        t0 = time.perf_counter()
-        ctx.set_regions(tasks.region_table(by_task) if has_regions else None)
-        n_rec = ctx.load_bam(bgzf, spans, block)["n_rec"]
-        t1 = time.perf_counter()
-        res = ctx.run(want_leads=True, want_cands=True, want_seqs=True)
-        t2 = time.perf_counter()
-        names = tasks.read_names(ctx) if read_names else None
-        t3 = time.perf_counter()
+        return tasks.load_and_run(ctx, config, block, windows, bgzf, spans)
     except binding.SnfbError as e:
-        contig_list = ", ".join(g[1] for g in group)
-        raise CallSampleError(f"the device pass over contig(s) {contig_list} ({sum(g[6] for g in group)} inflated BAM bytes) failed: {e}") from e
-    split["load_bam_s"], split["run_s"] = t1 - t0, t2 - t1
-    if read_names:
-        split["rnames_s"] = t3 - t2
-    rec_nm = abi.view(res._rec_nm_ptr, "<f8", n_rec).copy() if getattr(res, "_rec_nm_ptr", None) else None
-    return tasks.BlockRun(block, res, tasks.cand_ranges(res.cand, len(block.task)), rec_nm, read_names=names), split
+        contig_list = ", ".join(it.contig for it in group)
+        raise CallSampleError(f"the device pass over contig(s) {contig_list} ({sum(it.inflated for it in group)} inflated BAM bytes) failed: {e}") from e
 
 
-def run_pass(ctx, bam, group, config, tr_all, device=0, contigs=None, failed=None):
-    """one device pass over `group` (items of task_inputs): load_pass, then every task as a CallTask on the pass's BlockRun.  Returns
-    [(CallTask, calls)] in task order and the pass's split {"load_bam_s", "run_s", "finalize_s"}, with --output-rnames also "rnames_s".
-    contigs: the names tasks.reference_for loads (None: all); failed: receives (task id, contig, error class name) of every task that fails."""
-    br, split = load_pass(ctx, bam, group, config, tr_all, contigs, read_names=bool(getattr(config, "output_rnames", False)))
-    t2 = time.perf_counter()
+def device_passes(ctx, bam, planned, config, tr_all, budget, stats, contigs=None, failed=None):
+    """the device passes of a run over `planned` (task id, contig, start, end): the TaskInputs of task_inputs, grouped by group_passes
+    under `budget` and run by load_pass, one pass at a time.  Yields (group, BlockRun); the next pass loads only when the caller asks for
+    it, so everything the caller does with a pass sees its block on the context.  stats: receives read_s, passes, pass_inflated_bytes and
+    per pass load_bam_s, run_s and, with --output-rnames, rnames_s.  contigs: as load_pass; failed: as task_inputs."""
+    for group in group_passes(task_inputs(bam, planned, stats, config.regions_by_contig, failed), budget, size=lambda it: it.inflated):
+        br, split = load_pass(ctx, bam, group, config, tr_all, contigs)
+        stats["passes"] += 1
+        stats["pass_inflated_bytes"].append(sum(it.inflated for it in group))
+        for k in ("load_bam_s", "run_s", "rnames_s"):
+            if k in split:
+                stats.setdefault(k, []).append(split[k])
+        yield group, br
+
+
+def run_pass(group, br, config, device, stats, failed=None):
+    """every task of a pass (`group`, run as `br` by device_passes) as a CallTask on the pass's BlockRun: [(CallTask, calls)] in task
+    order, the time added to stats["finalize_s"].  failed: receives (task id, contig, error class name) of every task that fails."""
+    t0 = time.perf_counter()
     done = []
-    for k, (tid, name, s, e, *_) in enumerate(group):
-        task = tasks.CallTask(id=tid, sv_id=0, contig=name, start=s, end=e, config=config, block_run=br, task_index=k, device=device)
+    for k, it in enumerate(group):
+        task = tasks.CallTask(id=it.id, sv_id=0, contig=it.contig, start=it.start, end=it.end, config=config, block_run=br, task_index=k, device=device)
         try:
             calls, _ = task.execute()
         except tasks.CallTaskError as err:      # logged and left out, as the reference's worker leaves a failed task out
-            log.error(f"Error in worker process while executing CallTask(id={tid}, contig={name}, start={s}, end={e}): {err}")
-            if failed is not None:
-                failed.append((tid, name, type(err).__name__))
+            task.log_failure(log, err, failed)
             continue
         done.append((task, calls))
-    split["finalize_s"] = time.perf_counter() - t2
-    return done, split
+    stats["finalize_s"] += time.perf_counter() - t0
+    return done
 
 
 def plan_sample(config):
@@ -245,25 +233,14 @@ def call_sample(config, device=0, budget=None, stats=None):
     st.update(passes=0, pass_inflated_bytes=[], load_bam_s=[], run_s=[], rnames_s=[], finalize_s=0.0, vcf_write_s=0.0, snf_write_s=0.0, read_s=0.0)
     st["index_s"] = time.perf_counter() - t0
     parts, written = [], 0
-    with contextlib.ExitStack() as stack:
+    # a .vcf.gz is compressed and indexed when the run ends without an error
+    with vcf.open_output(config, ctx) if config.vcf is not None else contextlib.nullcontext() as handle:
         writer = None
-        if config.vcf is not None:
-            handle = vcf.open_output(config, ctx)
-            if config.vcf_output_bgz:
-                stack.enter_context(handle)               # compressed and indexed when the run ends without an error
-            else:
-                stack.callback(handle.close)
+        if handle is not None:
             writer = vcf.VCFWriter(config, handle, reference)
             writer.write_header(contig_lengths)
-        for group in group_passes(task_inputs(bam, planned, st, config.regions_by_contig), budget, size=lambda item: item[6]):
-            done, split = run_pass(ctx, bam, group, config, tr_all, device)
-            st["passes"] += 1
-            st["pass_inflated_bytes"].append(sum(g[6] for g in group))
-            st["load_bam_s"].append(split["load_bam_s"])
-            st["run_s"].append(split["run_s"])
-            if "rnames_s" in split:
-                st["rnames_s"].append(split["rnames_s"])
-            st["finalize_s"] += split["finalize_s"]
+        for group, br in device_passes(ctx, bam, planned, config, tr_all, budget, st):
+            done = run_pass(group, br, config, device, st)
             t1 = time.perf_counter()
             if writer is not None:
                 if reference is not None:
@@ -309,17 +286,10 @@ def run_rank_tasks(config, device, budget, rank, world):
         budget = device_budget(device)
     st.update(tasks=len(mine), weight=sum(w for w, o in zip(weights, owner) if o == rank), index_s=time.perf_counter() - t0)
     out, failed, nm = [], [], None
-    for group in group_passes(task_inputs(bam, mine, st, config.regions_by_contig, failed), budget, size=lambda item: item[6]):
-        done, split = run_pass(ctx, bam, group, config, tr_all, device, contigs, failed)
+    for group, br in device_passes(ctx, bam, mine, config, tr_all, budget, st, contigs, failed):
+        done = run_pass(group, br, config, device, st, failed)
         # the config holds the N-mismatch mean of the pass's last task: the SNF header of rank 0 takes that of the run's last task
-        nm = (group[-1][0], config.average_regional_nm, config.qc_nm_threshold)
-        st["passes"] += 1
-        st["pass_inflated_bytes"].append(sum(g[6] for g in group))
-        st["load_bam_s"].append(split["load_bam_s"])
-        st["run_s"].append(split["run_s"])
-        if "rnames_s" in split:
-            st["rnames_s"].append(split["rnames_s"])
-        st["finalize_s"] += split["finalize_s"]
+        nm = (group[-1].id, config.average_regional_nm, config.qc_nm_threshold)
         t1 = time.perf_counter()
         if config.vcf is not None and reference is not None:
             reference.prefetch(vcf.reference_intervals([c for _, calls in done for c in calls], config))
@@ -353,12 +323,7 @@ def write_rank_outputs(config, contig_lengths, payloads, ctx=None):
     written, vcf_s, snf_s = 0, 0.0, 0.0
     if config.vcf is not None:
         t0 = time.perf_counter()
-        with contextlib.ExitStack() as stack:
-            handle = vcf.open_output(config, ctx)
-            if config.vcf_output_bgz:
-                stack.enter_context(handle)           # compressed and indexed when the writing ends without an error
-            else:
-                stack.callback(handle.close)
+        with vcf.open_output(config, ctx) as handle:          # a .vcf.gz is compressed and indexed when the writing ends without an error
             vcf.VCFWriter(config, handle).write_header(contig_lengths)
             for _, text, n, _ in done:
                 handle.write(text)

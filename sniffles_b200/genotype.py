@@ -5,10 +5,10 @@ vcf.py:352-478; result.py:118-130).
     input is read as BGZF text (bamio.BgzfReader), where the reference goes through pysam.VariantFile (DESIGN §4);
   * `plan` makes one task per processed contig, [0, contig_len - 1), holding the contig's targets with start <= pos < end;
   * matching and the coverage probes run on the device (snfb_genotype_targets); `genotype_of` and the rewrite stay on the host;
-  * `genotype_vcf(config)` drives the mode in the device passes of call.call_sample: the tasks with targets, in task-id order, grouped
-    so that their inflated BAM bytes fit a budget (call.group_passes over call.task_inputs, so host memory holds one pass's BGZF bytes).
-    A pass is call.load_pass (N mask, snfb_load_bam, snfb_run), one snfb_genotype_targets call for the targets of its tasks, then its
-    tasks' records, rewritten through vcf.open_output, before the next pass loads.  The records come in task order, and in target-file
+  * `genotype_vcf(config)` drives the mode in the device passes of call.call_sample (call.device_passes): the tasks with targets, in
+    task-id order, grouped so that their inflated BAM bytes fit a budget (host memory holds one pass's BGZF bytes).  A pass is
+    call.load_pass (N mask, snfb_load_bam, snfb_run), one snfb_genotype_targets call for the targets of its tasks, then its tasks'
+    records, rewritten through vcf.open_output, before the next pass loads.  The records come in task order, and in target-file
     order inside a task, so the output is the same at every budget.  The genotype step's device memory (about 63 bytes per target
     and 28 per candidate of the pass, kept on the context) sits inside the margin call.device_budget leaves (DESIGN §8)."""
 import io
@@ -215,7 +215,7 @@ def write_tasks(handle, br, jobs, config):
         try:
             done, _ = task.execute()
         except tasks.GenotypeTaskError as err:
-            log.error(f"Error in worker process while executing {task.label()}: {err}")
+            task.log_failure(log, err)
             continue
         for t in done:
             handle.write(rewrite_line(t, config) + "\n")
@@ -245,7 +245,7 @@ def genotype_vcf(config, device=0, budget=None, stats=None):
         try:
             tasks.fetch_windows(name, s, e, config.regions_by_contig.get(name))
         except ValueError as err:                       # the task fails in the reference's worker: its targets are not written
-            log.error(f"Error in worker process while executing GenotypeTask(id={tid}, contig={name}, start={s}, end={e}): {err}")
+            tasks.GenotypeTask(tid, 0, name, s, e, config).log_failure(log, err)
             continue
         planned.append((tid, name, s, e))
         targets_of[tid] = ts
@@ -261,21 +261,16 @@ def genotype_vcf(config, device=0, budget=None, stats=None):
         st["write_s"] += time.perf_counter() - t1
         # a pass's targets are matched against the candidates and coverage of the block resident on the context: every step of a pass
         # ends before the next pass loads
-        for group in call.group_passes(call.task_inputs(bam, planned, st, config.regions_by_contig), budget, size=lambda item: item[6]):
-            br, split = call.load_pass(ctx, bam, group, config, tr_all)
-            st["passes"] += 1
-            st["pass_inflated_bytes"].append(sum(g[6] for g in group))
-            st["load_bam_s"].append(split["load_bam_s"])
-            st["run_s"].append(split["run_s"])
+        for group, br in call.device_passes(ctx, bam, planned, config, tr_all, budget, st):
             t1 = time.perf_counter()
             try:
-                br.genotype = device_targets(ctx, [(k, targets_of[g[0]]) for k, g in enumerate(group)], bam.name_to_id, config)
+                br.genotype = device_targets(ctx, [(k, targets_of[it.id]) for k, it in enumerate(group)], bam.name_to_id, config)
             except binding.SnfbError as e:
-                names = ", ".join(g[1] for g in group)
+                names = ", ".join(it.contig for it in group)
                 raise call.CallSampleError(f"the target genotyping of the device pass over contig(s) {names} "
                                            f"({st['pass_inflated_bytes'][-1]} inflated BAM bytes) failed: {e}") from e
             t2 = time.perf_counter()
-            written += write_tasks(handle, br, [(tid, name, s, e, targets_of[tid], k) for k, (tid, name, s, e, *_) in enumerate(group)], config)
+            written += write_tasks(handle, br, [(it.id, it.contig, it.start, it.end, targets_of[it.id], k) for k, it in enumerate(group)], config)
             st["genotype_s"].append(t2 - t1)
             st["write_s"] += time.perf_counter() - t2
         t1 = time.perf_counter()

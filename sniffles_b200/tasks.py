@@ -3,10 +3,14 @@ same method names and meaning — build_leadtab / call_candidates / finalize_can
 execute — with the three hot calls forwarded to libsnfb200 through ctypes.
 
 A `Task` works on one contig (one snfb_task); several tasks can share one record block and one
-device run (`run_block`), which is how the contigs of a genome are processed per GPU."""
+device run, which is how the contigs of a genome are processed per GPU.  Every device pass -- a
+pass of call.call_sample or genotype.genotype_vcf, a task's own BAM region, a block handed to
+`run_block` -- is packed by `pass_block` (when it comes from a BAM) and loaded and run by
+`load_and_run`."""
 import logging
+import time
 from dataclasses import dataclass, field
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import numpy as np
 
@@ -91,15 +95,68 @@ def read_names(ctx):
     return names
 
 
-def run_block(block, config, device: int = 0, ctx=None) -> BlockRun:
-    """leadprov -> cluster -> consensus for every task of the block in one device pass."""
-    ctx = ctx or device_context(device)
+class TaskInput(NamedTuple):
+    """one task of a device pass (call.task_inputs): bamio.BamFile.device_input over its fetch windows (BGZF bytes and spans), the bytes
+    snfb_load_bam inflates them to, and its fetch windows when its contig has regions (else None)"""
+    id: int
+    contig: str
+    start: int
+    end: int
+    bgzf: Optional[np.ndarray]
+    spans: Optional[np.ndarray]
+    inflated: Optional[int]
+    regions: Optional[list]
+
+
+def pass_block(ctx, bam, items, config, tandem_repeats, contigs=None, records=()):
+    """the record block of one device pass over `items` (TaskInput; the k-th is task index k of the block): the task, contig and
+    tandem-repeat tables of bamio.pack_records, then mask_block with the tasks' regions.  tandem_repeats: {contig: intervals}
+    (load_tandem_repeats); contigs: the names reference_for loads (None: all); records: host-decoded (task index, record, region index)
+    packed with the tables (the host reader; snfb_load_bam needs none)."""
+    from . import bamio
+    tr = {k: [(int(a), int(b)) for a, b in tandem_repeats[it.contig]] for k, it in enumerate(items) if tandem_repeats.get(it.contig)}
+    # a task with regions: its records carry their region's window, its own bounds only clip the N mask (the host clips it to the regions)
+    bounds = [(0, bam.get_reference_length(it.contig)) if it.regions else (int(it.start), int(it.end)) for it in items]
+    block = bamio.pack_records(bam.contigs, list(records), [(bam.name_to_id[it.contig], s, e, int(it.id)) for it, (s, e) in zip(items, bounds)],
+                               tandem_repeats=tr or None)
+    regions = {k: it.regions for k, it in enumerate(items) if it.regions}
+    # mask_block's optional arguments go only to a pass that uses them: without regions or a contig subset the call stays
+    # mask_block(block, config, ctx), the form a stand-in N mask (tests/test_gpu_reference.py) replaces
+    if regions or contigs is not None:
+        return mask_block(block, config, ctx, regions or None, contigs)
+    return mask_block(block, config, ctx)
+
+
+def load_and_run(ctx, config, block, windows=None, bgzf=None, spans=None, cigar16=True):
+    """one device pass over `block` on `ctx`: set_config, set_regions (windows: [(task index, [(start, end)])] of every task when some task
+    has regions, else None), the load -- snfb_load_bam of `bgzf` / `spans` into the block's tables, or without them snfb_load_records of
+    the block's own records (cigar16 as Context.load takes it) -- and snfb_run; with config.output_rnames also the candidates' read names
+    (read_names), before the next load replaces the records.  Returns the BlockRun and its split {"load_bam_s", "run_s"}, with the read
+    names also "rnames_s"."""
     ctx.set_config(abi.Config.from_sniffles(config))
-    ctx.load(block)
+    t0 = time.perf_counter()
+    ctx.set_regions(region_table(windows) if windows else None)
+    if bgzf is not None:
+        n_rec = ctx.load_bam(bgzf, spans, block)["n_rec"]
+    else:
+        ctx.load(block, cigar16=cigar16)
+        n_rec = len(block.rec)
+    t1 = time.perf_counter()
     res = ctx.run(want_leads=True, want_cands=True, want_seqs=True)
-    rec_nm = abi.view(res._rec_nm_ptr, "<f8", len(block.rec)).copy() if getattr(res, "_rec_nm_ptr", None) else None
-    names = read_names(ctx) if getattr(config, "output_rnames", False) else None
-    return BlockRun(block, res, cand_ranges(res.cand, len(block.task)), rec_nm, read_names=names)
+    t2 = time.perf_counter()
+    split = {"load_bam_s": t1 - t0, "run_s": t2 - t1}
+    names = None
+    if getattr(config, "output_rnames", False):
+        names = read_names(ctx)
+        split["rnames_s"] = time.perf_counter() - t2
+    rec_nm = abi.view(res._rec_nm_ptr, "<f8", n_rec).copy() if getattr(res, "_rec_nm_ptr", None) else None
+    return BlockRun(block, res, cand_ranges(res.cand, len(block.task)), rec_nm, read_names=names), split
+
+
+def run_block(block, config, device: int = 0, ctx=None) -> BlockRun:
+    """leadprov -> cluster -> consensus for every task of an already packed block in one device pass (no N mask: the caller masks the
+    block)."""
+    return load_and_run(ctx or device_context(device), config, block)[0]
 
 
 def cand_ranges(cand, n_task):
@@ -194,7 +251,8 @@ class Task:
     regions: list = None
     result: object = None
     # the device pass this task reads from, and its index in that block.  Either handed in (several tasks sharing one block and one
-    # device pass: run_block), or built by the task itself from its BAM region on first use, the way the reference's worker does.
+    # device pass: call.load_pass, run_block), or built by the task itself from its BAM region on first use, the way the reference's
+    # worker does.
     block_run: BlockRun = None
     task_index: int = 0
     coverage_average_total: float = 0.0
@@ -210,22 +268,18 @@ class Task:
             raise RuntimeError("Task has neither a block_run nor a BAM to read its region from")
         return bam
 
-    def _tables(self, bam, recs=()):
-        from . import bamio
-        cidx = bam.name_to_id[self.contig]
-        tr = {0: [(int(a), int(b)) for a, b in self.tandem_repeats]} if self.tandem_repeats else None
-        # with regions the records carry their region's window; the task's own bounds then only clip the N mask, which the host clips
-        s, e = (0, bam.contigs[cidx][1]) if self.regions else (int(self.start), int(self.end))
-        return bamio.pack_records(bam.contigs, list(recs), [(cidx, s, e, int(self.id))], tandem_repeats=tr)
-
-    def _own_block(self, windows):
-        """records of every fetch window from the task's BAM (`self.bam`: an open bamio.BamFile or a path; default config.input), region by
-        region, decoded and packed on the HOST (device_ingest=False; also what the tests compare the device ingest with)"""
-        bam = self._open()
-        return self._tables(bam, [(0, r, g) for g, (s, e) in enumerate(windows) for r in bam.fetch(self.contig, s, e)])
-
     def _ctx(self):
         return device_context(self.device)
+
+    def label(self):
+        return f"{type(self).__name__}(id={self.id}, contig={self.contig}, start={self.start}, end={self.end})"
+
+    def log_failure(self, log, err, failed=None):
+        """the reference worker's error line for this task, which fails and is left out; failed: receives (task id, contig, error class
+        name)"""
+        log.error(f"Error in worker process while executing {self.label()}: {err}")
+        if failed is not None:
+            failed.append((self.id, self.contig, type(err).__name__))
 
     def bind(self, worker=None):
         """device = worker.id % n_gpus: a context per process and device, created lazily after the fork"""
@@ -235,30 +289,27 @@ class Task:
 
     def build_leadtab(self):
         """parallel.py:90-102 — returns (externals, read_count).  Leads outside the region are dropped on the
-        device, exactly as the caller discards `externals` (parallel.py:264)."""
+        device, exactly as the caller discards `externals` (parallel.py:264).  Without a block_run the task first runs its own BAM
+        region (`self.bam`: an open bamio.BamFile or a path; default config.input) as a one-task device pass."""
         if self.block_run is None:
             ctx = self._ctx()
-            ctx.set_config(abi.Config.from_sniffles(self.config))
             windows = fetch_windows(self.contig, self.start, self.end, self.regions)
-            regions = {0: windows} if self.regions else None
+            bam = self._open()
             if self.device_ingest:
                 # the reference's `bam.fetch(contig, start, end)` (parallel.py:95-98, leadprov.py:488) with htslib's work on the GPU: the host
                 # only resolves the BAI index; BGZF inflate, record decode, region filter and CIGAR16 packing are snfb_load_bam
-                bam = self._open()
-                block = mask_block(self._tables(bam), self.config, ctx, regions)
                 bgzf, spans = bam.device_input([(self.contig, s, e) for s, e in windows], tags=[(0, g) for g in range(len(windows))])
-                ctx.set_regions(region_table([(0, windows)]) if regions else None)
-                n_rec = ctx.load_bam(bgzf, spans, block)["n_rec"]
+                recs = ()
             else:
-                block = mask_block(self._own_block(windows), self.config, ctx, regions)
-                ctx.set_regions(region_table([(0, windows)]) if regions else None)
-                ctx.load(block, cigar16=False)                   # BAM words: the library converts them (snfb_load_records)
-                n_rec = len(block.rec)
-            res = ctx.extract_leads()                            # snfb_extract_leads
-            rec_nm = abi.view(res._rec_nm_ptr, "<f8", n_rec).copy() if getattr(res, "_rec_nm_ptr", None) else None
-            self.block_run = BlockRun(block, res, None, rec_nm)
+                # the host reader (also what the tests compare the device ingest with): records decoded and packed region by region
+                bgzf = spans = None
+                recs = [(0, r, g) for g, (s, e) in enumerate(windows) for r in bam.fetch(self.contig, s, e)]
+            regions = windows if self.regions else None
+            item = TaskInput(self.id, self.contig, self.start, self.end, bgzf, spans, None, regions)
+            block = pass_block(ctx, bam, [item], self.config, {self.contig: self.tandem_repeats}, records=recs)
+            # the host reader ships BAM CIGAR words: the library converts them (snfb_load_records)
+            self.block_run, _ = load_and_run(ctx, self.config, block, [(0, windows)] if regions else None, bgzf, spans, cigar16=False)
             self.task_index = 0
-            self._staged = True
         r = self.block_run.result
         self.config.average_regional_nm = float(r.task_mean_nm[self.task_index])      # leadprov.py:577-578
         self.config.qc_nm_threshold = self.config.average_regional_nm
@@ -267,16 +318,6 @@ class Task:
     def call_candidates(self, keep_qc_fails, config):
         """parallel.py:104-127"""
         br = self.block_run
-        if getattr(self, "_staged", False):
-            ctx = self._ctx()
-            cv = ctx.cluster_call()                              # snfb_cluster_call: candidate records (ALT offsets already planned)
-            sv = ctx.consensus()                                 # snfb_consensus: annotate_sv's INS sequences, which the calls below carry
-            r = br.result
-            r.cand, r.cand_leads, r.rnames, r.rn_off, r.task_cov_mean, r.alt = cv.cand, cv.cand_leads, cv.rnames, cv.rn_off, cv.task_cov_mean, sv.alt
-            br.cand_range = cand_ranges(r.cand, len(br.block.task))
-            if getattr(config, "output_rnames", False):
-                br.read_names = read_names(ctx)
-            self._staged = False
         lo, hi = br.cand_range[self.task_index]
         need_leads = bool(config.mosaic) or bool(config.phase)
         calls = postprocess.calls_from_result(br.result, self.task_index, lo, hi, br.block.contig_names, self.contig, self.id, config,
@@ -343,9 +384,6 @@ class GenotypeTaskError(RuntimeError):
 
 
 class GenotypeTask(Task):
-    def label(self):
-        return f"GenotypeTask(id={self.id}, contig={self.contig}, start={self.start}, end={self.end})"
-
     def execute(self, worker=None):
         """parallel.py:300-369: candidates finalized with QC fails kept, each target matched to the nearest candidate of its bins and
         probed for coverage on the device (snfb_genotype_targets), then genotyped.  Returns (targets, read_count)."""

@@ -56,7 +56,7 @@ def test_any_budget_gives_the_same_files(case, inputs, tmp_path):
     gold = GOLD["cases"][case]
     cfg = _config(case, inputs[gold["input"]], str(tmp_path))
     bam = bamio.BamFile(cfg.input)
-    sizes = [it[6] for it in call.task_inputs(bam, tasks.plan(bam.contigs, cfg)[1])]
+    sizes = [it.inflated for it in call.task_inputs(bam, tasks.plan(bam.contigs, cfg)[1])]
     bam.close()
     outs = []
     for k, budget in enumerate((1 << 40, 1, max(sum(sizes) - 1, max(sizes)))):

@@ -40,7 +40,7 @@ def _run_cases(rank, world, runs, budget, fail_rank=None):
     if rank == fail_rank:
         def failing_pass(*args, **kwargs):
             raise call.CallSampleError(f"injected failure of a device pass on rank {rank}")
-        call.run_pass = failing_pass
+        call.load_pass = failing_pass
     out = {}
     for tag, args in runs:
         stats = {}

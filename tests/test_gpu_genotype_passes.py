@@ -18,7 +18,7 @@ def _sizes(cfg):
     bam = bamio.BamFile(cfg.input)
     _, targets = genotype.read_targets(cfg.genotype_vcf)
     planned = [p[:4] for p in genotype.plan(bam.contigs, targets, cfg) if p[4]]
-    sizes = [it[6] for it in call.task_inputs(bam, planned, regions_by_contig=cfg.regions_by_contig)]
+    sizes = [it.inflated for it in call.task_inputs(bam, planned, regions_by_contig=cfg.regions_by_contig)]
     bam.close()
     return sizes
 

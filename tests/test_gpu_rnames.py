@@ -62,7 +62,7 @@ def test_every_budget_and_two_ranks_give_the_same_files(case, inputs, tmp_path):
     one.mkdir()
     call.call_sample(_config(case, paths, str(one)), budget=1 << 40)
     bam = bamio.BamFile(paths["bam"])
-    total = sum(it[6] for it in call.task_inputs(bam, tasks.plan(bam.contigs, _config(case, paths, str(one)))[1]))
+    total = sum(it.inflated for it in call.task_inputs(bam, tasks.plan(bam.contigs, _config(case, paths, str(one)))[1]))
     bam.close()
     quarter = tmp_path / "quarter"
     quarter.mkdir()
