@@ -10,14 +10,17 @@ sniffles:371-481, parallel.py:372-572 and result.py:133-243.
   * with --combine-population, the population SNF's variants of the planned contigs are loaded to the device once, and every call a pass
     makes gets POPULATION_AF / POPULATION_SIZE from one snfb_population_match call (SVGroup.call, sv.py:475-479);
   * each task's calls are ordered as CombineResult orders them, or, above --combine-max-inmemory-results inputs, as CombineResultTmpFile
-    keeps them (a sorted batch's calls below the task's highest stored position are dropped), and written through vcf.open_output.
+    keeps them (a sorted batch's calls below the task's highest stored position are dropped), and written through vcf.open_output;
+  * with --reference, the FASTA's planned contigs are loaded to the device once (tasks.reference_for, as sniffles:253-256 and
+    result.py:210-214 open it for the writer of either ordering), every allele interval the records of a pass can ask for is gathered in
+    one Reference.prefetch, and VCFWriter.write_call takes REF / ALT from it after the population annotation.
 
 Deviations from the reference: an SNF that is missing, unreadable or whose header has no contig_lengths is refused with a message instead
 of a traceback; a header without snf_format_version (as this package's SNF writer leaves it) is taken as the current version; the dropped
 calls of CombineResultTmpFile are counted and logged, not written to an `-unsorted.part.vcf`; a population SNF that is missing, has no
 `population` header record or holds blocks that are not PopulationVariant lists is refused before any output is opened; an INS population
 variant with svlen 0 that reaches the alignment test, where the reference's worker divides by zero, stops the run with a message naming
-it."""
+it; a FASTA that cannot be opened is logged once, where CombineResultTmpFile logs it for every task's part."""
 import contextlib
 import logging
 import os
@@ -392,10 +395,11 @@ def combine_snfs(config, device=0, budget=None, stats=None):
     """the combine run mode: config.input (SNF files or one .tsv) -> config.vcf.  budget: the candidates one pass may hold (default
     PASS_CANDIDATES).  stats: a dict that receives the wall-clock split (header_s, decode_s, device_s, call_group_s, write_s, passes and
     per-pass task and candidate counts, dropped; with --combine-population population_s for the decode and load of the population SNF and
-    population_match_s for its matches).  Returns the number of VCF records written."""
+    population_match_s for its matches; with --reference reference_s for the FASTA load and, per pass, prefetch_s and prefetch_bytes of
+    its allele gather).  Returns the number of VCF records written."""
     st = stats if stats is not None else {}
     st.update(passes=0, pass_tasks=[], pass_candidates=[], header_s=0.0, decode_s=0.0, device_s=0.0, call_group_s=0.0, write_s=0.0, dropped=0,
-              population_s=0.0, population_match_s=0.0)
+              population_s=0.0, population_match_s=0.0, reference_s=0.0, prefetch_s=[], prefetch_bytes=[])
     t0 = time.perf_counter()
     config.mode = "combine"
     check_outputs(config)
@@ -413,10 +417,11 @@ def combine_snfs(config, device=0, budget=None, stats=None):
                 log.warning("Result will be unsorted and uncompressed")
     log.info(f"Verified headers for {len(config.snf_input_info)} .snf files.")
     st["header_s"] = time.perf_counter() - t0
+    contigs = list(dict.fromkeys(t.contig for t in planned))
     pop = None
     if config.combine_population:                        # sniffles:433-435, parallel.py:454-455: opened and checked before any output
         tp = time.perf_counter()
-        pop = Population(config.combine_population, list(dict.fromkeys(t.contig for t in planned)))
+        pop = Population(config.combine_population, contigs)
         st["population_s"] += time.perf_counter() - tp
     readers = {}
     ctx = tasks.device_context(device)
@@ -428,6 +433,12 @@ def combine_snfs(config, device=0, budget=None, stats=None):
             raise CombineError(f"Loading the population SNF {pop.path} (--combine-population) to the device failed: {e}") from e
         st["population_s"] += time.perf_counter() - tp
         log.info(f"Population SNF {pop.path}: {len(pop.variants)} variants in the run's contigs")
+    reference = None
+    if getattr(config, "reference", None):               # sniffles:253-256; logged and left out when it cannot be read
+        log.info(f"Opening for reading: {config.reference}")
+        tr = time.perf_counter()
+        reference = tasks.reference_for(ctx, config.reference, contigs)
+        st["reference_s"] = time.perf_counter() - tr
     if budget is None:
         budget = PASS_CANDIDATES
     written = 0
@@ -439,7 +450,7 @@ def combine_snfs(config, device=0, budget=None, stats=None):
                 stack.enter_context(handle)               # compressed and indexed when the run ends without an error
             else:
                 stack.callback(handle.close)
-            writer = vcf.VCFWriter(config, handle)
+            writer = vcf.VCFWriter(config, handle, reference)
             writer.write_header(contig_lengths)
             for group in call.group_passes(_decoded(config, planned, readers, st), budget, size=lambda fp: len(fp.cands)):
                 fp = join(group)
@@ -467,7 +478,8 @@ def _decoded(config, planned, readers, st):
 
 def _run_pass(ctx, fp, config, reqc, writer, tmpfile, st, pop=None):
     """one device call for the pass's tasks, SVGroup.call on the host, the population annotation of every call the pass made (one device
-    call), the records written; returns the records written"""
+    call), with the writer's reference the allele intervals of every call the pass stores (one device gather), the records written;
+    returns the records written"""
     from . import binding
     flat = fp.arrays()
     t0 = time.perf_counter()
@@ -489,16 +501,24 @@ def _run_pass(ctx, fp, config, reqc, writer, tmpfile, st, pop=None):
             raise CombineError(f"the population match of the pass from task {fp.tasks[0].id} failed: {e}") from e
     t2 = time.perf_counter()
     st["population_match_s"] += t2 - tp
-    written = 0
+    stored = []
     for k in range(len(fp.tasks)):
         calls, dropped = stored_calls(batches[k], tmpfile, config.sort)
         st["dropped"] += dropped
-        for c in calls:
-            written += writer.write_call(c)
+        stored.extend(calls)
+    prefetch_s = 0.0
+    if writer.reference is not None:                     # after the annotation: the population match compares the SNF ALT
+        tr = time.perf_counter()
+        st["prefetch_bytes"].append(writer.reference.prefetch(vcf.reference_intervals(stored, config)))
+        prefetch_s = time.perf_counter() - tr
+        st["prefetch_s"].append(prefetch_s)
+    written = 0
+    for c in stored:
+        written += writer.write_call(c)
     st["passes"] += 1
     st["pass_tasks"].append(len(fp.tasks))
     st["pass_candidates"].append(len(fp.cands))
     st["device_s"] += t1 - t0
     st["call_group_s"] += tp - t1
-    st["write_s"] += time.perf_counter() - t2
+    st["write_s"] += time.perf_counter() - t2 - prefetch_s
     return written

@@ -231,7 +231,8 @@ class Reference:
         return got
 
     def prefetch(self, intervals):
-        """one snfb_fetch_reference call for every (contig, start, end) not cached yet; intervals `fetch` would refuse are skipped"""
+        """one snfb_fetch_reference call for every (contig, start, end) not cached yet; intervals `fetch` would refuse are skipped.
+        Returns the number of bases gathered."""
         keys = set()
         for contig, start, end in intervals:
             try:
@@ -243,6 +244,7 @@ class Reference:
         keys = sorted(keys)
         for k, s in zip(keys, self._gather(keys) if keys else []):
             self._cache[k] = s
+        return sum(e - s for _, s, e in keys)
 
     # ---- the N mask ----
     def n_runs(self):

@@ -25,23 +25,26 @@ def device_context(device: int = 0) -> binding.Context:
     return _CTX[device]
 
 
-_REF = {}      # per (device context, FASTA path, loaded contigs): the fasta.Reference loaded on it, or None when it could not be loaded
+_REF = {}      # per device context: ((FASTA path, loaded contigs), the fasta.Reference resident on it, or None when it could not be loaded)
 
 
 def reference_for(ctx, path, contigs=None):
     """the reference FASTA resident on `ctx`, loaded on first use.  contigs: the names to load (None: all), as one rank of a multi-GPU
     run loads only the contigs of its tasks; every caller of a run passes the same names, so the N mask and the VCF writer share one
-    object.  A FASTA that cannot be opened or read (a missing or stale index, a damaged BGZF block) is logged once as the reference logs
-    it (vcf.py:116-119) and the run goes on without it."""
-    key = (ctx, str(path), None if contigs is None else tuple(sorted(set(contigs))))
-    if key not in _REF:
+    object.  A context holds one genome: another path or set of names is loaded in place of the last one, whose object is dropped (its
+    gathers would read the new genome).  A FASTA that cannot be opened or read (a missing or stale index, a damaged BGZF block) is logged
+    once as the reference logs it (vcf.py:116-119) and the run goes on without it."""
+    key = (str(path), None if contigs is None else tuple(sorted(set(contigs))))
+    held = _REF.get(ctx)
+    if held is None or held[0] != key:
         from . import fasta
         try:
-            _REF[key] = fasta.Reference(path, ctx, contigs=contigs)
+            ref = fasta.Reference(path, ctx, contigs=contigs)
         except (OSError, ValueError, RuntimeError) as e:
             logging.error(f"Unable to open reference file {path}: {e}")
-            _REF[key] = None
-    return _REF[key]
+            ref = None
+        _REF[ctx] = held = (key, ref)
+    return held[1]
 
 
 def mask_block(block, config, ctx, regions=None, contigs=None):
