@@ -340,57 +340,31 @@ def write_rank_outputs(config, contig_lengths, payloads, ctx=None):
     return written, vcf_s, snf_s
 
 
-def _error_text(e):
-    return str(e) if isinstance(e, CallSampleError) else f"{type(e).__name__}: {e}"
-
-
 def call_sample_ranks(config, device, budget=None, stats=None):
-    """call_sample over the ranks of an initialised torch.distributed process group (one process per GPU; gloo, since the only
-    collectives carry host objects).  Rank 0 checks the outputs and broadcasts the verdict; every rank plans alike, runs its own tasks
-    (run_rank_tasks) and sends its payload to rank 0 with gather_object, an error included, so that every rank reaches the gather.  Rank 0
-    writes the files (write_rank_outputs) and broadcasts (ok, records written or the error): every rank returns the same count or raises
-    the same CallSampleError.  Rank 0 holds every rank's VCF text and SNF parts at once, host memory in proportion to the output files.
+    """call_sample over the ranks of an initialised torch.distributed process group, through dist.rank_run: rank 0 checks the outputs
+    and broadcasts the verdict; every rank plans alike, runs its own tasks (run_rank_tasks) and sends its payload to rank 0, an error
+    included.  Rank 0 writes the files (write_rank_outputs): every rank returns the same count or raises the same CallSampleError.  Rank 0
+    holds every rank's VCF text and SNF parts at once, host memory in proportion to the output files.
 
     stats on rank 0: the keys of call_sample for rank 0's own work, plus "ranks" (per rank its split, tasks, inflated bytes, index weight
     and failed tasks), "gather_s" and "write_s"."""
-    import torch.distributed as tdist
-    rank, world = tdist.get_rank(), tdist.get_world_size()
-    t0 = time.perf_counter()
-    verdict = [None]
-    if rank == 0:
-        try:
-            check_outputs(config)
-        except CallSampleError as e:
-            verdict[0] = str(e)
-    tdist.broadcast_object_list(verdict, src=0)
-    if verdict[0] is not None:
-        raise CallSampleError(verdict[0])
-    try:
-        payload = run_rank_tasks(config, device, budget, rank, world)
-    except Exception as e:                   # into the payload: a rank that raised before the gather would leave the others waiting
-        log.error(_error_text(e))
-        payload = {"rank": rank, "tasks": [], "failed": [], "nm": None, "stats": {}, "error": _error_text(e)}
-    t1 = time.perf_counter()
-    gathered = [None] * world if rank == 0 else None
-    tdist.gather_object(payload, gathered, dst=0)
-    status = [None]
-    if rank == 0:
-        t2 = time.perf_counter()
-        try:
-            written, vcf_s, snf_s = write_rank_outputs(config, getattr(config, "contig_lengths", []), gathered, tasks.device_context(device))
-            status[0] = (True, written)
-        except Exception as e:
-            status[0] = (False, _error_text(e))
-        t3 = time.perf_counter()
-        if status[0][0] and stats is not None:
-            stats.update({k: v for k, v in payload["stats"].items() if k not in ("tasks", "weight", "inflated_bytes")})
-            stats["vcf_write_s"] += vcf_s
-            stats["snf_write_s"] = snf_s
-            stats["ranks"] = [dict(p["stats"], failed=p["failed"]) for p in gathered]
-            stats["gather_s"], stats["write_s"] = t2 - t1, t3 - t2
-            stats["wall_s"] = t3 - t0
-    tdist.broadcast_object_list(status, src=0)
-    ok, value = status[0]
-    if not ok:
-        raise CallSampleError(value)
-    return value
+    from . import dist
+    timing, merged = {}, {}
+
+    def write(gathered):
+        written, merged["vcf_s"], merged["snf_s"] = write_rank_outputs(config, getattr(config, "contig_lengths", []), gathered,
+                                                                       tasks.device_context(device))
+        merged["gathered"] = gathered
+        return written
+
+    written = dist.rank_run(lambda: check_outputs(config), lambda rank, world: run_rank_tasks(config, device, budget, rank, world), write,
+                            CallSampleError, log,
+                            lambda rank, text: {"rank": rank, "tasks": [], "failed": [], "nm": None, "stats": {}, "error": text}, timing)
+    if timing and stats is not None:         # rank 0
+        gathered = merged["gathered"]
+        stats.update({k: v for k, v in gathered[0]["stats"].items() if k not in ("tasks", "weight", "inflated_bytes")})
+        stats["vcf_write_s"] += merged["vcf_s"]
+        stats["snf_write_s"] = merged["snf_s"]
+        stats["ranks"] = [dict(p["stats"], failed=p["failed"]) for p in gathered]
+        stats.update(timing)
+    return written

@@ -13,14 +13,18 @@ sniffles:371-481, parallel.py:372-572 and result.py:133-243.
     keeps them (a sorted batch's calls below the task's highest stored position are dropped), and written through vcf.open_output;
   * with --reference, the FASTA's planned contigs are loaded to the device once (tasks.reference_for, as sniffles:253-256 and
     result.py:210-214 open it for the writer of either ordering), every allele interval the records of a pass can ask for is gathered in
-    one Reference.prefetch, and VCFWriter.write_call takes REF / ALT from it after the population annotation.
+    one Reference.prefetch, and VCFWriter.write_call takes REF / ALT from it after the population annotation;
+  * with --gpus N > 1, under torchrun, every rank plans alike, runs the tasks dist.lpt_assign gives it over their SNF bytes
+    (dist.combine_task_weights) and formats their records into text, and rank 0 writes the file of one GPU (combine_snfs_ranks).
 
 Deviations from the reference: an SNF that is missing, unreadable or whose header has no contig_lengths is refused with a message instead
 of a traceback; a header without snf_format_version (as this package's SNF writer leaves it) is taken as the current version; the dropped
 calls of CombineResultTmpFile are counted and logged, not written to an `-unsorted.part.vcf`; a population SNF that is missing, has no
 `population` header record or holds blocks that are not PopulationVariant lists is refused before any output is opened; an INS population
 variant with svlen 0 that reaches the alignment test, where the reference's worker divides by zero, stops the run with a message naming
-it; a FASTA that cannot be opened is logged once, where CombineResultTmpFile logs it for every task's part."""
+it; a FASTA that cannot be opened is logged once, where CombineResultTmpFile logs it for every task's part (on several GPUs, once by
+every rank that cannot read its contigs of it, and every rank then runs without it, as one GPU does).  On several GPUs a run in which any rank fails writes no file at all, and every rank raises the same CombineError
+naming the first failed rank and its message, where one GPU leaves a plain .vcf written up to the failure."""
 import contextlib
 import logging
 import os
@@ -396,52 +400,31 @@ def combine_snfs(config, device=0, budget=None, stats=None):
     PASS_CANDIDATES).  stats: a dict that receives the wall-clock split (header_s, decode_s, device_s, call_group_s, write_s, passes and
     per-pass task and candidate counts, dropped; with --combine-population population_s for the decode and load of the population SNF and
     population_match_s for its matches; with --reference reference_s for the FASTA load and, per pass, prefetch_s and prefetch_bytes of
-    its allele gather).  Returns the number of VCF records written."""
-    st = stats if stats is not None else {}
-    st.update(passes=0, pass_tasks=[], pass_candidates=[], header_s=0.0, decode_s=0.0, device_s=0.0, call_group_s=0.0, write_s=0.0, dropped=0,
-              population_s=0.0, population_match_s=0.0, reference_s=0.0, prefetch_s=[], prefetch_bytes=[])
-    t0 = time.perf_counter()
+    its allele gather).  Returns the number of VCF records written.
+
+    With --gpus N > 1 and an initialised process group of N ranks (torchrun --nproc-per-node N -m sniffles_b200 ... --gpus N) the run goes
+    through combine_snfs_ranks; without a process group it runs on one GPU, as it does with --gpus 1."""
     config.mode = "combine"
+    gpus = getattr(config, "gpus", 1)
+    if gpus > 1:
+        world = call._world_size()
+        if world == gpus:
+            return combine_snfs_ranks(config, device, budget, stats)
+        if world > 1:
+            raise CombineError(f"--gpus {gpus} does not match the {world} ranks of the process group")
+        log.warning(f"--gpus {gpus}: combine mode runs on one GPU without torchrun; to run it on {gpus} GPUs launch torchrun --standalone "
+                    f"--nproc-per-node {gpus} -m sniffles_b200 ... --gpus {gpus}")
+    st = stats if stats is not None else {}
+    st.update(_new_stats())
+    t0 = time.perf_counter()
     check_outputs(config)
-    contig_lengths, reqc = read_inputs(config)
-    planned = plan_tasks(config, contig_lengths)
-    tmpfile = len(config.snf_input_info) > config.combine_max_inmemory_results
-    if tmpfile:
-        log.info("Using tmp file aggregation for merge.")
-        if config.sort:
-            log.warning(f"Sorting is not supported above --combine-max-inmemory-results ({config.combine_max_inmemory_results}) inputs: "
-                        f"the calls of a task that come out of order are dropped")
-            if config.vcf_output_bgz:                    # sniffles:453-457
-                config.vcf = config.vcf.removesuffix(".gz").removesuffix(".bgz")
-                config.no_sort = True
-                log.warning("Result will be unsorted and uncompressed")
-    log.info(f"Verified headers for {len(config.snf_input_info)} .snf files.")
+    contig_lengths, reqc, planned, tmpfile = _prepare(config)
     st["header_s"] = time.perf_counter() - t0
     contigs = list(dict.fromkeys(t.contig for t in planned))
-    pop = None
-    if config.combine_population:                        # sniffles:433-435, parallel.py:454-455: opened and checked before any output
-        tp = time.perf_counter()
-        pop = Population(config.combine_population, contigs)
-        st["population_s"] += time.perf_counter() - tp
-    readers = {}
-    ctx = tasks.device_context(device)
-    if pop is not None:
-        tp = time.perf_counter()
-        try:
-            pop.load(ctx)
-        except Exception as e:
-            raise CombineError(f"Loading the population SNF {pop.path} (--combine-population) to the device failed: {e}") from e
-        st["population_s"] += time.perf_counter() - tp
-        log.info(f"Population SNF {pop.path}: {len(pop.variants)} variants in the run's contigs")
-    reference = None
-    if getattr(config, "reference", None):               # sniffles:253-256; logged and left out when it cannot be read
-        log.info(f"Opening for reading: {config.reference}")
-        tr = time.perf_counter()
-        reference = tasks.reference_for(ctx, config.reference, contigs)
-        st["reference_s"] = time.perf_counter() - tr
+    ctx, pop, reference = _device_inputs(config, device, contigs, st)
     if budget is None:
         budget = PASS_CANDIDATES
-    written = 0
+    written, readers = 0, {}
     try:
         readers = {s["internal_id"]: snf.SNFReader(s["filename"]) for s in config.snf_input_info}
         with contextlib.ExitStack() as stack:
@@ -452,19 +435,81 @@ def combine_snfs(config, device=0, budget=None, stats=None):
                 stack.callback(handle.close)
             writer = vcf.VCFWriter(config, handle, reference)
             writer.write_header(contig_lengths)
+
+            def write(task, calls):
+                return sum(writer.write_call(c) for c in calls)
+
             for group in call.group_passes(_decoded(config, planned, readers, st), budget, size=lambda fp: len(fp.cands)):
-                fp = join(group)
-                written += _run_pass(ctx, fp, config, reqc, writer, tmpfile, st, pop)
+                written += _run_pass(ctx, join(group), config, reqc, write, tmpfile, st, pop, reference)
             t1 = time.perf_counter()
         st["write_s"] += time.perf_counter() - t1
     finally:
         for r in readers.values():
             r.close()
-    if st["dropped"]:
-        log.warning(f"{st['dropped']} calls came out of position order in their task and were left out (CombineResultTmpFile)")
-    log.info(f"Wrote {written} called SVs to {config.vcf}")
+    _log_written(config, written, st["dropped"])
     st["wall_s"] = time.perf_counter() - t0
     return written
+
+
+def _new_stats():
+    return dict(passes=0, pass_tasks=[], pass_candidates=[], header_s=0.0, decode_s=0.0, device_s=0.0, call_group_s=0.0, write_s=0.0, dropped=0,
+                population_s=0.0, population_match_s=0.0, reference_s=0.0, prefetch_s=[], prefetch_bytes=[])
+
+
+def _prepare(config, warn=True):
+    """the header pass and the plan every run of the inputs makes alike -> (contig lengths, {internal id: re-QC}, planned tasks, whether
+    the results are kept as CombineResultTmpFile keeps them).  Above --combine-max-inmemory-results inputs a sorted .vcf.gz becomes the
+    plain, unsorted file (sniffles:453-457).  warn: log the warnings of that ordering (one rank of several logs them)."""
+    contig_lengths, reqc = read_inputs(config)
+    planned = plan_tasks(config, contig_lengths)
+    tmpfile = len(config.snf_input_info) > config.combine_max_inmemory_results
+    if tmpfile:
+        log.info("Using tmp file aggregation for merge.")
+        if config.sort:
+            if warn:
+                log.warning(f"Sorting is not supported above --combine-max-inmemory-results ({config.combine_max_inmemory_results}) inputs: "
+                            f"the calls of a task that come out of order are dropped")
+            if config.vcf_output_bgz:
+                config.vcf = config.vcf.removesuffix(".gz").removesuffix(".bgz")
+                config.no_sort = True
+                if warn:
+                    log.warning("Result will be unsorted and uncompressed")
+    log.info(f"Verified headers for {len(config.snf_input_info)} .snf files.")
+    return contig_lengths, reqc, planned, tmpfile
+
+
+def _device_inputs(config, device, contigs, st, load=True):
+    """the device context of `device`, and, when `load`, with --combine-population the population SNF's variants of `contigs` (read before
+    the context is made, so that a bad file is refused before any device work: sniffles:433-435, parallel.py:454-455) loaded on it, and
+    with --reference the FASTA's `contigs` resident on it (sniffles:253-256; logged and left out when it cannot be read).  Returns (ctx,
+    Population or None, fasta.Reference or None)."""
+    pop = None
+    if config.combine_population and load:
+        tp = time.perf_counter()
+        pop = Population(config.combine_population, contigs)
+        st["population_s"] += time.perf_counter() - tp
+    ctx = tasks.device_context(device)
+    if pop is not None:
+        tp = time.perf_counter()
+        try:
+            pop.load(ctx)
+        except Exception as e:
+            raise CombineError(f"Loading the population SNF {pop.path} (--combine-population) to the device failed: {e}") from e
+        st["population_s"] += time.perf_counter() - tp
+        log.info(f"Population SNF {pop.path}: {len(pop.variants)} variants in the run's contigs")
+    reference = None
+    if getattr(config, "reference", None) and load:
+        log.info(f"Opening for reading: {config.reference}")
+        tr = time.perf_counter()
+        reference = tasks.reference_for(ctx, config.reference, contigs)
+        st["reference_s"] = time.perf_counter() - tr
+    return ctx, pop, reference
+
+
+def _log_written(config, written, dropped):
+    if dropped:
+        log.warning(f"{dropped} calls came out of position order in their task and were left out (CombineResultTmpFile)")
+    log.info(f"Wrote {written} called SVs to {config.vcf}")
 
 
 def _decoded(config, planned, readers, st):
@@ -476,10 +521,10 @@ def _decoded(config, planned, readers, st):
         yield fp
 
 
-def _run_pass(ctx, fp, config, reqc, writer, tmpfile, st, pop=None):
+def _run_pass(ctx, fp, config, reqc, write, tmpfile, st, pop=None, reference=None):
     """one device call for the pass's tasks, SVGroup.call on the host, the population annotation of every call the pass made (one device
-    call), with the writer's reference the allele intervals of every call the pass stores (one device gather), the records written;
-    returns the records written"""
+    call), with `reference` the allele intervals of every call the pass stores (one device gather), then write(task, its stored calls) ->
+    records written, per task in task order; returns the records written"""
     from . import binding
     flat = fp.arrays()
     t0 = time.perf_counter()
@@ -505,20 +550,128 @@ def _run_pass(ctx, fp, config, reqc, writer, tmpfile, st, pop=None):
     for k in range(len(fp.tasks)):
         calls, dropped = stored_calls(batches[k], tmpfile, config.sort)
         st["dropped"] += dropped
-        stored.extend(calls)
+        stored.append(calls)
     prefetch_s = 0.0
-    if writer.reference is not None:                     # after the annotation: the population match compares the SNF ALT
+    if reference is not None:                            # after the annotation: the population match compares the SNF ALT
         tr = time.perf_counter()
-        st["prefetch_bytes"].append(writer.reference.prefetch(vcf.reference_intervals(stored, config)))
+        st["prefetch_bytes"].append(reference.prefetch(vcf.reference_intervals([c for calls in stored for c in calls], config)))
         prefetch_s = time.perf_counter() - tr
         st["prefetch_s"].append(prefetch_s)
-    written = 0
-    for c in stored:
-        written += writer.write_call(c)
+    written = sum(write(task, calls) for task, calls in zip(fp.tasks, stored))
     st["passes"] += 1
     st["pass_tasks"].append(len(fp.tasks))
     st["pass_candidates"].append(len(fp.cands))
     st["device_s"] += t1 - t0
     st["call_group_s"] += tp - t1
     st["write_s"] += time.perf_counter() - t2 - prefetch_s
+    return written
+
+
+def run_rank_tasks(config, device, budget, rank, world, plan=None):
+    """one rank's share of a multi-GPU combine run: the header pass and plan every rank makes alike (_prepare; its warnings logged by rank
+    0 alone), the tasks dist.lpt_assign gives this rank over dist.combine_task_weights, then the pass loop of combine_snfs over them in
+    task-id order under this rank's own candidate budget, each task's stored calls formatted here into VCF text.  With
+    --combine-population / --reference only the contigs of this rank's tasks are loaded, and nothing when it has none.
+
+    Before any pass, every rank reaches one all_gather_object of (set-up ok, FASTA read): a rank whose set-up failed raises its error,
+    the others then run no task (the failed rank's payload names it); and when any rank could not read its contigs of the FASTA, every
+    rank runs without it, as one GPU runs without a FASTA any of whose planned contigs it cannot read.  plan: a dict that receives the
+    contig lengths (rank 0 writes the header from them).  Returns the payload rank 0 merges (write_rank_outputs): {"rank", "tasks":
+    [(task id, VCF text, records)], "dropped", "stats", "error": None}."""
+    import io
+    import torch.distributed as tdist
+    from . import dist
+    st = _new_stats()
+    t0 = time.perf_counter()
+    out, readers, failure, reference = [], {}, None, None
+    try:
+        try:
+            contig_lengths, reqc, planned, tmpfile = _prepare(config, warn=rank == 0)
+            readers = {s["internal_id"]: snf.SNFReader(s["filename"]) for s in config.snf_input_info}
+            weights = dist.combine_task_weights(readers, planned)
+            owner = dist.lpt_assign(weights, world)
+            mine = [t for t, o in zip(planned, owner) if o == rank]
+            st.update(tasks=len(mine), weight=sum(w for w, o in zip(weights, owner) if o == rank), header_s=time.perf_counter() - t0)
+            ctx, pop, reference = _device_inputs(config, device, list(dict.fromkeys(t.contig for t in mine)), st, load=bool(mine))
+            fasta_read = reference is not None or not (getattr(config, "reference", None) and mine)
+        except Exception as e:               # after the all-gather below: a rank that raised before it would leave the others waiting
+            failure, fasta_read = e, True
+        verdicts = [None] * world
+        tdist.all_gather_object(verdicts, (failure is None, fasta_read))
+        if failure is not None:
+            raise failure
+        if not all(ok for ok, _ in verdicts):
+            st["wall_s"] = time.perf_counter() - t0
+            return {"rank": rank, "tasks": [], "dropped": 0, "stats": st, "error": None}
+        if not all(read for _, read in verdicts):
+            if reference is not None:
+                log.warning("another rank could not read its contigs of the reference FASTA: this rank runs without it, as one GPU would")
+            reference = None
+        if plan is not None:
+            plan["contig_lengths"] = contig_lengths
+
+        def write(task, calls):
+            buf = io.StringIO()
+            writer = vcf.VCFWriter(config, buf, reference)
+            n = sum(writer.write_call(c) for c in calls)
+            out.append((task.id, buf.getvalue(), n))
+            return n
+
+        for group in call.group_passes(_decoded(config, mine, readers, st), PASS_CANDIDATES if budget is None else budget,
+                                       size=lambda fp: len(fp.cands)):
+            _run_pass(ctx, join(group), config, reqc, write, tmpfile, st, pop, reference)
+    finally:
+        for r in readers.values():
+            r.close()
+    st["wall_s"] = time.perf_counter() - t0
+    return {"rank": rank, "tasks": out, "dropped": st["dropped"], "stats": st, "error": None}
+
+
+def write_rank_outputs(config, contig_lengths, payloads, device=0):
+    """rank 0's merge of every rank's payload (run_rank_tasks): when any rank failed, no file is written and CombineError names the first
+    failed rank and its message; otherwise the VCF header, then every task's text in task-id order through vcf.open_output (a .vcf.gz
+    compressed on `device` and indexed).  Logs the run's dropped calls and records.  Returns (records written, calls dropped)."""
+    failed = [p for p in payloads if p["error"] is not None]
+    if failed:
+        raise CombineError(f"rank {failed[0]['rank']}: {failed[0]['error']}")
+    done = sorted((t for p in payloads for t in p["tasks"]), key=lambda t: t[0])
+    dropped = sum(p["dropped"] for p in payloads)
+    written = 0
+    ctx = tasks.device_context(device) if config.vcf_output_bgz else None
+    with vcf.open_output(config, ctx) as handle:          # a .vcf.gz is compressed and indexed when the writing ends without an error
+        vcf.VCFWriter(config, handle).write_header(contig_lengths)
+        for _, text, n in done:
+            handle.write(text)
+            written += n
+    _log_written(config, written, dropped)
+    return written, dropped
+
+
+def combine_snfs_ranks(config, device, budget=None, stats=None):
+    """combine_snfs over the ranks of an initialised torch.distributed process group, through dist.rank_run: rank 0 checks the outputs
+    (check_outputs; no other rank calls it) and broadcasts the verdict; every rank runs its own tasks (run_rank_tasks) and sends its
+    payload to rank 0, an error included.  Rank 0 writes the file (write_rank_outputs): every rank returns the same count or raises the
+    same CombineError.  Rank 0 holds every rank's VCF text at once, host memory in proportion to the output file.
+
+    stats on rank 0: the keys of combine_snfs for rank 0's own work, with "dropped" summed over the ranks and "write_s" the time of rank
+    0's merge and write (each rank's own formatting time is its "write_s" under "ranks"), plus "ranks" (per rank its split, task count
+    and weight) and "gather_s"."""
+    from . import dist
+    plan, timing, merged = {}, {}, {}
+
+    def write(gathered):
+        # a rank 0 whose header pass failed has no contig lengths: write_rank_outputs names the failed rank before it needs them
+        written, merged["dropped"] = write_rank_outputs(config, plan.get("contig_lengths", []), gathered, device)
+        merged["gathered"] = gathered
+        return written
+
+    written = dist.rank_run(lambda: check_outputs(config), lambda rank, world: run_rank_tasks(config, device, budget, rank, world, plan),
+                            write, CombineError, log, lambda rank, text: {"rank": rank, "tasks": [], "dropped": 0, "stats": {}, "error": text},
+                            timing)
+    if timing and stats is not None:         # rank 0
+        gathered = merged["gathered"]
+        stats.update({k: v for k, v in gathered[0]["stats"].items() if k not in ("tasks", "weight")})
+        stats["dropped"] = merged["dropped"]
+        stats["ranks"] = [p["stats"] for p in gathered]
+        stats.update(timing)
     return written

@@ -4,9 +4,11 @@ the per-rank candidate buffers before VCF emission.  torch.distributed is used f
 collective only (NCCL over NVLink on the GPU box, gloo in the CPU tests).
 
 Calling a sample on several GPUs (call.call_sample_ranks) weighs its tasks with task_weights,
-assigns them with lpt_assign, and gathers each rank's finished VCF text and SNF parts instead."""
+assigns them with lpt_assign, and gathers each rank's finished VCF text and SNF parts instead.  Combining samples on several GPUs
+(combine_run.combine_snfs_ranks) weighs its combine tasks with combine_task_weights.  Both run through rank_run."""
 import bisect
 import os
+import time
 
 import numpy as np
 
@@ -58,6 +60,70 @@ def task_weights(bam, planned, regions_by_contig=None):
             continue
         out.append(sum(chunk_bytes(vb, ve) for a, b in windows for vb, ve in bam.merged_chunks(name, a, b)))
     return out
+
+
+def combine_task_weights(readers, planned):
+    """per planned combine.CombineTask, the compressed SNF bytes of its blocks summed over every sample: the lengths of the parts each
+    SNFReader.index ({contig: {str(block): [(offset, length), ...]}}) lists for the task's block_indices.  Read from the headers alone:
+    no block is decoded.  readers: {internal id: snf.SNFReader}"""
+    out = []
+    for task in planned:
+        w = 0
+        for r in readers.values():
+            blocks = r.index.get(task.contig, {})
+            w += sum(length for b in task.block_indices for _, length in blocks.get(str(b), ()))
+        out.append(w)
+    return out
+
+
+def rank_run(check, work, write, error, log, failed_payload, timing=None):
+    """One run over the ranks of an initialised torch.distributed process group (one process per GPU; gloo, since the only collectives
+    carry host objects).  Rank 0 alone runs check() and broadcasts its verdict (an `error` raised there stops every rank with its
+    message).  Every rank then runs work(rank, world) -> its payload; an exception is logged and caught into failed_payload(rank, text), so
+    that every rank reaches the gather.  gather_object brings the payloads, in rank order, to rank 0, which runs write(payloads) and
+    broadcasts (ok, its value or the error): every rank returns the same value or raises the same `error`.
+
+    timing: a dict that receives, on rank 0 when the write succeeds, gather_s (from the end of its own work to the end of the gather),
+    write_s and wall_s."""
+    import torch.distributed as tdist
+
+    def text(e):
+        return str(e) if isinstance(e, error) else f"{type(e).__name__}: {e}"
+
+    rank, world = tdist.get_rank(), tdist.get_world_size()
+    t0 = time.perf_counter()
+    verdict = [None]
+    if rank == 0:
+        try:
+            check()
+        except error as e:
+            verdict[0] = str(e)
+    tdist.broadcast_object_list(verdict, src=0)
+    if verdict[0] is not None:
+        raise error(verdict[0])
+    try:
+        payload = work(rank, world)
+    except Exception as e:                   # into the payload: a rank that raised before the gather would leave the others waiting
+        log.error(text(e))
+        payload = failed_payload(rank, text(e))
+    t1 = time.perf_counter()
+    gathered = [None] * world if rank == 0 else None
+    tdist.gather_object(payload, gathered, dst=0)
+    status = [None]
+    if rank == 0:
+        t2 = time.perf_counter()
+        try:
+            status[0] = (True, write(gathered))
+        except Exception as e:
+            status[0] = (False, text(e))
+        t3 = time.perf_counter()
+        if status[0][0] and timing is not None:
+            timing.update(gather_s=t2 - t1, write_s=t3 - t2, wall_s=t3 - t0)
+    tdist.broadcast_object_list(status, src=0)
+    ok, value = status[0]
+    if not ok:
+        raise error(value)
+    return value
 
 
 def subset_block(block, task_ids):
