@@ -13,16 +13,16 @@ pytestmark = pytest.mark.gpu
 SLICES = (1, 2, 4, 7)
 
 
-def _runs(blk, *args):
-    """{k: Result} over SLICES on one context, and the oracle's result"""
+def _runs(blk, *args, slices=SLICES, seq_on_demand=False):
+    """{k: Result} over `slices` on one context, and the oracle's result"""
     import oracle.oracle as orc
     cfg = abi.Config.from_sniffles(sconfig.default_config(*args))
     ctx = binding.Context(0)
     got = {}
     try:
         ctx.set_config(cfg)
-        ctx.load(blk)
-        for k in SLICES:
+        ctx.load(blk, seq_on_demand=seq_on_demand)
+        for k in slices:
             ctx.set_consensus_slices(k)
             got[k] = ctx.run(want_leads=False)
     finally:
@@ -30,13 +30,13 @@ def _runs(blk, *args):
     return got, orc.run(blk, cfg, 3, 4)
 
 
-def _check(blk, *args):
-    got, want = _runs(blk, *args)
-    one = got[1]
+def _check(blk, *args, slices=SLICES, seq_on_demand=False):
+    got, want = _runs(blk, *args, slices=slices, seq_on_demand=seq_on_demand)
+    one = got[slices[0]]
     for k, res in got.items():
         for name in ("cand", "cand_leads", "rnames", "rn_off", "alt"):
             a, b = getattr(one, name), getattr(res, name)
-            assert a.dtype == b.dtype and a.shape == b.shape and a.tobytes() == b.tobytes(), f"{name} with {k} slices differs from 1 slice"
+            assert a.dtype == b.dtype and a.shape == b.shape and a.tobytes() == b.tobytes(), f"{name} with {k} slices differs from {slices[0]}"
         devcheck.assert_same(want, res, check_leads=False)
     return one
 
