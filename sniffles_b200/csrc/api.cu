@@ -932,7 +932,10 @@ static int enqueue_stage_c(snfb_ctx* ctx) {
         CUDA_TRY(cudaMemcpyAsync(ctx->h_fin, ctr, sizeof(DevCounters), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
         const unsigned long long nreq = ctx->h_fin->n_req, nunits = ctx->h_fin->n_req_units;
-        if (nreq <= ctx->cap.req && nunits <= ctx->cap.req16 && nreq) {
+        // slices that do not fit the arena are not gathered and their offsets point past it: the kernels would read outside the arena.
+        // caps_fit sees the counts at the end of the run and redoes it with a larger arena, so stage C is left out of this attempt.
+        if (nreq > ctx->cap.req || nunits > ctx->cap.req16) return 0;
+        if (nreq) {
             if (ctx->h_seq_req.ensure(sizeof(consensus::SeqReq) * (nreq + 1)) || ctx->h_seq_arena.ensure(nunits * 16 + 64)) return fail(ctx, "out of pinned memory (seq arena)");
             CUDA_TRY(cudaMemcpyAsync(ctx->h_seq_req.p, ctx->seq_req, sizeof(consensus::SeqReq) * nreq, cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaStreamSynchronize(st));

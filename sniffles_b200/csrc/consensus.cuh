@@ -45,6 +45,8 @@ struct C {
 };
 
 __device__ __forceinline__ uint8_t seq_code(const uint8_t* sq, long long q) { const uint8_t v = sq[q >> 1]; return (q & 1) ? (v & 15) : (v >> 4); }
+// bytes of a read's 4-bit copy in scratch (the seq arena's packing, from nibble 0): whole 8-byte words
+__device__ __forceinline__ uint32_t packed_bytes(uint32_t len) { return ((len + 15u) & ~15u) / 2u; }
 
 // choose the best read, size the outputs
 __global__ void k_plan(C c) {
@@ -52,17 +54,19 @@ __global__ void k_plan(C c) {
     for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < nc; i += (unsigned long long)gridDim.x * blockDim.x) {
         uint32_t al = 0, sl = 0, heavy_n = 0, light_n = 0, tiles = 0; bool big = false;
         if (c.cand[i].svtype == SNFB_INS && !c.cfg.symbolic) {
-            const snfb_cand* cd = &c.cand[i]; long nm = 0, bi = -1; long long bd = 0; long long tot = 0;
+            const snfb_cand* cd = &c.cand[i]; long nm = 0, bi = -1; long long bd = 0; long long tot = 0, bpk = 0;
             for (int k = 0; k < cd->lead_n; ++k) { const snfb_lead* l = &c.cand_leads[cd->lead_off + k]; if (!(l->flags & SNFB_LF_HAS_SEQ)) continue;
                 // abs(len(seq) - svlen) + abs(ref_start - pos) * 1.5, compared exactly in halves
                 long long a = (long long)l->seq_len - cd->svlen; if (a < 0) a = -a; long long p = (long long)l->ref_start - cd->pos; if (p < 0) p = -p;
-                const long long d = 2 * a + 3 * p; if (nm == 0 || d < bd) { bd = d; bi = k; } ++nm; tot += ((long long)l->seq_len + 7) & ~7ll; }
+                const long long d = 2 * a + 3 * p; if (nm == 0 || d < bd) { bd = d; bi = k; } ++nm;
+                const long long pk = c.out_pn[cd->lead_off + k] != 1 ? packed_bytes((uint32_t)l->seq_len) : 0; tot += pk; if (bi == k) bpk = pk; }
             if (nm > 0) {
                 const uint32_t L = (uint32_t)c.cand_leads[cd->lead_off + bi].seq_len; al = L;
                 const bool cons = (nm - 1 >= c.cfg.consensus_min_reads) && !c.cfg.no_consensus;
-                c.plan_best[i] = (uint32_t)bi; c.plan_nother[i] = cons ? (uint32_t)(nm - 1) : 0u; c.plan_otot[i] = (uint32_t)(tot - ((L + 7u) & ~7u));
-                // scratch: best codes | others' codes (every read in a slot of align8(len) bytes) | one row of align4(L) per other read | accept flags | anchor table; 16-byte units
-                const unsigned long long bytes = cons ? (unsigned long long)tot + 8 + (unsigned long long)(nm - 1) * ((L + 3u) & ~3u) + (unsigned long long)(nm - 1) * 16 + 64 + 16 + TAB * 8 : (unsigned long long)L + 24;
+                c.plan_best[i] = (uint32_t)bi; c.plan_nother[i] = cons ? (uint32_t)(nm - 1) : 0u; c.plan_otot[i] = (uint32_t)(tot - bpk);
+                // scratch: best codes | best read packed | the merged other reads packed (a slot of packed_bytes(len) each; a read of one
+                // piece is read from the seq arena) | one row of align4(L) per other read | accept flags | anchor table; 16-byte units
+                const unsigned long long bytes = cons ? (unsigned long long)((L + 7u) & ~7u) + packed_bytes(L) + (unsigned long long)(tot - bpk) + 8 + (unsigned long long)(nm - 1) * ((L + 3u) & ~3u) + (unsigned long long)(nm - 1) * 16 + 64 + 16 + TAB * 8 : (unsigned long long)L + 24;
                 sl = (uint32_t)((bytes + 15) / 16);
                 c.cand_rw[i].alt_len = (int)L;
                 // prep queue: the heavy tail (long insertions with many reads) is scheduled first; one align item per supporting read
@@ -91,7 +95,7 @@ __global__ void k_plan_finish(C c) {
         uint32_t row = 0, ro = 0;
         for (int k = 0; no && k < cd->lead_n; ++k) { const snfb_lead* l = &c.cand_leads[cd->lead_off + k]; if (!(l->flags & SNFB_LF_HAS_SEQ) || (uint32_t)k == bi) continue;
             if ((unsigned long long)base + row < c.item_cap) { C::Item it; it.cand = (uint32_t)i; it.k = (uint32_t)k; it.row = row; it.rd_off = ro; dst[base + row] = it; }
-            ++row; ro += ((uint32_t)l->seq_len + 7u) & ~7u; }
+            ++row; if (c.out_pn[cd->lead_off + k] != 1) ro += packed_bytes((uint32_t)l->seq_len); }
         const uint32_t nt = c.q_cnt[Q_TILE * col + i], tb = c.q_off[Q_TILE * col + i];
         for (uint32_t t = 0; t < nt; ++t) if ((unsigned long long)tb + t < c.tile_cap) c.tiles[tb + t] = make_uint2((uint32_t)i, t);
     }
@@ -116,19 +120,39 @@ __global__ void k_plan_slices(C c, int k) {
     c.work->slice[s] = sl;
 }
 
-// unpack `len` bases starting at nibble `off` of sq into dst (one code per byte); `tid`/`nthr` = cooperating threads.
-// A thread takes 8 consecutive bases per step: two aligned words of the 4-bit arena (the second only when the bases reach
-// into it), nibbles swapped into little-endian order, one funnel shift to the first base, two spreads, one 8-byte store.
 __device__ __forceinline__ uint32_t nib_swap(uint32_t w) { return ((w & 0x0f0f0f0fu) << 4) | ((w >> 4) & 0x0f0f0f0fu); }
 __device__ __forceinline__ uint32_t spread4(uint32_t x) { const uint32_t t = (x | (x << 8)) & 0x00ff00ffu; return (t | (t << 4)) & 0x0f0f0f0fu; }
+// A 4-bit string: base q is nibble o + q from the aligned word w on (o < 8; high nibble first in each byte, as in the seq arena).
+// get8 returns bases [q, q + 8), q >= 0, with base q + t in bits 4t..4t+3: two aligned words (the second only when the first n bases
+// reach into it, so no byte past base q + n - 1's word is read), nibbles swapped into little-endian order, one funnel shift to the
+// first base.  Plain loads: k_align reads a merged read's copy that the same kernel wrote.  get8<false> reads a string whose words
+// already hold base q in nibble q (the best read's copy), without the swap.
+struct Nib {
+    const uint32_t* w; int o;
+    __device__ static __forceinline__ Nib at(const uint8_t* p, long long q) {
+        const uintptr_t A = (uintptr_t)(p + (q >> 1));
+        Nib r; r.w = reinterpret_cast<const uint32_t*>(A & ~(uintptr_t)3); r.o = (int)((A & 3) << 1) | (int)(q & 1); return r;
+    }
+    template <bool SWAP = true> __device__ __forceinline__ uint32_t get8(int q, int n) const {
+        const int b = o + q; const uint32_t* x = w + (b >> 3); const int qn = b & 7;
+        const uint32_t lo = SWAP ? nib_swap(x[0]) : x[0], hi = qn + n > 8 ? (SWAP ? nib_swap(x[1]) : x[1]) : 0u;
+        return __funnelshift_r(lo, hi, 4 * qn);
+    }
+    // bases [r, r + m) (m <= 8) of the string's first n bases at bits 4t; bases outside [0, n) read as 0
+    __device__ __forceinline__ uint32_t take(int r, int m, int n) const {
+        const int a = r < 0 ? 0 : r, e = r + m < n ? r + m : n;
+        if (e <= a) return 0u;
+        const int k = e - a; uint32_t x = get8(a, k);
+        if (k < 8) x &= (1u << (4 * k)) - 1u;
+        return x << (4 * (a - r));
+    }
+};
 __device__ __forceinline__ uint2 unpack8(const uint8_t* __restrict__ sq, long long q, int n) {
-    const uintptr_t A = (uintptr_t)(sq + (q >> 1));
-    const uint32_t* w = reinterpret_cast<const uint32_t*>(A & ~(uintptr_t)3);
-    const int qn = (int)((A & 3) << 1) | (int)(q & 1);
-    const uint32_t lo = nib_swap(__ldg(w)), hi = qn + n > 8 ? nib_swap(__ldg(w + 1)) : 0u;
-    const uint32_t x = __funnelshift_r(lo, hi, 4 * qn);
+    const uint32_t x = Nib::at(sq, q).get8(0, n);
     return make_uint2(spread4(x & 0xffffu), spread4(x >> 16));
 }
+// unpack `len` bases starting at nibble `off` of sq into dst (one code per byte); `tid`/`nthr` = cooperating threads.
+// A thread takes 8 consecutive bases per step (unpack8: get8, two spreads) and stores them as one 8-byte word.
 __device__ __forceinline__ void unpack_span(const uint8_t* __restrict__ sq, long long off, int len, uint8_t* __restrict__ dst, int tid, int nthr) {
     const int full = ((uintptr_t)dst & 7) == 0 ? (len & ~7) : 0;          // whole 8-base groups go out as aligned 8-byte stores, eight loads in flight
     int jb = tid * 8;
@@ -145,6 +169,11 @@ __device__ __forceinline__ void unpack_span(const uint8_t* __restrict__ sq, long
         for (int t = 0; t < n; ++t) dst[jb + t] = (uint8_t)(((t < 4 ? v.x : v.y) >> (8 * (t & 3))) & 15u);
     }
 }
+// the bases of kept lead `slot` in the seq arena (the full arena, or with seq on demand the compact one)
+__device__ __forceinline__ Nib lead_bases(const C& c, uint32_t slot) {
+    const snfb_lead* l = &c.kleads[slot];
+    return c.arena_off ? Nib::at(c.seq + (size_t)c.arena_off[slot] * 16, l->seq_off & 1) : Nib::at(c.seq + c.rec[l->rec].seq_off, l->seq_off);
+}
 // unpack the (possibly merged) sequence of candidate lead `cl_index` as 4-bit codes, one byte per base, by `nthr` cooperating threads
 __device__ inline void unpack_lead(const C& c, uint32_t cl_index, uint8_t* dst, int tid, int nthr) {
     const uint32_t plo = c.out_plo[cl_index], pn = c.out_pn[cl_index];
@@ -156,6 +185,35 @@ __device__ inline void unpack_lead(const C& c, uint32_t cl_index, uint8_t* dst, 
         o += l->seq_len;
     }
 }
+// pack the (possibly merged) sequence of candidate lead `cl_index`, `len` bases, as one 4-bit string from nibble 0 of the 4-byte
+// aligned dst (packed_bytes(len) bytes, the tail of the last word 0), by `nthr` cooperating threads; in the seq arena's order
+// (`arena_order`, high nibble first) or with base q in nibble q of the little-endian words.  A thread writes whole words; a word
+// gathers 8 bases from the part(s) it overlaps, which it finds by walking the parts forward with its words.
+__device__ inline void pack_lead(const C& c, uint32_t cl_index, long len, uint32_t* dst, int tid, int nthr, bool arena_order) {
+    const uint32_t plo = c.out_plo[cl_index], pn = c.out_pn[cl_index];
+    const long nw = (long)(packed_bytes((uint32_t)len) / 4);
+    uint32_t p = 0; int o = 0, n = 0; Nib b{};
+    if (pn) { const uint32_t slot = c.ord[plo]; b = lead_bases(c, slot); n = c.kleads[slot].seq_len; }
+    for (long w = tid; w < nw; w += nthr) {
+        const int q = 8 * (int)w; uint32_t x = 0;
+        if (pn) {
+            while (o + n <= q && p + 1 < pn) { o += n; ++p; const uint32_t slot = c.ord[plo + p]; b = lead_bases(c, slot); n = c.kleads[slot].seq_len; }
+            x = b.take(q - o, 8, n);
+            int o2 = o + n;
+            for (uint32_t p2 = p + 1; p2 < pn && o2 < q + 8; ++p2) {      // a word that straddles parts
+                const uint32_t slot = c.ord[plo + p2]; const int n2 = c.kleads[slot].seq_len;
+                x |= lead_bases(c, slot).take(q - o2, 8, n2); o2 += n2;
+            }
+        }
+        dst[w] = arena_order ? nib_swap(x) : x;
+    }
+}
+// the bases of candidate lead `cl_index` as k_align reads them: straight from the seq arena when it is one piece, else from its packed
+// copy at `copy` (which the caller fills with pack_lead first)
+__device__ __forceinline__ Nib lead_reader(const C& c, uint32_t cl_index, const uint8_t* copy) {
+    if (c.out_pn[cl_index] == 1) return lead_bases(c, c.ord[c.out_plo[cl_index]]);
+    Nib r; r.w = reinterpret_cast<const uint32_t*>(copy); r.o = 0; return r;
+}
 
 __device__ __forceinline__ uint32_t kmer6(const uint8_t* s) { return (uint32_t)s[0] | ((uint32_t)s[1] << 4) | ((uint32_t)s[2] << 8) | ((uint32_t)s[3] << 12) | ((uint32_t)s[4] << 16) | ((uint32_t)s[5] << 20); }
 // the same from an unaligned pointer with aligned 32-bit loads (reads at most 3 bytes past s + 5)
@@ -166,6 +224,8 @@ __device__ __forceinline__ uint32_t kmer6_u(const uint8_t* s) {
     uint32_t t = x0 & 0x0f0f0f0fu; t = (t | (t >> 4)) & 0x00ff00ffu; t = (t | (t >> 8)) & 0xffffu;
     return t | ((x1 & 15u) << 16) | (((x1 >> 8) & 15u) << 20);
 }
+// kmer6 of the bases [q, q + 6) of a 4-bit string: they are already in kmer6's order
+__device__ __forceinline__ uint32_t kmer6_n(const Nib& s, int q) { return s.get8(q, 6) & 0xffffffu; }
 __device__ __forceinline__ uint32_t kslot(uint32_t key) { return (key * 2654435761u) >> 21; }    // top 11 bits
 
 // seq on demand: the base slices stage C will read, as (source byte offset in the host seq arena, bytes, destination unit)
@@ -195,44 +255,12 @@ __global__ void k_seq_requests(C c, SeqReq* req, unsigned long long req_cap, uin
 
 
 // ================================================================================================
-// k_prep (block per candidate: unpack the best read, build its anchor table in global
+// k_prep (block per candidate: unpack the best read and pack a nibble-aligned 4-bit copy of it, build its anchor table in global
 // scratch, or copy the best read to ALT when there is no consensus) -> k_align (one warp per (candidate, read)
 // item from a heavy-first queue: no block barriers, the heaviest candidate's reads spread over the whole GPU)
 // -> k_vote (one block per (candidate, 4096-column tile)).
 // ================================================================================================
-// ---- byte-string helpers on unaligned pointers, four bytes per step (sliding aligned 32-bit windows).  They may read up to
-//      7 bytes past the last byte asked for; every buffer they are used on is followed by other scratch of the same candidate.
-__device__ __forceinline__ int match_count(const uint8_t* a, const uint8_t* b, long n) {
-    const uint32_t sa = ((uintptr_t)a & 3) * 8, sb = ((uintptr_t)b & 3) * 8;
-    const uint32_t* wa = reinterpret_cast<const uint32_t*>((uintptr_t)a & ~(uintptr_t)3); const uint32_t* wb = reinterpret_cast<const uint32_t*>((uintptr_t)b & ~(uintptr_t)3);
-    uint32_t alo = wa[0], blo = wb[0]; int mt = 0;
-    long q = 0;
-    #pragma unroll 2
-    for (; q + 4 <= n; q += 4) {
-        const uint32_t ahi = *++wa, bhi = *++wb;
-        const uint32_t x = __funnelshift_r(alo, ahi, sa) ^ __funnelshift_r(blo, bhi, sb);
-        mt += __popc(~(((x & 0x7f7f7f7fu) + 0x7f7f7f7fu) | x) & 0x80808080u);       // 0x80 in every byte that is equal
-        alo = ahi; blo = bhi;
-    }
-    if (q < n) {
-        const uint32_t ahi = *++wa, bhi = *++wb;
-        const uint32_t x = __funnelshift_r(alo, ahi, sa) ^ __funnelshift_r(blo, bhi, sb);
-        mt += __popc(~(((x & 0x7f7f7f7fu) + 0x7f7f7f7fu) | x) & 0x80808080u & ((1u << (8 * (n - q))) - 1u));
-    }
-    return mt;
-}
-__device__ __forceinline__ void copy_bytes(uint8_t* dst, const uint8_t* src, long n) {
-    long q = 0;
-    while (q < n && ((uintptr_t)(dst + q) & 3)) { dst[q] = src[q]; ++q; }
-    if (q + 4 <= n) {
-        const uint8_t* s0 = src + q; const uint32_t sh = ((uintptr_t)s0 & 3) * 8;
-        const uint32_t* ws = reinterpret_cast<const uint32_t*>((uintptr_t)s0 & ~(uintptr_t)3); uint32_t lo = ws[0];
-        uint32_t* wd = reinterpret_cast<uint32_t*>(dst + q);
-        #pragma unroll 4
-        for (; q + 4 <= n; q += 4) { const uint32_t hi = *++ws; *wd++ = __funnelshift_r(lo, hi, sh); lo = hi; }
-    }
-    for (; q < n; ++q) dst[q] = src[q];
-}
+// ---- the row's dashes, four bytes per step where the row is word aligned
 __device__ __forceinline__ void fill_dash(uint8_t* dst, long n) {
     long q = 0;
     while (q < n && ((uintptr_t)(dst + q) & 3)) dst[q++] = DASH;
@@ -240,19 +268,18 @@ __device__ __forceinline__ void fill_dash(uint8_t* dst, long n) {
     for (; q < n; ++q) dst[q] = DASH;
 }
 
-__device__ __forceinline__ uint32_t load_u32_unaligned(const uint8_t* p) {
-    const uintptr_t A = (uintptr_t)p; const uint32_t* w = reinterpret_cast<const uint32_t*>(A & ~(uintptr_t)3);
-    return __funnelshift_r(w[0], w[1], (uint32_t)(A & 3) * 8);
-}
-// match_count with the words of [0, n) dealt round robin to the G lanes of a group; the caller adds the lanes up
+// how many of the bases [0, n) of a + ia and b + ib are equal: 8 bases per 32-bit XOR, at any nibble offset on either side (b is the
+// best read's copy, in base order); the 8-base words of [0, n) are dealt round robin to the G lanes of a group, the caller adds the
+// lanes up
 template <int G>
-__device__ __forceinline__ int group_match(const uint8_t* a, const uint8_t* b, long n, int sub) {
+__device__ __forceinline__ int group_match(const Nib& a, long ia, const Nib& b, long ib, long n, int sub) {
     int mt = 0;
-    #pragma unroll 2
-    for (long q = 4L * sub; q < n; q += 4L * G) {
-        const uint32_t x = load_u32_unaligned(a + q) ^ load_u32_unaligned(b + q);
-        uint32_t eq = ~(((x & 0x7f7f7f7fu) + 0x7f7f7f7fu) | x) & 0x80808080u;
-        if (n - q < 4) eq &= (1u << (8 * (n - q))) - 1u;
+    for (long q = 8L * sub; q < n; q += 8L * G) {
+        const int k = n - q < 8 ? (int)(n - q) : 8;
+        uint32_t x = a.get8((int)(ia + q), k) ^ b.get8<false>((int)(ib + q), k);
+        x |= x >> 1; x |= x >> 2;                                       // bit 4t: base t differs
+        uint32_t eq = ~x & 0x11111111u;
+        if (k < 8) eq &= (1u << (4 * k)) - 1u;
         mt += __popc(eq);
     }
     return mt;
@@ -323,10 +350,10 @@ struct BlockGrp {
     }
 };
 
-// (3a) of k_align with G lanes per segment (1: short segments, a lane walks its own; 8: long segments, coalesced words); `tid` of
+// (3a) of k_align with G lanes per segment (1: short segments, a lane walks its own; 4: long segments, 32 bases per group step); `tid` of
 // `nthr` cooperating threads (whole warps)
 template <int G>
-__device__ __forceinline__ long segments_pass(const int* hi, const int* hj, int* hcl, int na, long c0, long j0, long L, const uint8_t* rd, const uint8_t* best, int tid, int nthr) {
+__device__ __forceinline__ long segments_pass(const int* hi, const int* hj, int* hcl, int na, long c0, long j0, long L, const Nib& rd, const Nib& best, int tid, int nthr) {
     const int PER = nthr / G; const int grp = tid / G, sub = tid % G; long span = 0;
     for (int mb = 1; mb < na; mb += PER) {
         const int m = mb + grp; const bool v = m < na;
@@ -335,22 +362,23 @@ __device__ __forceinline__ long segments_pass(const int* hi, const int* hj, int*
         const long d = j - lj; long fwd_j = d; if (cs + fwd_j > L) fwd_j = L - cs;
         const bool el = v && i - li == fwd_j && fwd_j > 0;
         long nc = 0; if (el) { nc = L - 1 - li; if (nc > d) nc = d; if (nc < 0) nc = 0; }      // positions past the end of the best read never match
-        const int mt = group_sum<G>(group_match<G>(rd + lj + 1, best + li + 1, nc, sub));
+        const int mt = group_sum<G>(group_match<G>(rd, lj + 1, best, li + 1, nc, sub));
         // column identity of the copied bases.  Without drift (cs == li, nothing clamped) it is the same sum shifted by one
         // position, and both end positions are anchor k-mer bases that match by construction: reuse mt
         int st = -1; bool second = false;
         if (el) { if (sub == 0) span += d; if (__ddiv_rn((double)mt, (double)d) >= 0.5) { if (cs == li && fwd_j == d && nc == d) st = mt; else second = true; } }
-        const int m2 = group_sum<G>(group_match<G>(rd + lj, best + cs, second ? fwd_j : 0, sub));
+        const int m2 = group_sum<G>(group_match<G>(rd, lj, best, cs, second ? fwd_j : 0, sub));
         if (second) st = m2;
         if (v && sub == 0) hcl[m] = st;
     }
     return span;
 }
 
-// scratch layout of one consensus candidate: best[align8(L)] | other reads' codes [otot] | rows[no][Ls] (Ls = align4(L)) | accept[no] | ... | table
-struct Layout { uint8_t* best; uint8_t* oth; uint8_t* rows; uint8_t* acc; uint32_t Ls; };
+// scratch layout of one consensus candidate: best[align8(L)] | best packed in base order [packed_bytes(L)] | merged other reads packed [otot] |
+// rows[no][Ls] (Ls = align4(L)) | accept[no] | ... | table
+struct Layout { uint8_t* best; uint8_t* best4; uint8_t* oth; uint8_t* rows; uint8_t* acc; uint32_t Ls; };
 __device__ __forceinline__ Layout cand_layout(const C& c, uint32_t ci, uint32_t L, uint32_t no) {
-    Layout y; y.best = c.scr + (size_t)c.scr_off[ci] * 16; y.oth = y.best + ((L + 7u) & ~7u);
+    Layout y; y.best = c.scr + (size_t)c.scr_off[ci] * 16; y.best4 = y.best + ((L + 7u) & ~7u); y.oth = y.best4 + packed_bytes(L);
     y.rows = reinterpret_cast<uint8_t*>(((uintptr_t)(y.oth + c.plan_otot[ci]) + 3) & ~(uintptr_t)3); y.Ls = (L + 3u) & ~3u; y.acc = y.rows + (size_t)no * y.Ls;
     return y;
 }
@@ -379,6 +407,7 @@ __global__ void __launch_bounds__(128) k_prep(C c, int s) {
         unpack_lead(c, cd.lead_off + c.plan_best[ci], best, threadIdx.x, blockDim.x);
         const uint32_t no = c.plan_nother[ci];
         if (no == 0 || L == 0) { __syncthreads(); uint8_t* out = c.alt + c.alt_off[ci]; for (uint32_t h = threadIdx.x; h < L; h += blockDim.x) out[h] = (uint8_t)CODE[best[h]]; continue; }
+        pack_lead(c, cd.lead_off + c.plan_best[ci], L, reinterpret_cast<uint32_t*>(best + ((L + 7u) & ~7u)), threadIdx.x, blockDim.x, false);
         for (int i = threadIdx.x; i < TAB; i += blockDim.x) { tk[i] = 0xffffffffu; tp[i] = -1; }
         __syncthreads();
         const long skip = c.cfg.consensus_kmer_skip_base + (long)__dmul_rn((double)L, c.cfg.consensus_kmer_skip_seqlen_mult);
@@ -400,19 +429,20 @@ __device__ __forceinline__ void align_item(const C& c, const C::Item it, const G
     uint32_t* t_key; int* t_pos; cand_table(c, ci, &t_key, &t_pos);
     const uint32_t no = c.plan_nother[ci];
     const Layout y = cand_layout(c, ci, L, no);
-    uint8_t* best = y.best; uint8_t* acc = y.acc;
+    uint8_t* acc = y.acc; const Nib best = Nib::at(y.best4, 0);
     const snfb_lead* l = &c.cand_leads[cd->lead_off + it.k];
-    const long Lo = l->seq_len; uint8_t* rd = y.oth + it.rd_off; uint8_t* row = y.rows + (size_t)it.row * y.Ls;
+    const long Lo = l->seq_len; uint8_t* row = y.rows + (size_t)it.row * y.Ls;
     const long skip = c.cfg.consensus_kmer_skip_base + (long)__dmul_rn((double)L, c.cfg.consensus_kmer_skip_seqlen_mult);
-    unpack_lead(c, cd->lead_off + it.k, rd, tid, NT);
-    g.sync();
+    // the read in 4-bit form: from the seq arena, or, merged from several pieces, from the one packed copy it gets here first
+    const Nib rd = lead_reader(c, cd->lead_off + it.k, y.oth + it.rd_off);
+    if (c.out_pn[cd->lead_off + it.k] != 1) { pack_lead(c, cd->lead_off + it.k, Lo, reinterpret_cast<uint32_t*>(y.oth + it.rd_off), tid, NT, true); g.sync(); }
     // (1) anchor hits in j order (table lives in global scratch, L2 resident); four k-mers per thread in flight
     int nh = 0;
     const long nk = Lo - klen > 0 ? (Lo - klen + skip - 1) / skip : 0;
     for (long kb = 0; kb < nk; kb += 4 * NT) {
         uint32_t key[4], sl[4], tk[4]; int ai[4];
         #pragma unroll
-        for (int u = 0; u < 4; ++u) { const long kk = kb + u * NT + tid; key[u] = kk < nk ? kmer6_u(rd + kk * skip) : 0u; sl[u] = kslot(key[u]); }
+        for (int u = 0; u < 4; ++u) { const long kk = kb + u * NT + tid; key[u] = kk < nk ? kmer6_n(rd, (int)(kk * skip)) : 0u; sl[u] = kslot(key[u]); }
         #pragma unroll
         for (int u = 0; u < 4; ++u) tk[u] = kb + u * NT + tid < nk ? t_key[sl[u]] : 0xffffffffu;
         #pragma unroll
@@ -448,7 +478,7 @@ __device__ __forceinline__ void align_item(const C& c, const C::Item it, const G
     const long j0 = na ? hj[0] : 0, c0 = (na && j0 > 0) ? hi[0] : 0;
     // (3a) agreement with the best read along the diagonal decides copy / dash; a copied segment also gets its column identity
     //      (the bases it shares with the best read at the columns it lands on)
-    long span = skip > 12 ? segments_pass<8>(hi, hj, hcl, na, c0, j0, (long)L, rd, best, tid, NT) : segments_pass<1>(hi, hj, hcl, na, c0, j0, (long)L, rd, best, tid, NT);
+    long span = skip > 12 ? segments_pass<4>(hi, hj, hcl, na, c0, j0, (long)L, rd, best, tid, NT) : segments_pass<1>(hi, hj, hcl, na, c0, j0, (long)L, rd, best, tid, NT);
     span = g.sum(span);
     g.sync();
     // (3b) dash-free runs (= chains of copied segments) survive only with identity > 0.5 and more than 5 matches
@@ -476,20 +506,21 @@ __device__ __forceinline__ void align_item(const C& c, const C::Item it, const G
         g.sync();
     }
     // (3c) the row: every copied segment lands at row[cs + t] = rd[lj + t] with cs - lj = c0 - j0 for all of them, so the row is
-    //      one shifted copy of the read between the first and the last anchor (coalesced words), dashes outside, and the
-    //      rejected segments dashed afterwards
+    //      one shifted copy of the read between the first and the last anchor (eight bases unpacked per thread step, two words),
+    //      dashes outside, and the rejected segments dashed afterwards
     {
         long cl = 0; if (na) { cl = c0 + hj[na - 1] - j0; if (cl > (long)L) cl = (long)L; }
-        const uint8_t* src0 = rd + (j0 - c0);
-        #pragma unroll 4
-        for (long X = 4L * tid; X < (long)L; X += 4L * NT) {
-            uint32_t v = 0xffffffffu;
-            if (X + 4 > c0 && X < cl) {
-                v = load_u32_unaligned(src0 + X);
-                if (X < c0) v |= (1u << (8 * (c0 - X))) - 1u;                         // bytes before c0
-                if (X + 4 > cl) v |= ~((1u << (8 * (cl - X))) - 1u);                    // bytes from cl on
+        for (long X = 8L * tid; X < (long)L; X += 8L * NT) {
+            unsigned long long v = ~0ull;
+            if (X + 8 > c0 && X < cl) {
+                const int q = (int)(X + j0 - c0);                                        // below 0 only where X < c0
+                const uint32_t x = q >= 0 && q + 8 <= (int)Lo ? rd.get8(q, 8) : rd.take(q, 8, (int)Lo);
+                v = (unsigned long long)spread4(x & 0xffffu) | ((unsigned long long)spread4(x >> 16) << 32);
+                if (X < c0) v |= (1ull << (8 * (c0 - X))) - 1ull;                         // bytes before c0
+                if (X + 8 > cl) v |= ~((1ull << (8 * (cl - X))) - 1ull);                    // bytes from cl on
             }
-            *reinterpret_cast<uint32_t*>(row + X) = v;
+            *reinterpret_cast<uint32_t*>(row + X) = (uint32_t)v;                           // rows are 4-byte aligned, align4(L) long
+            if (X + 4 < (long)L) *reinterpret_cast<uint32_t*>(row + X + 4) = (uint32_t)(v >> 32);
         }
         g.sync();
         for (int m = 1 + tid; m < na; m += NT) {
