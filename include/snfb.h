@@ -386,6 +386,39 @@ int         snfb_inflate_bgzf(snfb_ctx* ctx, const uint8_t* bgzf, uint64_t n_byt
  * NULL) = byte offset of member k in out.  The BGZF EOF marker is not appended.  Device buffers belong to the context and grow on
  * demand; n_in is limited to 65535 blocks (~4 GiB) per call.  Records a "deflate" timing mark (snfb_last_timings). */
 int         snfb_deflate_bgzf(snfb_ctx* ctx, const uint8_t* in, uint64_t n_in, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* coffset);
+
+/* The tables of a BAI (min_shift 14, depth 5) or CSI index of a coordinate-sorted BAM, built on the device with no index to start from
+ * (what `samtools index` computes; SAM spec §5).  The file streams through the device in windows of whole BGZF members of at most
+ * window_bytes inflated bytes (at least one member): each window is inflated and CRC-checked, its record starts found from the carried
+ * entry offset by pointer jumping over the offsets that pass a strict record test, one row per record computed (reference, begin,
+ * bam_endpos, virtual offsets, mapped) and the sort order checked.  The tables are then built from all rows: bins by reg2bin, chunks as runs
+ * of the same (reference, bin), htslib's finishing rules (a bin spanning < 0x10000 compressed bytes moves its chunks to an existing parent,
+ * level by level from the leaves; chunks starting in the block where the previous one ends merge), the linear index at min_shift (an
+ * empty window takes the next window's offset, as htslib's update_loff fills it) and the per-bin loffset, the per-reference pseudo-bin.  Fails (snfb_last_error names the record or the block) on a file that is not BGZF,
+ * a block that fails to inflate or its CRC-32, a broken record chain, a truncated file, unsorted records, or (BAI) an end beyond 2^29. */
+typedef struct snfb_index_input {
+    const char* path;             /* the BAM file                                                                 */
+    uint64_t first_record;        /* virtual offset of the first record (the end of the header)                  */
+    const int64_t* contig_len;    /* n_ref contig lengths from the header                                        */
+    uint32_t n_ref;
+    int32_t min_shift, depth;     /* bin geometry: 14 / 5 for a BAI                                               */
+    int32_t _pad;
+    uint64_t window_bytes;        /* inflated bytes per window                                                   */
+} snfb_index_input;
+typedef struct snfb_index_view {  /* library-owned, valid until the next snfb_index_bam on the context           */
+    const uint64_t* ref;          /* [n_ref][5]: first v0 (~0: no record), last v1, mapped, unmapped, linear-index windows */
+    const uint64_t* lin_off;      /* [n_ref + 1]: reference t's linear index is lin[lin_off[t] .. lin_off[t + 1])  */
+    const uint64_t* lin;
+    const uint64_t* bin_key;      /* [n_bin] ascending: reference * n_bins + bin, n_bins = ((1 << 3 (depth + 1)) - 1) / 7; every bin
+                                   * that held records, so one whose chunks moved to its parent has none */
+    const uint64_t* bin_loff;     /* [n_bin] CSI loffset of the bin                                               */
+    const uint32_t* chunk_bin;    /* [n_chunk] index into bin_key; chunks grouped by bin, ascending offsets inside one */
+    const uint64_t* chunk_beg;
+    const uint64_t* chunk_end;
+    uint64_t n_bin, n_chunk, n_no_coor, n_records, n_windows, device_bytes;   /* device_bytes: device buffers held at the widest point */
+    double device_ms;             /* the device's time in the call (CUDA events around each phase of work it was given)        */
+} snfb_index_view;
+int         snfb_index_bam(snfb_ctx* ctx, const snfb_index_input* in, snfb_index_view* out);
 /* device-time accounting of the last run: per-kernel milliseconds from CUDA events on
  * the ctx stream; names[i] is a static string.  Returns the number of entries. */
 int         snfb_last_timings(snfb_ctx* ctx, const char** names, float* ms, uint64_t* bytes, int cap);

@@ -194,6 +194,16 @@ class GtOut(C.Structure):                                       # snfb_gt_out
     _fields_ = [("match", C.c_void_p), ("cov_start", C.c_void_p), ("cov_center", C.c_void_p), ("cov_end", C.c_void_p), ("bnd_no_prev", C.c_void_p)]
 
 
+class IndexInput(C.Structure):                                  # snfb_index_input
+    _fields_ = [("path", C.c_char_p), ("first_record", C.c_uint64), ("contig_len", C.c_void_p), ("n_ref", C.c_uint32),
+                ("min_shift", C.c_int32), ("depth", C.c_int32), ("_pad", C.c_int32), ("window_bytes", C.c_uint64)]
+
+
+class IndexView(C.Structure):                                   # snfb_index_view
+    _fields_ = [(n, C.c_void_p) for n in ("ref", "lin_off", "lin", "bin_key", "bin_loff", "chunk_bin", "chunk_beg", "chunk_end")] + \
+               [(n, C.c_uint64) for n in ("n_bin", "n_chunk", "n_no_coor", "n_records", "n_windows", "device_bytes")] + [("device_ms", C.c_double)]
+
+
 class RnamesView(C.Structure):                                  # snfb_rnames_view
     _fields_ = [("n_names", C.c_uint64), ("n_text", C.c_uint64), ("text", C.c_void_p), ("off", C.c_void_p), ("collisions", C.c_uint64)]
 

@@ -179,28 +179,44 @@ def reg2bin(beg, end):
     return 0
 
 
+def read_header(bgzf):
+    """the BAM header through a BgzfReader -> ([(contig name, length)], virtual offset of the first record)"""
+    head, v = bgzf.read_from(0, 12)
+    if head[:4] != b"BAM\1":
+        raise ValueError("not a BAM file")
+    l_text = struct.unpack("<i", head[4:8])[0]
+    data, v = bgzf.read_from(0, 12 + l_text)
+    if len(data) < 12 + l_text:
+        raise ValueError("truncated BAM header")
+    n_ref = struct.unpack("<i", data[8 + l_text:12 + l_text])[0]
+    contigs = []
+    for _ in range(n_ref):
+        d, v = bgzf.read_from(v, 4)
+        if len(d) < 4:
+            raise ValueError("truncated BAM header")
+        l_name = struct.unpack("<i", d)[0]
+        d, v = bgzf.read_from(v, l_name + 4)
+        if len(d) < l_name + 4:
+            raise ValueError("truncated BAM header")
+        contigs.append((d[:l_name - 1].decode(), struct.unpack("<i", d[l_name:l_name + 4])[0]))
+    return contigs, v
+
+
+def find_index(path):
+    """the index BamFile opens for `path` when none is named: path.bai, path.csi or the .bai beside a .bam, the first that exists; None"""
+    return next((p for p in (path + ".bai", path + ".csi", path[:-4] + ".bai" if path.endswith(".bam") else path + ".bai") if os.path.exists(p)), None)
+
+
 class BamFile:
     """`fetch(contig, start, end)` over an indexed BAM; yields decoded records in file (coordinate) order"""
 
     def __init__(self, path, index_path=None):
         self.path = path
         self.bgzf = BgzfReader(path)
-        head, v = self.bgzf.read_from(0, 12)
-        if head[:4] != b"BAM\1":
-            raise ValueError("not a BAM file")
-        l_text = struct.unpack("<i", head[4:8])[0]
-        data, v = self.bgzf.read_from(0, 12 + l_text)
-        n_ref = struct.unpack("<i", data[8 + l_text:12 + l_text])[0]
-        self.contigs = []
-        for _ in range(n_ref):
-            d, v = self.bgzf.read_from(v, 4)
-            l_name = struct.unpack("<i", d)[0]
-            d, v = self.bgzf.read_from(v, l_name + 4)
-            self.contigs.append((d[:l_name - 1].decode(), struct.unpack("<i", d[l_name:l_name + 4])[0]))
-        self.first_record = v
+        self.contigs, self.first_record = read_header(self.bgzf)
         self.name_to_id = {n: i for i, (n, _) in enumerate(self.contigs)}
         if index_path is None:
-            index_path = next((p for p in (path + ".bai", path + ".csi", path[:-4] + ".bai" if path.endswith(".bam") else path + ".bai") if os.path.exists(p)), path + ".bai")
+            index_path = find_index(path) or path + ".bai"
         self.min_shift, self.depth = 14, 5
         self.index = self._load_csi(index_path) if index_path.endswith(".csi") else self._load_bai(index_path)
         self.meta_bin = ((1 << ((self.depth + 1) * 3)) - 1) // 7 + 1          # 37450 for the BAI layout
@@ -525,6 +541,95 @@ def tabix_index(text: bytes, coffsets) -> bytes:
     out = [b"TBI\1", struct.pack("<8i", len(names), 2, 1, 2, 0, ord("#"), 0, len(nm)), nm]   # n_ref, VCF preset: format, col_seq/beg/end, meta, skip
     out += [_bai_ref_bytes(*t) for t in bin_index(placed, len(names))]
     return b"".join(out)
+
+
+# ------------------------------------------------------------------------------------------------ building an index (sniffles_b200.index)
+# device memory per inflated byte of a window (the window's inflated and compressed bytes, the candidate masks and the chain's nodes) and
+# the share of the free memory a window may plan on
+INDEX_DEVICE_BYTES_PER_INFLATED_BYTE = 4
+INDEX_FREE_MEMORY_SHARE = 0.8
+
+
+def csi_depth(contigs, min_shift):
+    """htslib's CSI depth for a BAM (bam_index): the fewest levels whose top bin covers the longest contig + 256"""
+    max_len, depth, s = max((ln for _, ln in contigs), default=0) + 256, 0, 1 << min_shift
+    while max_len > s:
+        depth += 1
+        s <<= 3
+    return depth
+
+
+def index_window_bytes(device=0):
+    """the inflated bytes of one window of build_index: the device's free memory share over INDEX_DEVICE_BYTES_PER_INFLATED_BYTE"""
+    import torch
+    free, _ = torch.cuda.mem_get_info(device)
+    return max(1 << 20, int(free * INDEX_FREE_MEMORY_SHARE / INDEX_DEVICE_BYTES_PER_INFLATED_BYTE))
+
+
+def index_bytes(tab, n_ref, fmt, min_shift, depth) -> bytes:
+    """the uncompressed index file of tables `tab` (the dict of binding.Context.index_bam): BAI (SAM spec §5.2) or the CSI body (§5.3).
+    Bins are written in ascending order, each reference's pseudo-bin last; htslib writes them in its hash table's order, so two indexes
+    compare as tables, not as bytes."""
+    n_bins = ((1 << (3 * (depth + 1))) - 1) // 7
+    meta = n_bins + 1
+    keys = np.asarray(tab["bin_key"], dtype=np.uint64)
+    ref_of = keys // np.uint64(n_bins)
+    bin_of = keys % np.uint64(n_bins)
+    cb = np.asarray(tab["chunk_bin"], dtype=np.int64)
+    starts = np.searchsorted(cb, np.arange(len(keys) + 1))            # chunks are grouped by bin, in bin order
+    live = np.diff(starts) > 0                                        # a bin that moved its chunks to its parent is not written
+    out = [b"BAI\1" + struct.pack("<i", n_ref)] if fmt == "bai" else [b"CSI\1" + struct.pack("<iiii", min_shift, depth, 0, n_ref)]
+    first = np.searchsorted(ref_of, np.arange(n_ref + 1, dtype=np.uint64))
+    for t in range(n_ref):
+        st = tab["ref"][t]
+        has = int(st[0]) != 0xFFFFFFFFFFFFFFFF
+        out.append(struct.pack("<i", int(live[first[t]:first[t + 1]].sum()) + has))
+        for b in range(int(first[t]), int(first[t + 1])):
+            c0, c1 = int(starts[b]), int(starts[b + 1])
+            if c0 == c1:
+                continue
+            head = struct.pack("<Ii", int(bin_of[b]), c1 - c0) if fmt == "bai" else struct.pack("<IQi", int(bin_of[b]), int(tab["bin_loff"][b]), c1 - c0)
+            pairs = np.empty((c1 - c0, 2), "<u8")
+            pairs[:, 0], pairs[:, 1] = tab["chunk_beg"][c0:c1], tab["chunk_end"][c0:c1]
+            out.append(head + pairs.tobytes())
+        if has:
+            head = struct.pack("<Ii", meta, 2) if fmt == "bai" else struct.pack("<IQi", meta, 0, 2)
+            out.append(head + struct.pack("<QQQQ", int(st[0]), int(st[1]), int(st[2]), int(st[3])))
+        if fmt == "bai":
+            lo, hi = int(tab["lin_off"][t]), int(tab["lin_off"][t + 1])
+            out.append(struct.pack("<i", hi - lo) + np.asarray(tab["lin"][lo:hi], "<u8").tobytes())
+    out.append(struct.pack("<Q", int(tab["n_no_coor"])))
+    return b"".join(out)
+
+
+def build_index(path, fmt="bai", min_shift=14, device=0, window_bytes=None, ctx=None, stats=None) -> bytes:
+    """The .bai / .csi file of the coordinate-sorted BAM at `path`, as `samtools index [-c [-m min_shift]]` builds it: the record
+    boundaries, rows and tables on the GPU (snfb_index_bam), the file streamed through the device in windows of `window_bytes` inflated
+    bytes (default: index_window_bytes); the host only serializes the tables, and a CSI is BGZF-compressed on the GPU.  Raises
+    ValueError for a file that is not a BAM, binding.SnfbError (naming the record or the block) for one the device refuses.  stats: a dict
+    that receives n_records, n_windows, device_bytes and device_ms."""
+    from . import binding
+    if fmt not in ("bai", "csi"):
+        raise ValueError(f"unknown index format {fmt!r}")
+    reader = BgzfReader(path)
+    try:
+        contigs, first = read_header(reader)
+    finally:
+        reader.close()
+    min_shift, depth = (14, 5) if fmt == "bai" else (int(min_shift), csi_depth(contigs, int(min_shift)))
+    own = ctx is None
+    ctx = ctx or binding.Context(device)
+    try:
+        tab = ctx.index_bam(path, first, [ln for _, ln in contigs], min_shift, depth, window_bytes or index_window_bytes(device))
+        body = index_bytes(tab, len(contigs), fmt, min_shift, depth)
+        if fmt == "csi":
+            body = ctx.deflate_bgzf(body)[0] + _BGZF_EOF
+    finally:
+        if own:
+            ctx.close()
+    if stats is not None:
+        stats.update((k, tab[k]) for k in ("n_records", "n_windows", "device_bytes", "device_ms"))
+    return body
 
 
 # ------------------------------------------------------------------------------------------------ writer (tests / benchmark inputs)

@@ -19,7 +19,8 @@ EXPORTS = ["snfb_version", "snfb_sizeof", "snfb_hash_name", "snfb_ctx_create", "
            "snfb_nccl_unique_id", "snfb_comm_init", "snfb_allgather_candidates", "snfb_selftest_sqrt_frac", "snfb_poa", "snfb_combine_groups", "snfb_combine_plan", "snfb_selftest_edit_distance",
            "snfb_load_bam", "snfb_set_regions", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf", "snfb_deflate_bgzf",
            "snfb_genotype_targets", "snfb_load_reference", "snfb_reference_runs", "snfb_fetch_reference",
-           "snfb_population_load", "snfb_population_match", "snfb_read_names", "snfb_set_consensus_slices"]
+           "snfb_population_load", "snfb_population_match", "snfb_read_names", "snfb_set_consensus_slices",
+           "snfb_index_bam"]
 
 
 def lib():
@@ -67,6 +68,7 @@ def lib():
         L.snfb_poa.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
         L.snfb_genotype_targets.argtypes = [C.c_void_p, C.POINTER(abi.GtIn), C.POINTER(abi.GtOut)]
         L.snfb_read_names.argtypes = [C.c_void_p, C.POINTER(abi.RnamesView)]
+        L.snfb_index_bam.argtypes = [C.c_void_p, C.POINTER(abi.IndexInput), C.POINTER(abi.IndexView)]
         L.snfb_load_reference.argtypes = [C.c_void_p, C.POINTER(abi.RefInput)]
         L.snfb_reference_runs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
         L.snfb_fetch_reference.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
@@ -326,6 +328,26 @@ class Context:
         self._check(self._lib.snfb_read_names(self._h, C.byref(v)), "snfb_read_names")
         return ReadNames(abi.view(v.text, "u1", v.n_text).copy(), abi.view(v.off, "<u4", v.n_names + 1).copy() if v.n_names else np.zeros(1, "<u4"),
                          int(v.collisions))
+
+    def index_bam(self, path, first_record, contig_lengths, min_shift, depth, window_bytes):
+        """The tables of a BAI / CSI index of the coordinate-sorted BAM at `path`, built on the device (snfb_index_bam).  first_record: the
+        virtual offset after the header; contig_lengths: the header's; window_bytes: inflated bytes per window.  Returns a dict of numpy
+        copies: ref [n_ref, 5] (first v0, last v1, mapped, unmapped, linear windows), lin_off, lin, bin_key (reference * n_bins + bin), bin_loff,
+        chunk_bin, chunk_beg, chunk_end, and n_no_coor, n_records, n_windows, device_bytes, device_ms."""
+        clen = np.ascontiguousarray(contig_lengths, dtype="<i8")
+        I, V = abi.IndexInput(), abi.IndexView()
+        I.path, I.first_record, I.contig_len, I.n_ref = os.fsencode(path), int(first_record), clen.ctypes.data, len(clen)
+        I.min_shift, I.depth, I.window_bytes = int(min_shift), int(depth), int(window_bytes)
+        self._check(self._lib.snfb_index_bam(self._h, C.byref(I), C.byref(V)), "snfb_index_bam")
+        n_ref = len(clen)
+        lin_off = abi.view(V.lin_off, "<u8", n_ref + 1).copy()
+        out = dict(ref=abi.view(V.ref, "<u8", 5 * n_ref).reshape(n_ref, 5).copy() if n_ref else np.zeros((0, 5), "<u8"), lin_off=lin_off,
+                   lin=abi.view(V.lin, "<u8", int(lin_off[-1])).copy(), bin_key=abi.view(V.bin_key, "<u8", V.n_bin).copy(),
+                   bin_loff=abi.view(V.bin_loff, "<u8", V.n_bin).copy(), chunk_bin=abi.view(V.chunk_bin, "<u4", V.n_chunk).copy(),
+                   chunk_beg=abi.view(V.chunk_beg, "<u8", V.n_chunk).copy(), chunk_end=abi.view(V.chunk_end, "<u8", V.n_chunk).copy())
+        out.update(n_no_coor=int(V.n_no_coor), n_records=int(V.n_records), n_windows=int(V.n_windows), device_bytes=int(V.device_bytes),
+                   device_ms=float(V.device_ms))
+        return out
 
     def load_reference(self, data, contigs, is_bgzf=False):
         """Reference FASTA -> the unwrapped genome resident on this context, and its 'N' runs (snfb_load_reference).  data: the file's bytes

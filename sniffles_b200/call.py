@@ -47,6 +47,14 @@ def total_mapped(bam):
     return sum(bam.count_mapped(name) or 0 for name, _ in bam.contigs)
 
 
+def open_indexed(path):
+    """bamio.BamFile over `path` and its index; CallSampleError with the reference's message (sniffles:171-178) when there is no index"""
+    if bamio.find_index(path) is None:
+        raise CallSampleError(f"Unable to load index for input file '{path}'. Please verify that your input file is sorted + indexed and that the "
+                              f"index .bai file is valid and in the right location. Build one on the GPU with: python -m sniffles_b200.index {path}")
+    return bamio.BamFile(path)
+
+
 def check_outputs(config):
     """the reference's checks before it opens any output (sniffles:122-127, 238-248, 265-267)"""
     if config.vcf is None and config.snf is None:
@@ -179,7 +187,7 @@ def plan_sample(config):
     config.contig_lengths and config.sample_ids_vcf, plan the tasks and load the tandem repeats with the reference's fatal check.
     Returns (bam, processed contigs [(name, length)], planned tasks [(task id, name, start, end)], {contig: tandem repeats})."""
     path = config.input[0] if isinstance(config.input, (list, tuple)) else config.input
-    bam = bamio.BamFile(path)
+    bam = open_indexed(path)
     config.task_read_id_offset_mult = read_id_offset_mult(total_mapped(bam))
     contig_lengths, planned = tasks.plan(bam.contigs, config)
     config.contig_lengths = contig_lengths

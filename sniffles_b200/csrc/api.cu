@@ -30,6 +30,7 @@
 #include "genotype.cuh"
 #include "rnames.cuh"
 #include "reference.cuh"
+#include "bam_index.cuh"
 
 // one owning allocation of device memory, or of pinned host memory when Pinned; freed by the destructor
 template <bool Pinned> struct Buf {
@@ -113,6 +114,9 @@ struct snfb_ctx {
     DevBuf b_pop, b_popq; population::P pop{}; bool have_pop = false;
     DevBuf b_ref, b_ref_work; std::vector<refseq::Contig> ref_ctg; bool have_ref = false;     // the unwrapped reference genome; tables / counters / N-run scratch
     HostBuf h_ref_runs, h_ref_coff, h_ref_out; uint64_t ref_n_runs = 0;                       // N runs and per-contig offsets; gather staging
+    // BAM index (snfb_index_bam): per-window candidate masks, chain nodes, the carried record; all rows; the table work; the tables on the host
+    DevBuf b_ix_mask, b_ix_node, b_ix_carry, b_ix_rows, b_ix_tab;
+    std::vector<uint64_t> ix_ref, ix_lin_off, ix_lin, ix_bin_key, ix_bin_loff, ix_chunk_u, ix_chunk_v; std::vector<uint32_t> ix_chunk_bin;
     std::vector<snfb_task> tasks;
     // region table (snfb_set_regions): host copy, device copy followed by each task's last region index; cov_view: some task's regions
     // are not increasing and disjoint, so stage A builds the coordinate-ordered (pos, end, flags) the coverage readers search
@@ -1850,3 +1854,325 @@ int snfb_fetch_reference(snfb_ctx* ctx, const snfb_ref_query* q, uint64_t n, uin
 }
 
 }  // extern "C"
+
+// ------------------------------------------------------------------------------------------------ BAM index (bam_index.cuh)
+namespace {
+// one window's members on the host: global inflated end and file offset of each, the inflated start of the first, the file offset after the last
+struct IxWin { uint64_t first_beg = 0, coff_end = 0; std::vector<uint64_t> end, coff; };
+uint64_t ix_voff(const IxWin& w, uint64_t u) {
+    const size_t j = (size_t)(std::lower_bound(w.end.begin(), w.end.end(), u) - w.end.begin());
+    if (j < w.end.size() && w.end[j] > u) return w.coff[j] << 16 | (u - (j ? w.end[j - 1] : w.first_beg));
+    return (j + 1 < w.end.size() ? w.coff[j + 1] : w.coff_end) << 16;
+}
+std::string voff_str(uint64_t v) { return std::to_string(v >> 16) + ":" + std::to_string(v & 0xffff); }
+// the BGZF member at z[o..n): 0 and its total size / ISIZE; 1 when z ends inside it; 2 when it is not a BGZF member (SAM spec §4.1)
+int ix_member(const uint8_t* z, uint64_t n, uint64_t o, uint32_t* bsize, uint32_t* isize) {
+    if (o + 18 > n) return 1;
+    if (z[o] != 0x1f || z[o + 1] != 0x8b || z[o + 2] != 8 || !(z[o + 3] & 4)) return 2;
+    const uint32_t xlen = z[o + 10] | (z[o + 11] << 8);
+    if (o + 12 + xlen > n) return 1;
+    uint32_t bs = 0;
+    for (uint64_t e = o + 12; e + 4 <= o + 12 + xlen; e += 4 + (z[e + 2] | (z[e + 3] << 8)))
+        if (z[e] == 66 && z[e + 1] == 67 && (z[e + 2] | (z[e + 3] << 8)) == 2 && e + 6 <= o + 12 + xlen) bs = (z[e + 4] | (z[e + 5] << 8)) + 1u;
+    if (!bs || bs < 12 + xlen + 8) return 2;
+    if (o + bs > n) return 1;
+    memcpy(isize, z + o + bs - 4, 4); *bsize = bs;
+    return *isize > 65536u ? 2 : 0;
+}
+}  // namespace
+
+// the name of the record at R[p] of the window on the device
+static std::string ix_name(const uint8_t* d_raw, uint64_t p) {
+    uint8_t h[36 + 256] = {0};
+    if (cudaMemcpy(h, d_raw + p, sizeof(h), cudaMemcpyDeviceToHost) != cudaSuccess) return "?";
+    const uint32_t l = h[12];
+    return std::string(reinterpret_cast<const char*>(h + 36), l ? strnlen(reinterpret_cast<const char*>(h + 36), l) : 0);
+}
+
+extern "C" int snfb_index_bam(snfb_ctx* ctx, const snfb_index_input* in, snfb_index_view* out) {
+    using bamidx::Row;
+    if (!ctx || !in || !out || !in->path || (in->n_ref && !in->contig_len)) return ctx ? fail(ctx, "snfb_index_bam: null argument") : 1;
+    if (in->min_shift < 1 || in->depth < 1 || in->min_shift + 3 * in->depth > 40) return fail(ctx, "snfb_index_bam: min_shift + 3 * depth must be in 4..40");
+    cudaSetDevice(ctx->device);
+    ctx->n_ev = 0;
+    const uint64_t win = std::min<uint64_t>(std::max<uint64_t>(in->window_bytes, 1), 1ull << 31);
+    const bamidx::Geo geo{ in->min_shift, in->depth };
+    const uint32_t n_bins = (uint32_t)(((1ull << (3 * (in->depth + 1))) - 1) / 7);
+    const long long max_end = 1ll << (in->min_shift + 3 * in->depth);
+    const int n_ref = (int)in->n_ref;
+    cudaStream_t st = ctx->st;
+    // device time: events around each phase of work the host hands the stream; the host's file reading between phases is not counted
+    struct PhaseTimer { cudaEvent_t a = nullptr, b = nullptr; double ms = 0; PhaseTimer() { cudaEventCreate(&a); cudaEventCreate(&b); } ~PhaseTimer() { cudaEventDestroy(a); cudaEventDestroy(b); } } tm;
+    auto t_begin = [&]() { cudaEventRecord(tm.a, st); };
+    auto t_end = [&]() { cudaEventRecord(tm.b, st); cudaEventSynchronize(tm.b); float x = 0; cudaEventElapsedTime(&x, tm.a, tm.b); tm.ms += x; };
+    long long* d_clen = nullptr;
+    if (carve(ctx->b_ix_tab, [&](Carver& c) { d_clen = c.take<long long>(n_ref + 1); })) return fail(ctx, "snfb_index_bam: out of device memory");
+    if (n_ref) CUDA_TRY(cudaMemcpyAsync(d_clen, in->contig_len, 8ull * n_ref, cudaMemcpyHostToDevice, st));
+    FILE* f = fopen(in->path, "rb");
+    if (!f) return fail(ctx, std::string("cannot open ") + in->path);
+    struct Closer { FILE* f; ~Closer() { fclose(f); } } closer{ f };
+
+    std::vector<uint8_t> hb; uint64_t hb_off = 0; bool eof = false;      // read-ahead: file bytes from hb_off
+    fseeko(f, 0, SEEK_END); const uint64_t file_size = (uint64_t)ftello(f); fseeko(f, 0, SEEK_SET);
+    auto fill = [&](uint64_t target) {                                     // at most the rest of the file, in reads of up to 64 MiB
+        target = std::min<uint64_t>(target, file_size - hb_off + 1);
+        while (!eof && hb.size() < target) {
+            const size_t old = hb.size(), want = (size_t)std::min<uint64_t>(std::max<uint64_t>(target - old, 1 << 20), 64ull << 20);
+            hb.resize(old + want);
+            const size_t got = fread(hb.data() + old, 1, want, f);
+            hb.resize(old + got);
+            if (got == 0) eof = true;
+        }
+    };
+    // the entry: global inflated offset of the next record, its virtual offset; the previous row's tid / beg for the order check
+    uint64_t G = 0, n_windows = 0;
+    uint64_t u_entry = 0, v_entry = in->first_record; bool entry_known = false;
+    int prev_tid = -2, prev_beg = 0;
+    uint64_t carry = 0;
+    std::vector<Row> rows;
+    for (;;) {
+        fill(std::max<uint64_t>(win, 1 << 17) + 65536 + 64);
+        if (hb.empty()) break;
+        uint64_t sel = 0, isum = 0; uint32_t nsel = 0;
+        for (;;) {
+            uint32_t bs = 0, isz = 0;
+            if (sel == hb.size()) break;
+            const int rc = ix_member(hb.data(), hb.size(), sel, &bs, &isz);
+            if (rc == 2) return fail(ctx, "not a BGZF block at file offset " + std::to_string(hb_off + sel) + ": not a BGZF-compressed BAM file");
+            if (rc == 1) {
+                if (eof) return fail(ctx, "truncated BGZF block at file offset " + std::to_string(hb_off + sel) + ": the file is truncated");
+                if (nsel) break;
+                fill(hb.size() + (1 << 17));
+                continue;
+            }
+            if (nsel && isum + isz > win) break;
+            sel += bs; isum += isz; ++nsel;
+        }
+        std::vector<ingest::BgzfBlock> blocks; std::vector<uint64_t> cstart; uint64_t raw_len = 0;
+        if (walk_bgzf(ctx, hb.data(), sel, blocks, cstart, &raw_len)) return 1;
+        IxWin W; W.first_beg = G; W.coff_end = hb_off + sel;
+        for (size_t k = 0; k < blocks.size(); ++k) { W.end.push_back(G + blocks[k].out_off + blocks[k].isize); W.coff.push_back(hb_off + cstart[k]); }
+        if (!entry_known) {                                                    // the header's end, as a global inflated offset
+            const uint64_t c = in->first_record >> 16, u = in->first_record & 0xffff;
+            auto it = std::find(W.coff.begin(), W.coff.end(), c);
+            if (it != W.coff.end()) { const size_t k = (size_t)(it - W.coff.begin()); u_entry = (k ? W.end[k - 1] : G) + u; entry_known = true; }
+        }
+        const uint64_t base = G - carry, L = carry + raw_len;
+        // inflate and CRC-check the window behind the carried bytes
+        if (ctx->b_comp.ensure(sel + 64) || ctx->b_raw.ensure(L + 64)) return fail(ctx, "snfb_index_bam: out of device memory for the window");
+        for (auto& b : blocks) b.out_off += carry;
+        uint8_t* R = ctx->b_raw.as<uint8_t>();
+        ingest::IngestCounters* d_ctr = nullptr; ingest::BgzfBlock* d_blk = nullptr;
+        if (carve(ctx->b_ing, [&](Carver& c) { d_ctr = c.take<ingest::IngestCounters>(1); d_blk = c.take<ingest::BgzfBlock>(blocks.size() + 1); }))
+            return fail(ctx, "snfb_index_bam: out of device memory (ingest tables)");
+        t_begin();
+        if (carry) CUDA_TRY(cudaMemcpyAsync(R, ctx->b_ix_carry.p, carry, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(ctx->b_comp.p, hb.data(), sel, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemsetAsync(ctx->b_comp.as<uint8_t>() + sel, 0, 64, st));
+        CUDA_TRY(cudaMemsetAsync(R + L, 0, 64, st));
+        CUDA_TRY(cudaMemsetAsync(d_ctr, 0, sizeof(ingest::IngestCounters), st));
+        CUDA_TRY(cudaMemcpyAsync(d_blk, blocks.data(), sizeof(ingest::BgzfBlock) * blocks.size(), cudaMemcpyHostToDevice, st));
+        launch_inflate(ctx, d_blk, (unsigned)blocks.size(), d_ctr);
+        ingest::IngestCounters hc;
+        CUDA_TRY(cudaMemcpyAsync(&hc, d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, st));
+        t_end();
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if (hc.bad_blocks) {
+            const unsigned long long first = ~hc.first_bad_inv, b = first >> 8, code = first & 255u;
+            return fail(ctx, "BGZF block at file offset " + std::to_string(hb_off + cstart[b]) + (code == ingest::INF_CRC_MISMATCH ? ": CRC32 mismatch" : ": failed to inflate (code " + std::to_string(code) + ")"));
+        }
+        hb.erase(hb.begin(), hb.begin() + (ptrdiff_t)sel); hb_off += sel;
+        G += raw_len; ++n_windows;
+        if (!entry_known || u_entry >= base + L) continue;                   // still inside the header
+        const uint64_t e = u_entry - base;
+        // candidates
+        const uint64_t n_words = (L + 31) / 32;
+        uint32_t *mask = nullptr, *cnt = nullptr, *wbase = nullptr, *stmp = nullptr; unsigned long long* misc = nullptr; unsigned long long *d_end = nullptr, *d_coff = nullptr;
+        if (carve(ctx->b_ix_mask, [&](Carver& c) { mask = c.take<uint32_t>(n_words); cnt = c.take<uint32_t>(n_words); wbase = c.take<uint32_t>(n_words); stmp = c.take<uint32_t>(prims::scan_tmp_elems(n_words) + 16);
+                                                   misc = c.take<unsigned long long>(8); d_end = c.take<unsigned long long>(W.end.size()); d_coff = c.take<unsigned long long>(W.coff.size()); }))
+            return fail(ctx, "snfb_index_bam: out of device memory (candidate masks)");
+        t_begin();
+        CUDA_TRY(cudaMemcpyAsync(d_end, W.end.data(), 8 * W.end.size(), cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_coff, W.coff.data(), 8 * W.coff.size(), cudaMemcpyHostToDevice, st));
+        mark(ctx, "index_candidates", L);
+        launch(ctx->launches, bamidx::k_mark, grid_for(n_words * 32, 256), 256, 0, st, (const uint8_t*)R, (unsigned long long)L, (unsigned long long)e, n_ref, (const long long*)d_clen, mask, cnt, (unsigned long long)n_words);
+        prims::exclusive_scan(ctx->launches, cnt, wbase, stmp, nullptr, n_words, &misc[0], st);
+        unsigned long long n_cand = 0;
+        CUDA_TRY(cudaMemcpyAsync(&n_cand, &misc[0], 8, cudaMemcpyDeviceToHost, st));
+        t_end();
+        CUDA_TRY(cudaStreamSynchronize(st));
+        const uint64_t v_e = e == 0 && carry ? v_entry : ix_voff(W, base + e);
+        if (n_cand == 0) return fail(ctx, "the record at virtual offset " + voff_str(v_e) + " is not a valid BAM record");
+        const uint32_t n = (uint32_t)n_cand, n2 = n + 2;
+        const int K = std::max(1, bits_for(n2));
+        uint32_t *cand = nullptr, *J = nullptr, *is_rec = nullptr, *rec_idx = nullptr, *roff = nullptr, *ntmp = nullptr; uint8_t* pmark = nullptr; unsigned long long* res = nullptr; Row* d_rows = nullptr;
+        if (carve(ctx->b_ix_node, [&](Carver& c) { cand = c.take<uint32_t>(n); J = c.take<uint32_t>((size_t)K * n2); pmark = c.take<uint8_t>(n2); is_rec = c.take<uint32_t>(n + 1); rec_idx = c.take<uint32_t>(n + 1);
+                                                   roff = c.take<uint32_t>(n + 1); ntmp = c.take<uint32_t>(prims::scan_tmp_elems(n) + 16); res = c.take<unsigned long long>(8); d_rows = c.take<Row>(n + 1); }))
+            return fail(ctx, "snfb_index_bam: out of device memory (" + std::to_string(n) + " candidate record starts)");
+        t_begin();
+        mark(ctx, "index_chain", 0);
+        launch(ctx->launches, bamidx::k_compact, grid_for(n_words * 32, 256), 256, 0, st, (const uint32_t*)mask, (const uint32_t*)wbase, (unsigned long long)n_words, cand);
+        launch(ctx->launches, bamidx::k_link, grid_for(n2, 256), 256, 0, st, (const uint8_t*)R, (unsigned long long)L, n_ref, (const long long*)d_clen, (const uint32_t*)cand, n, J);
+        for (int k = 0; k + 1 < K; ++k) launch(ctx->launches, bamidx::k_jump, grid_for(n2, 256), 256, 0, st, (const uint32_t*)(J + (size_t)k * n2), J + (size_t)(k + 1) * n2, n2);
+        CUDA_TRY(cudaMemsetAsync(pmark, 0, n2, st));
+        CUDA_TRY(cudaMemsetAsync(pmark, 1, 1, st));
+        for (int k = K - 1; k >= 0; --k) launch(ctx->launches, bamidx::k_mark_path, grid_for(n2, 256), 256, 0, st, (const uint32_t*)(J + (size_t)k * n2), n2, pmark);
+        CUDA_TRY(cudaMemsetAsync(res, 0xff, 16, st));
+        launch(ctx->launches, bamidx::k_path_records, grid_for(n, 256), 256, 0, st, (const uint8_t*)pmark, (const uint32_t*)J, n, is_rec, (const uint32_t*)cand, res);
+        prims::exclusive_scan(ctx->launches, is_rec, rec_idx, ntmp, nullptr, n, &res[2], st);
+        unsigned long long hres[3]; uint32_t cand0 = 0; uint8_t end_marked = 0;
+        CUDA_TRY(cudaMemcpyAsync(hres, res, 24, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(&cand0, cand, 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(&end_marked, pmark + n + bamidx::END_NODE, 1, cudaMemcpyDeviceToHost, st));
+        t_end();
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if (cand0 != e) return fail(ctx, "the record at virtual offset " + voff_str(v_e) + " is not a valid BAM record");
+        if (hres[1] != ~0ull) {
+            uint32_t p = 0; CUDA_TRY(cudaMemcpy(&p, cand + hres[1], 4, cudaMemcpyDeviceToHost));
+            uint32_t bs = 0; CUDA_TRY(cudaMemcpy(&bs, R + p, 4, cudaMemcpyDeviceToHost));
+            const uint64_t vp = p == 0 && carry ? v_entry : ix_voff(W, base + p);
+            return fail(ctx, "the record chain breaks after record '" + ix_name(R, p) + "' at virtual offset " + voff_str(vp) + ": the bytes at virtual offset "
+                             + voff_str(ix_voff(W, base + p + 4 + bs)) + " are not a BAM record (corrupt or not a BAM file)");
+        }
+        if (hres[0] == ~0ull && !end_marked) return fail(ctx, "snfb_index_bam: the record chain did not resolve");
+        const uint64_t n_rows = hres[2];
+        const uint64_t row_base = rows.size();
+        if (n_rows) {
+            t_begin();
+            mark(ctx, "index_rows", 0);
+            bamidx::Window DW{ base, W.first_beg, W.coff_end, d_end, d_coff, (unsigned)W.end.size() };
+            launch(ctx->launches, bamidx::k_rows, grid_for((uint64_t)n * 32, 256), 256, 0, st, (const uint8_t*)R, (const uint32_t*)cand, (const uint32_t*)is_rec, (const uint32_t*)rec_idx, n, DW, d_rows, roff);
+            CUDA_TRY(cudaMemsetAsync(&res[3], 0xff, 8, st));
+            launch(ctx->launches, bamidx::k_check, grid_for(n_rows, 256), 256, 0, st, d_rows, (uint32_t)n_rows, (unsigned long long)v_entry, prev_tid, prev_beg, max_end, (unsigned long long)row_base, &res[3]);
+            rows.resize(row_base + n_rows);
+            unsigned long long bad = 0;
+            CUDA_TRY(cudaMemcpyAsync(rows.data() + row_base, d_rows, sizeof(Row) * n_rows, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(&bad, &res[3], 8, cudaMemcpyDeviceToHost, st));
+            t_end();
+            CUDA_TRY(cudaStreamSynchronize(st));
+            if (bad != bamidx::BAD_NONE) {
+                const uint64_t r = bad & ((1ull << 56) - 1), i = r - row_base; const unsigned code = (unsigned)(bad >> 56);
+                uint32_t p = 0; CUDA_TRY(cudaMemcpy(&p, roff + i, 4, cudaMemcpyDeviceToHost));
+                const Row& x = rows[r];
+                const int pt = r ? rows[r - 1].tid : prev_tid, pb = r ? rows[r - 1].beg : prev_beg;
+                std::string why;
+                if (code == bamidx::BAD_ORDER) why = "unsorted positions on reference #" + std::to_string(x.tid) + ": " + std::to_string(x.beg + 1) + " after " + std::to_string(pb + 1);
+                else if (code == bamidx::BAD_TID_AFTER_UNPLACED) why = "a record on reference #" + std::to_string(x.tid) + " after the unplaced records (reference -1), which must come last";
+                else if (code == bamidx::BAD_TID_BACK) why = "reference #" + std::to_string(x.tid) + " after reference #" + std::to_string(pt) + ": the records are not sorted by coordinate";
+                else why = "end " + std::to_string(x.end) + " beyond the " + std::to_string(max_end) + " positions the index geometry covers (a BAI covers 2^29: use -c for a CSI index)";
+                return fail(ctx, "record '" + ix_name(R, p) + "' (record " + std::to_string(r + 1) + " of the file, virtual offset " + voff_str(x.v0) + "): " + why);
+            }
+            v_entry = rows.back().v1; prev_tid = rows.back().tid; prev_beg = rows.back().beg;
+        }
+        mark(ctx, nullptr);
+        if (hres[0] != ~0ull) {                        // the chain ends in a record the window cannot finish: carry it into the next one
+            const uint64_t o = hres[0];
+            carry = L - o;
+            if (ctx->b_ix_carry.ensure(carry + 64)) return fail(ctx, "snfb_index_bam: out of device memory (carried record)");
+            CUDA_TRY(cudaMemcpyAsync(ctx->b_ix_carry.p, R + o, carry, cudaMemcpyDeviceToDevice, st));
+            u_entry = base + o;
+        } else { carry = 0; u_entry = base + L; }
+    }
+    if (!entry_known && in->first_record == hb_off << 16) entry_known = true, u_entry = G;      // a header-only file without the EOF member
+    if (!entry_known || u_entry != G)
+        return fail(ctx, "truncated BAM file: the record at virtual offset " + voff_str(v_entry) + " extends past the end of the data (" + std::to_string(G) + " inflated bytes)");
+    CUDA_TRY(cudaStreamSynchronize(st));
+
+    // ---- tables over all rows
+    const uint64_t n_rec = rows.size();
+    uint64_t n_placed = 0;
+    while (n_placed < n_rec && rows[n_placed].tid >= 0) ++n_placed;
+    if (n_rec >= (1ull << 32)) return fail(ctx, "snfb_index_bam: more than 2^32 records");
+    ctx->ix_ref.assign(5ull * n_ref, 0);
+    for (int t = 0; t < n_ref; ++t) ctx->ix_ref[5ull * t] = ~0ull;
+    uint64_t* d_ref = nullptr; Row* d_all = nullptr;
+    if (ctx->b_ix_rows.ensure(sizeof(Row) * (n_placed + 1))) return fail(ctx, "snfb_index_bam: out of device memory (rows)");
+    d_all = ctx->b_ix_rows.as<Row>();
+    if (carve(ctx->b_ix_tab, [&](Carver& c) { d_clen = c.take<long long>(n_ref + 1); d_ref = c.take<uint64_t>(5ull * n_ref + 1); })) return fail(ctx, "snfb_index_bam: out of device memory");
+    t_begin();
+    mark(ctx, "index_tables", sizeof(Row) * n_placed);
+    if (n_placed) CUDA_TRY(cudaMemcpyAsync(d_all, rows.data(), sizeof(Row) * n_placed, cudaMemcpyHostToDevice, st));
+    if (n_ref) CUDA_TRY(cudaMemcpyAsync(d_ref, ctx->ix_ref.data(), 8 * ctx->ix_ref.size(), cudaMemcpyHostToDevice, st));
+    if (n_placed) launch(ctx->launches, bamidx::k_ref_stats, grid_for(n_placed, 256), 256, 0, st, (const Row*)d_all, (uint32_t)n_placed, geo, (unsigned long long*)d_ref);
+    if (n_ref) CUDA_TRY(cudaMemcpyAsync(ctx->ix_ref.data(), d_ref, 8 * ctx->ix_ref.size(), cudaMemcpyDeviceToHost, st));
+    t_end();
+    CUDA_TRY(cudaStreamSynchronize(st));
+    ctx->ix_lin_off.assign(n_ref + 1, 0);
+    for (int t = 0; t < n_ref; ++t) ctx->ix_lin_off[t + 1] = ctx->ix_lin_off[t] + ctx->ix_ref[5ull * t + 4];
+    const uint64_t n_lin = ctx->ix_lin_off[n_ref];
+    const uint64_t np = n_placed;
+    uint64_t *lin_off = nullptr, *lin = nullptr, *rkey = nullptr, *ckey = nullptr, *ckey2 = nullptr, *ukey = nullptr, *cu = nullptr, *cv = nullptr, *bmin = nullptr, *bmax = nullptr, *loff = nullptr, *mu = nullptr, *mv = nullptr, *cnts = nullptr;
+    uint32_t *head = nullptr, *cidx = nullptr, *cval = nullptr, *cval2 = nullptr, *h = nullptr, *hidx = nullptr, *cur = nullptr, *mbin = nullptr, *stmp = nullptr, *hist = nullptr; int *parent = nullptr, *level = nullptr;
+    const size_t hist_n = prims::radix_hist_elems(np + 1);
+    if (carve(ctx->b_ix_tab, [&](Carver& c) {
+            lin_off = c.take<uint64_t>(n_ref + 1); lin = c.take<uint64_t>(n_lin + 1); rkey = c.take<uint64_t>(np + 1);
+            head = c.take<uint32_t>(np + 1); cidx = c.take<uint32_t>(np + 1); cu = c.take<uint64_t>(np + 1); cv = c.take<uint64_t>(np + 1); ckey = c.take<uint64_t>(np + 1); ckey2 = c.take<uint64_t>(np + 1);
+            cval = c.take<uint32_t>(np + 1); cval2 = c.take<uint32_t>(np + 1); h = c.take<uint32_t>(np + 1); hidx = c.take<uint32_t>(np + 1); ukey = c.take<uint64_t>(np + 1); cur = c.take<uint32_t>(np + 1);
+            parent = c.take<int>(np + 1); level = c.take<int>(np + 1); loff = c.take<uint64_t>(np + 1); bmin = c.take<uint64_t>(np + 1); bmax = c.take<uint64_t>(np + 1);
+            mbin = c.take<uint32_t>(np + 1); mu = c.take<uint64_t>(np + 1); mv = c.take<uint64_t>(np + 1); cnts = c.take<uint64_t>(8);
+            hist = c.take<uint32_t>(hist_n); stmp = c.take<uint32_t>(prims::scan_tmp_elems(std::max<uint64_t>(hist_n, np + 1)) + 16); }))
+        return fail(ctx, "snfb_index_bam: out of device memory (tables)");
+    CUDA_TRY(cudaMemcpyAsync(lin_off, ctx->ix_lin_off.data(), 8 * (n_ref + 1), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemsetAsync(lin, 0xff, 8 * (n_lin + 1), st));
+    uint64_t h_n[3] = { 0, 0, 0 };            // chunks, unique bins, merged chunks
+    t_begin();
+    if (np) {
+        const int grid = grid_for(np, 256);
+        launch(ctx->launches, bamidx::k_chunks, grid, 256, 0, st, (const Row*)d_all, (uint32_t)np, geo, n_bins, head, rkey, (const unsigned long long*)lin_off, (unsigned long long*)lin);
+        prims::exclusive_scan(ctx->launches, head, cidx, stmp, nullptr, np, (unsigned long long*)&cnts[0], st);
+        launch(ctx->launches, bamidx::k_chunk_rows, grid, 256, 0, st, (const Row*)d_all, (const uint32_t*)head, (const uint32_t*)cidx, (const uint64_t*)rkey, (uint32_t)np,
+               (unsigned long long*)cu, (unsigned long long*)cv, ckey, cval);
+        CUDA_TRY(cudaMemcpyAsync(&h_n[0], &cnts[0], 8, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+    }
+    if (n_ref) launch(ctx->launches, bamidx::k_lin_fill, n_ref, 256, 0, st, (unsigned long long*)lin, (const unsigned long long*)lin_off, n_ref);
+    const uint32_t nc = (uint32_t)h_n[0];
+    if (nc) {
+        const int grid = grid_for(nc, 256);
+        bool in_first = true;
+        int key_bits = 1; while (key_bits < 64 && ((uint64_t)n_ref * n_bins) >> key_bits) ++key_bits;
+        prims::radix_sort(ctx->launches, ckey, cval, ckey2, cval2, prims::RadixTemp{ hist, stmp }, (const unsigned long long*)&cnts[0], nc, key_bits, &in_first, st);
+        const uint64_t* sk = in_first ? ckey : ckey2; const uint32_t* sv = in_first ? cval : cval2;
+        launch(ctx->launches, bamidx::k_key_heads, grid, 256, 0, st, sk, nc, h);
+        prims::exclusive_scan(ctx->launches, h, hidx, stmp, nullptr, nc, (unsigned long long*)&cnts[1], st);
+        launch(ctx->launches, bamidx::k_unique_bins, grid, 256, 0, st, sk, sv, (const uint32_t*)h, (const uint32_t*)hidx, nc, ukey, cur);
+        CUDA_TRY(cudaMemcpyAsync(&h_n[1], &cnts[1], 8, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        const uint32_t nub = (uint32_t)h_n[1];
+        launch(ctx->launches, bamidx::k_bin_info, grid_for(nub, 256), 256, 0, st, (const uint64_t*)ukey, nub, n_bins, geo, (const unsigned long long*)lin_off, (const unsigned long long*)lin, parent, level, (unsigned long long*)loff);
+        for (int l = in->depth; l >= 1; --l) {
+            CUDA_TRY(cudaMemsetAsync(bmin, 0xff, 8ull * nub, st));
+            CUDA_TRY(cudaMemsetAsync(bmax, 0, 8ull * nub, st));
+            launch(ctx->launches, bamidx::k_bin_span, grid, 256, 0, st, (const uint32_t*)cur, (const int*)level, (const unsigned long long*)cu, (const unsigned long long*)cv, nc, l, (unsigned long long*)bmin, (unsigned long long*)bmax);
+            launch(ctx->launches, bamidx::k_bin_lift, grid, 256, 0, st, cur, (const int*)level, (const int*)parent, nc, l, (const unsigned long long*)bmin, (const unsigned long long*)bmax);
+        }
+        launch(ctx->launches, bamidx::k_cur_keys, grid, 256, 0, st, (const uint32_t*)cur, nc, ckey, cval);
+        prims::radix_sort(ctx->launches, ckey, cval, ckey2, cval2, prims::RadixTemp{ hist, stmp }, (const unsigned long long*)&cnts[0], nc, std::max(1, bits_for(nub)), &in_first, st);
+        const uint64_t* sb = in_first ? ckey : ckey2; const uint32_t* sc = in_first ? cval : cval2;
+        launch(ctx->launches, bamidx::k_merge_heads, grid, 256, 0, st, sb, sc, (const unsigned long long*)cu, (const unsigned long long*)cv, nc, h);
+        prims::exclusive_scan(ctx->launches, h, hidx, stmp, nullptr, nc, (unsigned long long*)&cnts[2], st);
+        launch(ctx->launches, bamidx::k_merge_out, grid, 256, 0, st, sb, sc, (const unsigned long long*)cu, (const unsigned long long*)cv, (const uint32_t*)h, (const uint32_t*)hidx, nc, mbin,
+               (unsigned long long*)mu, (unsigned long long*)mv);
+        CUDA_TRY(cudaMemcpyAsync(&h_n[2], &cnts[2], 8, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+    }
+    mark(ctx, nullptr);
+    const uint64_t nub = h_n[1], nm = h_n[2];
+    ctx->ix_lin.resize(n_lin + 1); ctx->ix_bin_key.resize(nub + 1); ctx->ix_bin_loff.resize(nub + 1); ctx->ix_chunk_bin.resize(nm + 1); ctx->ix_chunk_u.resize(nm + 1); ctx->ix_chunk_v.resize(nm + 1);
+    if (n_lin) CUDA_TRY(cudaMemcpyAsync(ctx->ix_lin.data(), lin, 8 * n_lin, cudaMemcpyDeviceToHost, st));
+    if (nub) { CUDA_TRY(cudaMemcpyAsync(ctx->ix_bin_key.data(), ukey, 8 * nub, cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaMemcpyAsync(ctx->ix_bin_loff.data(), loff, 8 * nub, cudaMemcpyDeviceToHost, st)); }
+    if (nm) {
+        CUDA_TRY(cudaMemcpyAsync(ctx->ix_chunk_bin.data(), mbin, 4 * nm, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(ctx->ix_chunk_u.data(), mu, 8 * nm, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(ctx->ix_chunk_v.data(), mv, 8 * nm, cudaMemcpyDeviceToHost, st));
+    }
+    t_end();
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaGetLastError());
+    out->ref = ctx->ix_ref.data(); out->lin_off = ctx->ix_lin_off.data(); out->lin = ctx->ix_lin.data();
+    out->bin_key = ctx->ix_bin_key.data(); out->bin_loff = ctx->ix_bin_loff.data(); out->chunk_bin = ctx->ix_chunk_bin.data(); out->chunk_beg = ctx->ix_chunk_u.data(); out->chunk_end = ctx->ix_chunk_v.data();
+    out->n_bin = nub; out->n_chunk = nm; out->n_no_coor = n_rec - n_placed; out->n_records = n_rec; out->n_windows = n_windows;
+    out->device_ms = tm.ms;
+    out->device_bytes = ctx->b_comp.cap + ctx->b_raw.cap + ctx->b_ing.cap + ctx->b_ix_mask.cap + ctx->b_ix_node.cap + ctx->b_ix_carry.cap + ctx->b_ix_rows.cap + ctx->b_ix_tab.cap;
+    return 0;
+}

@@ -237,7 +237,7 @@ def genotype_vcf(config, device=0, budget=None, stats=None):
     st.update(passes=0, pass_inflated_bytes=[], load_bam_s=[], run_s=[], genotype_s=[], read_s=0.0, write_s=0.0, parse_s=time.perf_counter() - t0)
     t1 = time.perf_counter()
     path = config.input[0] if isinstance(config.input, (list, tuple)) else config.input
-    bam = bamio.BamFile(path)
+    bam = call.open_indexed(path)
     planned, targets_of = [], {}
     for tid, name, s, e, ts in plan(bam.contigs, targets, config):
         if not ts:                                      # a task without targets writes nothing
