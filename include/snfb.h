@@ -419,6 +419,47 @@ typedef struct snfb_index_view {  /* library-owned, valid until the next snfb_in
     double device_ms;             /* the device's time in the call (CUDA events around each phase of work it was given)        */
 } snfb_index_view;
 int         snfb_index_bam(snfb_ctx* ctx, const snfb_index_input* in, snfb_index_view* out);
+
+/* The BAM at `path` sorted by coordinate into out_path, as `samtools sort` writes it (samtools bam_sort.c: bam1_cmp_core for the order;
+ * htslib bam_hdr_write / bam_write1 -> bgzf_flush_try / bgzf_write, BGZF_BLOCK_SIZE 0xff00, for the member cuts).
+ *   Order: tid compared as unsigned (tid -1, no coordinate, last), then pos + 1, then the reverse-strand bit (flag 0x10), then input order.
+ *     The device key is (tid' << 33) | ((pos + 1) << 1) | rev with tid' = n_ref for tid -1; one stable radix sort over only the key's
+ *     bits, values = input ordinals.
+ *   Records are copied verbatim (bin, mate fields and tags are not recomputed).  The output header is the caller's `header` bytes (the
+ *     BAM header from the magic through the references; sniffles_b200.bamio.sort_header sets @HD SO:coordinate and changes nothing else).
+ *   Member cuts: the header fills members of 0xff00 bytes and is flushed; a record of 4 + block_size bytes first closes the current member
+ *     when that member is non-empty and the record would overflow it, then fills members of 0xff00 bytes, each closed when full; the last
+ *     partial member is closed and the 28-byte EOF marker appended.  The members are compressed by the device encoder (not zlib), so the
+ *     file is not byte-equal to samtools'; its inflated stream and member sizes are, and its bytes are a pure function of the input
+ *     whatever the budgets.
+ * Device pipeline: the keys pass streams the input in windows of whole members of at most window_bytes inflated bytes, exactly as
+ * snfb_index_bam does (inflate + CRC, carry, the record chain), and writes each record's key, length and inflated offset; the sort; the
+ * layout (one host loop over the sorted lengths cuts the members; buckets are runs of whole members starting at a record start, of at
+ * most bucket_bytes inflated bytes, or one record's members when it alone is larger); then per bucket the windows holding its records are
+ * read again, their records' bytes scattered into the bucket's buffer by a warp per record, the members compressed from device memory (at
+ * most 65535 per launch) and appended to the file.  Fails (snfb_last_error names the record or the block) on the inputs snfb_index_bam
+ * refuses except the order (a record whose tid < -1, tid >= n_ref or pos < -1 fails the strict record test and breaks the chain), on 2^32
+ * records or more, and when out_path cannot be written. */
+typedef struct snfb_sort_input {
+    const char* path;             /* the BAM file                                                                 */
+    const char* out_path;         /* the file written (created or truncated)                                     */
+    const uint8_t* header;        /* the output's BAM header: magic, l_text, text, n_ref, the references          */
+    uint64_t header_len;
+    uint64_t first_record;        /* virtual offset of the input's first record (the end of its header)          */
+    const int64_t* contig_len;    /* n_ref contig lengths from the header                                        */
+    uint32_t n_ref, _pad;
+    uint64_t window_bytes;        /* inflated bytes per input window                                             */
+    uint64_t bucket_bytes;        /* inflated output bytes per bucket                                            */
+} snfb_sort_input;
+typedef struct snfb_sort_view {
+    uint64_t n_records, n_windows, n_buckets, n_members;  /* n_windows: windows of the keys pass                  */
+    uint64_t n_input_reads;       /* window reads of the input: the keys pass's and those of every bucket pass     */
+    uint64_t bytes_in, bytes_out; /* file bytes read (both passes), file bytes written (with the EOF marker)      */
+    uint64_t device_bytes;        /* device buffers held at the widest point                                     */
+    double ms_keys, ms_sort, ms_layout, ms_scatter, ms_deflate;   /* device time per phase (CUDA events)          */
+    double ms_layout_host;        /* the host's member-cut loop over the sorted lengths                          */
+} snfb_sort_view;
+int         snfb_sort_bam(snfb_ctx* ctx, const snfb_sort_input* in, snfb_sort_view* out);
 /* device-time accounting of the last run: per-kernel milliseconds from CUDA events on
  * the ctx stream; names[i] is a static string.  Returns the number of entries. */
 int         snfb_last_timings(snfb_ctx* ctx, const char** names, float* ms, uint64_t* bytes, int cap);

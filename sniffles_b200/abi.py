@@ -204,6 +204,16 @@ class IndexView(C.Structure):                                   # snfb_index_vie
                [(n, C.c_uint64) for n in ("n_bin", "n_chunk", "n_no_coor", "n_records", "n_windows", "device_bytes")] + [("device_ms", C.c_double)]
 
 
+class SortInput(C.Structure):                                   # snfb_sort_input
+    _fields_ = [("path", C.c_char_p), ("out_path", C.c_char_p), ("header", C.c_void_p), ("header_len", C.c_uint64), ("first_record", C.c_uint64),
+                ("contig_len", C.c_void_p), ("n_ref", C.c_uint32), ("_pad", C.c_uint32), ("window_bytes", C.c_uint64), ("bucket_bytes", C.c_uint64)]
+
+
+class SortView(C.Structure):                                    # snfb_sort_view
+    _fields_ = [(n, C.c_uint64) for n in ("n_records", "n_windows", "n_buckets", "n_members", "n_input_reads", "bytes_in", "bytes_out", "device_bytes")] + \
+               [(n, C.c_double) for n in ("ms_keys", "ms_sort", "ms_layout", "ms_scatter", "ms_deflate", "ms_layout_host")]
+
+
 class RnamesView(C.Structure):                                  # snfb_rnames_view
     _fields_ = [("n_names", C.c_uint64), ("n_text", C.c_uint64), ("text", C.c_void_p), ("off", C.c_void_p), ("collisions", C.c_uint64)]
 

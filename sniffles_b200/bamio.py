@@ -632,6 +632,75 @@ def build_index(path, fmt="bai", min_shift=14, device=0, window_bytes=None, ctx=
     return body
 
 
+# ------------------------------------------------------------------------------------------------ sorting a BAM (sniffles_b200.sort)
+# device memory per inflated byte of the two budgets together: an input window takes INDEX_DEVICE_BYTES_PER_INFLATED_BYTE, an output bucket
+# three (its bytes, the encoder's member slots, the packed members); the rest is left for the per-record keys, lengths and offsets
+SORT_DEVICE_BYTES_PER_INFLATED_BYTE = 8
+
+
+def sort_budget_bytes(device=0):
+    """the default window_bytes and bucket_bytes of sort_bam: each the device's free memory share over SORT_DEVICE_BYTES_PER_INFLATED_BYTE"""
+    import torch
+    free, _ = torch.cuda.mem_get_info(device)
+    return max(1 << 20, int(free * INDEX_FREE_MEMORY_SHARE / SORT_DEVICE_BYTES_PER_INFLATED_BYTE))
+
+
+def read_header_bytes(bgzf):
+    """the BAM header through a BgzfReader -> (its inflated bytes from the magic through the references, contigs, virtual offset of the
+    first record)"""
+    contigs, first = read_header(bgzf)
+    l_text = struct.unpack("<i", bgzf.read_from(0, 8)[0][4:8])[0]
+    n = 12 + l_text + sum(9 + len(name.encode()) for name, _ in contigs)
+    return bgzf.read_from(0, n)[0], contigs, first
+
+
+def sort_header(header: bytes) -> bytes:
+    """the BAM header `header` as a coordinate sort writes it: the first text line, when it is @HD, gets SO:coordinate (its SO field
+    replaced, or appended); without an @HD line, "@HD\\tVN:1.6\\tSO:coordinate" is put first.  Everything else is kept byte for byte."""
+    l_text = struct.unpack("<i", header[4:8])[0]
+    text, rest = header[8:8 + l_text], header[8 + l_text:]
+    nl = text.find(b"\n")
+    first, tail = (text, b"") if nl < 0 else (text[:nl], text[nl:])
+    if first.startswith(b"@HD\t") or first == b"@HD":
+        fields = first.split(b"\t")
+        so = [k for k, f in enumerate(fields) if f.startswith(b"SO:")]
+        if so:
+            fields[so[0]] = b"SO:coordinate"
+        else:
+            fields.append(b"SO:coordinate")
+        text = b"\t".join(fields) + tail
+    else:
+        text = b"@HD\tVN:1.6\tSO:coordinate\n" + text
+    return header[:4] + struct.pack("<i", len(text)) + text + rest
+
+
+def sort_bam(path, out_path, device=0, window_bytes=None, bucket_bytes=None, ctx=None, stats=None):
+    """Write the BAM at `path` sorted by coordinate to `out_path`, as `samtools sort` orders it and cuts its BGZF members
+    (snfb_sort_bam; the rules are in include/snfb.h and DESIGN §4): the input streamed through the device in windows of `window_bytes`
+    inflated bytes for the keys, the output assembled and compressed on the device in buckets of `bucket_bytes` (defaults:
+    sort_budget_bytes).  The header is sort_header's.  Raises ValueError for a file that is not a BAM, binding.SnfbError (naming the record
+    or the block) for one the device refuses; out_path may then hold a partial file.  stats: a dict that receives n_records, n_windows,
+    n_buckets, n_members, n_input_reads, bytes_in, bytes_out, device_bytes and the device milliseconds ms_keys, ms_sort, ms_layout,
+    ms_scatter, ms_deflate (ms_layout_host: the host's member-cut loop)."""
+    from . import binding
+    reader = BgzfReader(path)
+    try:
+        header, contigs, first = read_header_bytes(reader)
+    finally:
+        reader.close()
+    own = ctx is None
+    ctx = ctx or binding.Context(device)
+    try:
+        budget = sort_budget_bytes(device) if window_bytes is None or bucket_bytes is None else 0
+        view = ctx.sort_bam(path, out_path, sort_header(header), first, [ln for _, ln in contigs], window_bytes or budget, bucket_bytes or budget)
+    finally:
+        if own:
+            ctx.close()
+    if stats is not None:
+        stats.update(view)
+    return view
+
+
 # ------------------------------------------------------------------------------------------------ writer (tests / benchmark inputs)
 def _bgzf_block(data: bytes, level: int = 6, strategy: int = zlib.Z_DEFAULT_STRATEGY) -> bytes:
     """one BGZF member: the header with its BC subfield, the raw DEFLATE stream of `data` from zlib, the CRC-32 / ISIZE trailer"""

@@ -20,7 +20,7 @@ EXPORTS = ["snfb_version", "snfb_sizeof", "snfb_hash_name", "snfb_ctx_create", "
            "snfb_load_bam", "snfb_set_regions", "snfb_ingest_sizes", "snfb_ingest_fetch", "snfb_inflate_bgzf", "snfb_deflate_bgzf",
            "snfb_genotype_targets", "snfb_load_reference", "snfb_reference_runs", "snfb_fetch_reference",
            "snfb_population_load", "snfb_population_match", "snfb_read_names", "snfb_set_consensus_slices",
-           "snfb_index_bam"]
+           "snfb_index_bam", "snfb_sort_bam"]
 
 
 def lib():
@@ -69,6 +69,7 @@ def lib():
         L.snfb_genotype_targets.argtypes = [C.c_void_p, C.POINTER(abi.GtIn), C.POINTER(abi.GtOut)]
         L.snfb_read_names.argtypes = [C.c_void_p, C.POINTER(abi.RnamesView)]
         L.snfb_index_bam.argtypes = [C.c_void_p, C.POINTER(abi.IndexInput), C.POINTER(abi.IndexView)]
+        L.snfb_sort_bam.argtypes = [C.c_void_p, C.POINTER(abi.SortInput), C.POINTER(abi.SortView)]
         L.snfb_load_reference.argtypes = [C.c_void_p, C.POINTER(abi.RefInput)]
         L.snfb_reference_runs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
         L.snfb_fetch_reference.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
@@ -348,6 +349,19 @@ class Context:
         out.update(n_no_coor=int(V.n_no_coor), n_records=int(V.n_records), n_windows=int(V.n_windows), device_bytes=int(V.device_bytes),
                    device_ms=float(V.device_ms))
         return out
+
+    def sort_bam(self, path, out_path, header, first_record, contig_lengths, window_bytes, bucket_bytes):
+        """The BAM at `path` sorted by coordinate into `out_path` on the device (snfb_sort_bam).  header: the output's BAM header bytes;
+        first_record: the input's virtual offset after its header; contig_lengths: the header's; window_bytes / bucket_bytes: inflated bytes
+        per input window / output bucket.  Returns a dict of the view's counts and per-phase milliseconds."""
+        clen = np.ascontiguousarray(contig_lengths, dtype="<i8")
+        hdr = np.frombuffer(bytes(header), dtype="u1")
+        I, V = abi.SortInput(), abi.SortView()
+        I.path, I.out_path, I.header, I.header_len = os.fsencode(path), os.fsencode(out_path), hdr.ctypes.data, len(hdr)
+        I.first_record, I.contig_len, I.n_ref = int(first_record), clen.ctypes.data, len(clen)
+        I.window_bytes, I.bucket_bytes = int(window_bytes), int(bucket_bytes)
+        self._check(self._lib.snfb_sort_bam(self._h, C.byref(I), C.byref(V)), "snfb_sort_bam")
+        return {n: (float if t is C.c_double else int)(getattr(V, n)) for n, t in abi.SortView._fields_}
 
     def load_reference(self, data, contigs, is_bgzf=False):
         """Reference FASTA -> the unwrapped genome resident on this context, and its 'N' runs (snfb_load_reference).  data: the file's bytes

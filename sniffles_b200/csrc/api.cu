@@ -8,6 +8,7 @@
 // capacity was too small (first run on a context, or a block unlike the previous one) the run is repeated with
 // capacities that fit — the counters always report what was needed.
 #include <algorithm>
+#include <chrono>
 #include <climits>
 #include <cstdio>
 #include <cstdlib>
@@ -31,6 +32,7 @@
 #include "rnames.cuh"
 #include "reference.cuh"
 #include "bam_index.cuh"
+#include "bam_sort.cuh"
 
 // one owning allocation of device memory, or of pinned host memory when Pinned; freed by the destructor
 template <bool Pinned> struct Buf {
@@ -117,6 +119,8 @@ struct snfb_ctx {
     // BAM index (snfb_index_bam): per-window candidate masks, chain nodes, the carried record; all rows; the table work; the tables on the host
     DevBuf b_ix_mask, b_ix_node, b_ix_carry, b_ix_rows, b_ix_tab;
     std::vector<uint64_t> ix_ref, ix_lin_off, ix_lin, ix_bin_key, ix_bin_loff, ix_chunk_u, ix_chunk_v; std::vector<uint32_t> ix_chunk_bin;
+    // BAM sort (snfb_sort_bam): per-record keys, lengths, offsets and their sort; one window's keys; bucket and window tables; a bucket's bytes
+    DevBuf b_st_rec, b_st_win, b_st_lay, b_st_bkt;
     std::vector<snfb_task> tasks;
     // region table (snfb_set_regions): host copy, device copy followed by each task's last region index; cov_view: some task's regions
     // are not increasing and disjoint, so stage A builds the coordinate-ordered (pos, end, flags) the coverage readers search
@@ -272,7 +276,8 @@ size_t snfb_sizeof(int which) {
                      case 8: return sizeof(snfb_gt_in); case 9: return sizeof(snfb_gt_out);
                      case 10: return sizeof(snfb_ref_contig); case 11: return sizeof(snfb_ref_input); case 12: return sizeof(snfb_ref_query); case 13: return sizeof(snfb_region);
                      case 14: return sizeof(snfb_combine_plan_in); case 15: return sizeof(snfb_combine_plan_out);
-                     case 16: return sizeof(snfb_pop_table); case 17: return sizeof(snfb_pop_query); case 18: return sizeof(snfb_rnames_view); default: return 0; }
+                     case 16: return sizeof(snfb_pop_table); case 17: return sizeof(snfb_pop_query); case 18: return sizeof(snfb_rnames_view);
+                     case 19: return sizeof(snfb_sort_input); case 20: return sizeof(snfb_sort_view); default: return 0; }
 }
 
 uint64_t snfb_hash_name(const char* s, size_t n) {
@@ -568,6 +573,33 @@ int snfb_inflate_bgzf(snfb_ctx* ctx, const uint8_t* bgzf, uint64_t n_bytes, uint
     return 0;
 }
 
+}  // extern "C"
+
+// BGZF members of device bytes: member k = d_in[moff[k], moff[k + 1]) (at most 0xff00 bytes, nb <= 65535) compressed by k_deflate into
+// ctx->b_zout, packed in member order; *n_out = their total size, h_offs[k] = member k's offset in b_zout.  Enqueued on ctx->st; the
+// caller synchronises before it reads h_offs / *n_out.
+static int deflate_members(snfb_ctx* ctx, const uint8_t* d_in, const std::vector<unsigned long long>& moff, unsigned long long* n_out, std::vector<uint32_t>& h_offs) {
+    const uint64_t nb = moff.size() - 1;
+    const unsigned grid = (unsigned)std::min<uint64_t>(nb, (uint64_t)NUM_SMS);
+    uint32_t *sizes = nullptr, *offs = nullptr, *tmp = nullptr; unsigned long long *total = nullptr, *d_moff = nullptr; uint16_t* scratch = nullptr;
+    auto lay = [&](Carver& c) { sizes = c.take<uint32_t>(nb + 1); offs = c.take<uint32_t>(nb + 1); tmp = c.take<uint32_t>(prims::scan_tmp_elems(nb));
+                                total = c.take<unsigned long long>(1); scratch = c.take<uint16_t>(2ull * deflate::BLOCK_IN * grid); d_moff = c.take<unsigned long long>(nb + 1); };
+    if (ctx->b_zslot.ensure(nb * deflate::MEMBER_MAX) || ctx->b_zout.ensure(nb * deflate::MEMBER_MAX) || carve(ctx->b_zwork, lay))
+        return fail(ctx, "out of device memory (BGZF compression)");
+    cudaStream_t st = ctx->st;
+    CUDA_TRY(cudaMemcpyAsync(d_moff, moff.data(), 8 * (nb + 1), cudaMemcpyHostToDevice, st));
+    launch(ctx->launches, bgzfw::k_deflate, grid, bgzfw::DEF_THREADS, bgzfw::DEF_SMEM_BYTES, st, d_in, (const unsigned long long*)d_moff, (unsigned)nb, scratch,
+           ctx->b_zslot.as<uint8_t>(), sizes);
+    prims::exclusive_scan(ctx->launches, sizes, offs, tmp, nullptr, nb, total, st);
+    launch(ctx->launches, bgzfw::k_pack, (unsigned)std::min<uint64_t>(nb, (uint64_t)NUM_SMS * 16), 256, 0, st, ctx->b_zslot.as<const uint8_t>(), sizes, offs, (unsigned)nb, ctx->b_zout.as<uint8_t>());
+    h_offs.resize(nb);
+    CUDA_TRY(cudaMemcpyAsync(n_out, total, sizeof(*n_out), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(h_offs.data(), offs, 4 * nb, cudaMemcpyDeviceToHost, st));
+    return 0;
+}
+
+extern "C" {
+
 int snfb_deflate_bgzf(snfb_ctx* ctx, const uint8_t* in, uint64_t n_in, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* coffset) {
     if (!ctx || !out_len || (n_in && (!in || !out))) return 1;
     cudaSetDevice(ctx->device);
@@ -577,25 +609,18 @@ int snfb_deflate_bgzf(snfb_ctx* ctx, const uint8_t* in, uint64_t n_in, uint8_t* 
     ctx->n_ev = 0;
     *out_len = 0;
     if (nb == 0) return 0;
-    const unsigned grid = (unsigned)std::min<uint64_t>(nb, (uint64_t)NUM_SMS);
-    uint32_t *sizes = nullptr, *offs = nullptr, *tmp = nullptr; unsigned long long* total = nullptr; uint16_t* scratch = nullptr;
-    auto lay = [&](Carver& c) { sizes = c.take<uint32_t>(nb + 1); offs = c.take<uint32_t>(nb + 1); tmp = c.take<uint32_t>(prims::scan_tmp_elems(nb));
-                                total = c.take<unsigned long long>(1); scratch = c.take<uint16_t>(2ull * deflate::BLOCK_IN * grid); };
-    if (ctx->b_zin.ensure(n_in + 64) || ctx->b_zslot.ensure(nb * deflate::MEMBER_MAX) || ctx->b_zout.ensure(nb * deflate::MEMBER_MAX) || carve(ctx->b_zwork, lay))
-        return fail(ctx, "out of device memory (BGZF compression)");
+    if (ctx->b_zin.ensure(n_in + 64)) return fail(ctx, "out of device memory (BGZF compression)");
+    std::vector<unsigned long long> moff(nb + 1);                   // fixed cuts: 0xff00 bytes per member, the rest in the last
+    for (uint64_t k = 0; k < nb; ++k) moff[k] = k * deflate::BLOCK_IN;
+    moff[nb] = n_in;
     cudaStream_t st = ctx->st;
     mark(ctx, "h2d_deflate", n_in);
     CUDA_TRY(cudaMemcpyAsync(ctx->b_zin.p, in, n_in, cudaMemcpyHostToDevice, st));
     mark(ctx, "deflate", n_in);
-    launch(ctx->launches, bgzfw::k_deflate, grid, bgzfw::DEF_THREADS, bgzfw::DEF_SMEM_BYTES, st, ctx->b_zin.as<const uint8_t>(), (unsigned long long)n_in, (unsigned)nb, scratch,
-           ctx->b_zslot.as<uint8_t>(), sizes);
-    prims::exclusive_scan(ctx->launches, sizes, offs, tmp, nullptr, nb, total, st);
-    launch(ctx->launches, bgzfw::k_pack, (unsigned)std::min<uint64_t>(nb, (uint64_t)NUM_SMS * 16), 256, 0, st, ctx->b_zslot.as<const uint8_t>(), sizes, offs, (unsigned)nb, ctx->b_zout.as<uint8_t>());
-    mark(ctx, "d2h_deflate", 0);
     unsigned long long n_out = 0;
-    std::vector<uint32_t> h_offs(nb);
-    CUDA_TRY(cudaMemcpyAsync(&n_out, total, sizeof(n_out), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(h_offs.data(), offs, 4 * nb, cudaMemcpyDeviceToHost, st));
+    std::vector<uint32_t> h_offs;
+    if (deflate_members(ctx, ctx->b_zin.as<const uint8_t>(), moff, &n_out, h_offs)) return 1;
+    mark(ctx, "d2h_deflate", 0);
     CUDA_TRY(cudaStreamSynchronize(st));
     CUDA_TRY(cudaMemcpyAsync(out, ctx->b_zout.p, n_out, cudaMemcpyDeviceToHost, st));
     mark(ctx, nullptr);
@@ -1889,27 +1914,35 @@ static std::string ix_name(const uint8_t* d_raw, uint64_t p) {
     return std::string(reinterpret_cast<const char*>(h + 36), l ? strnlen(reinterpret_cast<const char*>(h + 36), l) : 0);
 }
 
-extern "C" int snfb_index_bam(snfb_ctx* ctx, const snfb_index_input* in, snfb_index_view* out) {
-    using bamidx::Row;
-    if (!ctx || !in || !out || !in->path || (in->n_ref && !in->contig_len)) return ctx ? fail(ctx, "snfb_index_bam: null argument") : 1;
-    if (in->min_shift < 1 || in->depth < 1 || in->min_shift + 3 * in->depth > 40) return fail(ctx, "snfb_index_bam: min_shift + 3 * depth must be in 4..40");
-    cudaSetDevice(ctx->device);
-    ctx->n_ev = 0;
-    const uint64_t win = std::min<uint64_t>(std::max<uint64_t>(in->window_bytes, 1), 1ull << 31);
-    const bamidx::Geo geo{ in->min_shift, in->depth };
-    const uint32_t n_bins = (uint32_t)(((1ull << (3 * (in->depth + 1))) - 1) / 7);
-    const long long max_end = 1ll << (in->min_shift + 3 * in->depth);
-    const int n_ref = (int)in->n_ref;
+namespace {
+// device time: events around each phase of work the host hands the stream; the host's file reading between phases is not counted
+struct PhaseTimer {
+    cudaEvent_t a = nullptr, b = nullptr; double ms = 0;
+    PhaseTimer() { cudaEventCreate(&a); cudaEventCreate(&b); }
+    ~PhaseTimer() { cudaEventDestroy(a); cudaEventDestroy(b); }
+    void begin(cudaStream_t st) { cudaEventRecord(a, st); }
+    void end(cudaStream_t st) { cudaEventRecord(b, st); cudaEventSynchronize(b); float x = 0; cudaEventElapsedTime(&x, a, b); ms += x; }
+};
+// one window of the record chain, as stream_windows hands it over: the inflated bytes R[0, L) at global offset base (the carried bytes, then
+// the window's members from global offset G), the candidates cand[0, n) of which is_rec marks the n_rows complete chain records (rec_idx:
+// their index in the window, in file order); open: the chain ends in a record the window cannot finish (it is carried into the next one);
+// v_entry: the virtual offset of the window's first chain record
+struct ChainWin {
+    uint8_t* R; uint64_t base, L, G, coff_beg; const uint32_t *cand, *is_rec, *rec_idx; uint32_t n; uint64_t n_rows; bool open; uint64_t v_entry;
+    const IxWin* W; const unsigned long long *d_end, *d_coff;
+};
+}  // namespace
+
+// The BAM at `path` streamed through the device in windows of whole BGZF members of at most `win` inflated bytes: each window inflated and
+// CRC-checked behind the record the previous one could not finish, its record starts found from the entry by pointer jumping over the
+// offsets that pass the strict record test (bam_index.cuh), and on_window(const ChainWin&) called once the chain is resolved (nonzero: stop).
+// Failures name the block or the record; `what` prefixes the out-of-memory ones.  *n_windows, *file_bytes: windows read, bytes read.
+template <class OnWindow> static int stream_windows(snfb_ctx* ctx, const char* what, const char* path, uint64_t first_record, int n_ref, const long long* d_clen,
+                                                    uint64_t win, PhaseTimer& tm, uint64_t* n_windows_out, uint64_t* file_bytes, OnWindow&& on_window) {
     cudaStream_t st = ctx->st;
-    // device time: events around each phase of work the host hands the stream; the host's file reading between phases is not counted
-    struct PhaseTimer { cudaEvent_t a = nullptr, b = nullptr; double ms = 0; PhaseTimer() { cudaEventCreate(&a); cudaEventCreate(&b); } ~PhaseTimer() { cudaEventDestroy(a); cudaEventDestroy(b); } } tm;
-    auto t_begin = [&]() { cudaEventRecord(tm.a, st); };
-    auto t_end = [&]() { cudaEventRecord(tm.b, st); cudaEventSynchronize(tm.b); float x = 0; cudaEventElapsedTime(&x, tm.a, tm.b); tm.ms += x; };
-    long long* d_clen = nullptr;
-    if (carve(ctx->b_ix_tab, [&](Carver& c) { d_clen = c.take<long long>(n_ref + 1); })) return fail(ctx, "snfb_index_bam: out of device memory");
-    if (n_ref) CUDA_TRY(cudaMemcpyAsync(d_clen, in->contig_len, 8ull * n_ref, cudaMemcpyHostToDevice, st));
-    FILE* f = fopen(in->path, "rb");
-    if (!f) return fail(ctx, std::string("cannot open ") + in->path);
+    const std::string oom = std::string(what) + ": out of device memory";
+    FILE* f = fopen(path, "rb");
+    if (!f) return fail(ctx, std::string("cannot open ") + path);
     struct Closer { FILE* f; ~Closer() { fclose(f); } } closer{ f };
 
     std::vector<uint8_t> hb; uint64_t hb_off = 0; bool eof = false;      // read-ahead: file bytes from hb_off
@@ -1924,12 +1957,10 @@ extern "C" int snfb_index_bam(snfb_ctx* ctx, const snfb_index_input* in, snfb_in
             if (got == 0) eof = true;
         }
     };
-    // the entry: global inflated offset of the next record, its virtual offset; the previous row's tid / beg for the order check
+    // the entry: global inflated offset of the next record, its virtual offset
     uint64_t G = 0, n_windows = 0;
-    uint64_t u_entry = 0, v_entry = in->first_record; bool entry_known = false;
-    int prev_tid = -2, prev_beg = 0;
+    uint64_t u_entry = 0, v_entry = first_record; bool entry_known = false;
     uint64_t carry = 0;
-    std::vector<Row> rows;
     for (;;) {
         fill(std::max<uint64_t>(win, 1 << 17) + 65536 + 64);
         if (hb.empty()) break;
@@ -1953,19 +1984,19 @@ extern "C" int snfb_index_bam(snfb_ctx* ctx, const snfb_index_input* in, snfb_in
         IxWin W; W.first_beg = G; W.coff_end = hb_off + sel;
         for (size_t k = 0; k < blocks.size(); ++k) { W.end.push_back(G + blocks[k].out_off + blocks[k].isize); W.coff.push_back(hb_off + cstart[k]); }
         if (!entry_known) {                                                    // the header's end, as a global inflated offset
-            const uint64_t c = in->first_record >> 16, u = in->first_record & 0xffff;
+            const uint64_t c = first_record >> 16, u = first_record & 0xffff;
             auto it = std::find(W.coff.begin(), W.coff.end(), c);
             if (it != W.coff.end()) { const size_t k = (size_t)(it - W.coff.begin()); u_entry = (k ? W.end[k - 1] : G) + u; entry_known = true; }
         }
-        const uint64_t base = G - carry, L = carry + raw_len;
+        const uint64_t base = G - carry, L = carry + raw_len, G_win = G, coff_beg = hb_off;
         // inflate and CRC-check the window behind the carried bytes
-        if (ctx->b_comp.ensure(sel + 64) || ctx->b_raw.ensure(L + 64)) return fail(ctx, "snfb_index_bam: out of device memory for the window");
+        if (ctx->b_comp.ensure(sel + 64) || ctx->b_raw.ensure(L + 64)) return fail(ctx, oom + " for the window");
         for (auto& b : blocks) b.out_off += carry;
         uint8_t* R = ctx->b_raw.as<uint8_t>();
         ingest::IngestCounters* d_ctr = nullptr; ingest::BgzfBlock* d_blk = nullptr;
         if (carve(ctx->b_ing, [&](Carver& c) { d_ctr = c.take<ingest::IngestCounters>(1); d_blk = c.take<ingest::BgzfBlock>(blocks.size() + 1); }))
-            return fail(ctx, "snfb_index_bam: out of device memory (ingest tables)");
-        t_begin();
+            return fail(ctx, oom + " (ingest tables)");
+        tm.begin(st);
         if (carry) CUDA_TRY(cudaMemcpyAsync(R, ctx->b_ix_carry.p, carry, cudaMemcpyDeviceToDevice, st));
         CUDA_TRY(cudaMemcpyAsync(ctx->b_comp.p, hb.data(), sel, cudaMemcpyHostToDevice, st));
         CUDA_TRY(cudaMemsetAsync(ctx->b_comp.as<uint8_t>() + sel, 0, 64, st));
@@ -1975,7 +2006,7 @@ extern "C" int snfb_index_bam(snfb_ctx* ctx, const snfb_index_input* in, snfb_in
         launch_inflate(ctx, d_blk, (unsigned)blocks.size(), d_ctr);
         ingest::IngestCounters hc;
         CUDA_TRY(cudaMemcpyAsync(&hc, d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, st));
-        t_end();
+        tm.end(st);
         CUDA_TRY(cudaStreamSynchronize(st));
         if (hc.bad_blocks) {
             const unsigned long long first = ~hc.first_bad_inv, b = first >> 8, code = first & 255u;
@@ -1990,29 +2021,29 @@ extern "C" int snfb_index_bam(snfb_ctx* ctx, const snfb_index_input* in, snfb_in
         uint32_t *mask = nullptr, *cnt = nullptr, *wbase = nullptr, *stmp = nullptr; unsigned long long* misc = nullptr; unsigned long long *d_end = nullptr, *d_coff = nullptr;
         if (carve(ctx->b_ix_mask, [&](Carver& c) { mask = c.take<uint32_t>(n_words); cnt = c.take<uint32_t>(n_words); wbase = c.take<uint32_t>(n_words); stmp = c.take<uint32_t>(prims::scan_tmp_elems(n_words) + 16);
                                                    misc = c.take<unsigned long long>(8); d_end = c.take<unsigned long long>(W.end.size()); d_coff = c.take<unsigned long long>(W.coff.size()); }))
-            return fail(ctx, "snfb_index_bam: out of device memory (candidate masks)");
-        t_begin();
+            return fail(ctx, oom + " (candidate masks)");
+        tm.begin(st);
         CUDA_TRY(cudaMemcpyAsync(d_end, W.end.data(), 8 * W.end.size(), cudaMemcpyHostToDevice, st));
         CUDA_TRY(cudaMemcpyAsync(d_coff, W.coff.data(), 8 * W.coff.size(), cudaMemcpyHostToDevice, st));
         mark(ctx, "index_candidates", L);
-        launch(ctx->launches, bamidx::k_mark, grid_for(n_words * 32, 256), 256, 0, st, (const uint8_t*)R, (unsigned long long)L, (unsigned long long)e, n_ref, (const long long*)d_clen, mask, cnt, (unsigned long long)n_words);
+        launch(ctx->launches, bamidx::k_mark, grid_for(n_words * 32, 256), 256, 0, st, (const uint8_t*)R, (unsigned long long)L, (unsigned long long)e, n_ref, d_clen, mask, cnt, (unsigned long long)n_words);
         prims::exclusive_scan(ctx->launches, cnt, wbase, stmp, nullptr, n_words, &misc[0], st);
         unsigned long long n_cand = 0;
         CUDA_TRY(cudaMemcpyAsync(&n_cand, &misc[0], 8, cudaMemcpyDeviceToHost, st));
-        t_end();
+        tm.end(st);
         CUDA_TRY(cudaStreamSynchronize(st));
         const uint64_t v_e = e == 0 && carry ? v_entry : ix_voff(W, base + e);
         if (n_cand == 0) return fail(ctx, "the record at virtual offset " + voff_str(v_e) + " is not a valid BAM record");
         const uint32_t n = (uint32_t)n_cand, n2 = n + 2;
         const int K = std::max(1, bits_for(n2));
-        uint32_t *cand = nullptr, *J = nullptr, *is_rec = nullptr, *rec_idx = nullptr, *roff = nullptr, *ntmp = nullptr; uint8_t* pmark = nullptr; unsigned long long* res = nullptr; Row* d_rows = nullptr;
+        uint32_t *cand = nullptr, *J = nullptr, *is_rec = nullptr, *rec_idx = nullptr, *ntmp = nullptr; uint8_t* pmark = nullptr; unsigned long long* res = nullptr;
         if (carve(ctx->b_ix_node, [&](Carver& c) { cand = c.take<uint32_t>(n); J = c.take<uint32_t>((size_t)K * n2); pmark = c.take<uint8_t>(n2); is_rec = c.take<uint32_t>(n + 1); rec_idx = c.take<uint32_t>(n + 1);
-                                                   roff = c.take<uint32_t>(n + 1); ntmp = c.take<uint32_t>(prims::scan_tmp_elems(n) + 16); res = c.take<unsigned long long>(8); d_rows = c.take<Row>(n + 1); }))
-            return fail(ctx, "snfb_index_bam: out of device memory (" + std::to_string(n) + " candidate record starts)");
-        t_begin();
+                                                   ntmp = c.take<uint32_t>(prims::scan_tmp_elems(n) + 16); res = c.take<unsigned long long>(8); }))
+            return fail(ctx, oom + " (" + std::to_string(n) + " candidate record starts)");
+        tm.begin(st);
         mark(ctx, "index_chain", 0);
         launch(ctx->launches, bamidx::k_compact, grid_for(n_words * 32, 256), 256, 0, st, (const uint32_t*)mask, (const uint32_t*)wbase, (unsigned long long)n_words, cand);
-        launch(ctx->launches, bamidx::k_link, grid_for(n2, 256), 256, 0, st, (const uint8_t*)R, (unsigned long long)L, n_ref, (const long long*)d_clen, (const uint32_t*)cand, n, J);
+        launch(ctx->launches, bamidx::k_link, grid_for(n2, 256), 256, 0, st, (const uint8_t*)R, (unsigned long long)L, n_ref, d_clen, (const uint32_t*)cand, n, J);
         for (int k = 0; k + 1 < K; ++k) launch(ctx->launches, bamidx::k_jump, grid_for(n2, 256), 256, 0, st, (const uint32_t*)(J + (size_t)k * n2), J + (size_t)(k + 1) * n2, n2);
         CUDA_TRY(cudaMemsetAsync(pmark, 0, n2, st));
         CUDA_TRY(cudaMemsetAsync(pmark, 1, 1, st));
@@ -2024,7 +2055,7 @@ extern "C" int snfb_index_bam(snfb_ctx* ctx, const snfb_index_input* in, snfb_in
         CUDA_TRY(cudaMemcpyAsync(hres, res, 24, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(&cand0, cand, 4, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(&end_marked, pmark + n + bamidx::END_NODE, 1, cudaMemcpyDeviceToHost, st));
-        t_end();
+        tm.end(st);
         CUDA_TRY(cudaStreamSynchronize(st));
         if (cand0 != e) return fail(ctx, "the record at virtual offset " + voff_str(v_e) + " is not a valid BAM record");
         if (hres[1] != ~0ull) {
@@ -2034,49 +2065,85 @@ extern "C" int snfb_index_bam(snfb_ctx* ctx, const snfb_index_input* in, snfb_in
             return fail(ctx, "the record chain breaks after record '" + ix_name(R, p) + "' at virtual offset " + voff_str(vp) + ": the bytes at virtual offset "
                              + voff_str(ix_voff(W, base + p + 4 + bs)) + " are not a BAM record (corrupt or not a BAM file)");
         }
-        if (hres[0] == ~0ull && !end_marked) return fail(ctx, "snfb_index_bam: the record chain did not resolve");
-        const uint64_t n_rows = hres[2];
-        const uint64_t row_base = rows.size();
-        if (n_rows) {
-            t_begin();
-            mark(ctx, "index_rows", 0);
-            bamidx::Window DW{ base, W.first_beg, W.coff_end, d_end, d_coff, (unsigned)W.end.size() };
-            launch(ctx->launches, bamidx::k_rows, grid_for((uint64_t)n * 32, 256), 256, 0, st, (const uint8_t*)R, (const uint32_t*)cand, (const uint32_t*)is_rec, (const uint32_t*)rec_idx, n, DW, d_rows, roff);
-            CUDA_TRY(cudaMemsetAsync(&res[3], 0xff, 8, st));
-            launch(ctx->launches, bamidx::k_check, grid_for(n_rows, 256), 256, 0, st, d_rows, (uint32_t)n_rows, (unsigned long long)v_entry, prev_tid, prev_beg, max_end, (unsigned long long)row_base, &res[3]);
-            rows.resize(row_base + n_rows);
-            unsigned long long bad = 0;
-            CUDA_TRY(cudaMemcpyAsync(rows.data() + row_base, d_rows, sizeof(Row) * n_rows, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(&bad, &res[3], 8, cudaMemcpyDeviceToHost, st));
-            t_end();
-            CUDA_TRY(cudaStreamSynchronize(st));
-            if (bad != bamidx::BAD_NONE) {
-                const uint64_t r = bad & ((1ull << 56) - 1), i = r - row_base; const unsigned code = (unsigned)(bad >> 56);
-                uint32_t p = 0; CUDA_TRY(cudaMemcpy(&p, roff + i, 4, cudaMemcpyDeviceToHost));
-                const Row& x = rows[r];
-                const int pt = r ? rows[r - 1].tid : prev_tid, pb = r ? rows[r - 1].beg : prev_beg;
-                std::string why;
-                if (code == bamidx::BAD_ORDER) why = "unsorted positions on reference #" + std::to_string(x.tid) + ": " + std::to_string(x.beg + 1) + " after " + std::to_string(pb + 1);
-                else if (code == bamidx::BAD_TID_AFTER_UNPLACED) why = "a record on reference #" + std::to_string(x.tid) + " after the unplaced records (reference -1), which must come last";
-                else if (code == bamidx::BAD_TID_BACK) why = "reference #" + std::to_string(x.tid) + " after reference #" + std::to_string(pt) + ": the records are not sorted by coordinate";
-                else why = "end " + std::to_string(x.end) + " beyond the " + std::to_string(max_end) + " positions the index geometry covers (a BAI covers 2^29: use -c for a CSI index)";
-                return fail(ctx, "record '" + ix_name(R, p) + "' (record " + std::to_string(r + 1) + " of the file, virtual offset " + voff_str(x.v0) + "): " + why);
-            }
-            v_entry = rows.back().v1; prev_tid = rows.back().tid; prev_beg = rows.back().beg;
-        }
+        if (hres[0] == ~0ull && !end_marked) return fail(ctx, std::string(what) + ": the record chain did not resolve");
+        const ChainWin cw{ R, base, L, G_win, coff_beg, cand, is_rec, rec_idx, n, hres[2], hres[0] != ~0ull, v_entry, &W, d_end, d_coff };
+        if (on_window(cw)) return 1;
+        if (hres[2]) v_entry = ix_voff(W, hres[0] != ~0ull ? base + hres[0] : base + L);      // the virtual offset after the last complete record
         mark(ctx, nullptr);
         if (hres[0] != ~0ull) {                        // the chain ends in a record the window cannot finish: carry it into the next one
             const uint64_t o = hres[0];
             carry = L - o;
-            if (ctx->b_ix_carry.ensure(carry + 64)) return fail(ctx, "snfb_index_bam: out of device memory (carried record)");
+            if (ctx->b_ix_carry.ensure(carry + 64)) return fail(ctx, oom + " (carried record)");
             CUDA_TRY(cudaMemcpyAsync(ctx->b_ix_carry.p, R + o, carry, cudaMemcpyDeviceToDevice, st));
             u_entry = base + o;
         } else { carry = 0; u_entry = base + L; }
     }
-    if (!entry_known && in->first_record == hb_off << 16) entry_known = true, u_entry = G;      // a header-only file without the EOF member
+    if (!entry_known && first_record == hb_off << 16) entry_known = true, u_entry = G;      // a header-only file without the EOF member
     if (!entry_known || u_entry != G)
         return fail(ctx, "truncated BAM file: the record at virtual offset " + voff_str(v_entry) + " extends past the end of the data (" + std::to_string(G) + " inflated bytes)");
     CUDA_TRY(cudaStreamSynchronize(st));
+    *n_windows_out = n_windows; *file_bytes = hb_off;
+    return 0;
+}
+
+extern "C" int snfb_index_bam(snfb_ctx* ctx, const snfb_index_input* in, snfb_index_view* out) {
+    using bamidx::Row;
+    if (!ctx || !in || !out || !in->path || (in->n_ref && !in->contig_len)) return ctx ? fail(ctx, "snfb_index_bam: null argument") : 1;
+    if (in->min_shift < 1 || in->depth < 1 || in->min_shift + 3 * in->depth > 40) return fail(ctx, "snfb_index_bam: min_shift + 3 * depth must be in 4..40");
+    cudaSetDevice(ctx->device);
+    ctx->n_ev = 0;
+    const uint64_t win = std::min<uint64_t>(std::max<uint64_t>(in->window_bytes, 1), 1ull << 31);
+    const bamidx::Geo geo{ in->min_shift, in->depth };
+    const uint32_t n_bins = (uint32_t)(((1ull << (3 * (in->depth + 1))) - 1) / 7);
+    const long long max_end = 1ll << (in->min_shift + 3 * in->depth);
+    const int n_ref = (int)in->n_ref;
+    cudaStream_t st = ctx->st;
+    PhaseTimer tm;
+    auto t_begin = [&]() { tm.begin(st); };
+    auto t_end = [&]() { tm.end(st); };
+    long long* d_clen = nullptr;
+    if (carve(ctx->b_ix_tab, [&](Carver& c) { d_clen = c.take<long long>(n_ref + 1); })) return fail(ctx, "snfb_index_bam: out of device memory");
+    if (n_ref) CUDA_TRY(cudaMemcpyAsync(d_clen, in->contig_len, 8ull * n_ref, cudaMemcpyHostToDevice, st));
+    // the previous row's tid / beg for the order check
+    int prev_tid = -2, prev_beg = 0;
+    std::vector<Row> rows;
+    uint64_t n_windows = 0, file_bytes = 0;
+    auto on_window = [&](const ChainWin& c) -> int {
+        const uint64_t n_rows = c.n_rows;
+        if (!n_rows) return 0;
+        const uint64_t row_base = rows.size();
+        const uint32_t n = c.n;
+        uint32_t* roff = nullptr; Row* d_rows = nullptr; unsigned long long* bad_d = nullptr;
+        if (carve(ctx->b_ix_rows, [&](Carver& cv) { roff = cv.take<uint32_t>(n + 1); d_rows = cv.take<Row>(n + 1); bad_d = cv.take<unsigned long long>(1); }))
+            return fail(ctx, "snfb_index_bam: out of device memory (" + std::to_string(n) + " candidate record starts)");
+        t_begin();
+        mark(ctx, "index_rows", 0);
+        bamidx::Window DW{ c.base, c.W->first_beg, c.W->coff_end, c.d_end, c.d_coff, (unsigned)c.W->end.size() };
+        launch(ctx->launches, bamidx::k_rows, grid_for((uint64_t)n * 32, 256), 256, 0, st, (const uint8_t*)c.R, c.cand, c.is_rec, c.rec_idx, n, DW, d_rows, roff);
+        CUDA_TRY(cudaMemsetAsync(bad_d, 0xff, 8, st));
+        launch(ctx->launches, bamidx::k_check, grid_for(n_rows, 256), 256, 0, st, d_rows, (uint32_t)n_rows, (unsigned long long)c.v_entry, prev_tid, prev_beg, max_end, (unsigned long long)row_base, bad_d);
+        rows.resize(row_base + n_rows);
+        unsigned long long bad = 0;
+        CUDA_TRY(cudaMemcpyAsync(rows.data() + row_base, d_rows, sizeof(Row) * n_rows, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(&bad, bad_d, 8, cudaMemcpyDeviceToHost, st));
+        t_end();
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if (bad != bamidx::BAD_NONE) {
+            const uint64_t r = bad & ((1ull << 56) - 1), i = r - row_base; const unsigned code = (unsigned)(bad >> 56);
+            uint32_t p = 0; CUDA_TRY(cudaMemcpy(&p, roff + i, 4, cudaMemcpyDeviceToHost));
+            const Row& x = rows[r];
+            const int pt = r ? rows[r - 1].tid : prev_tid, pb = r ? rows[r - 1].beg : prev_beg;
+            std::string why;
+            if (code == bamidx::BAD_ORDER) why = "unsorted positions on reference #" + std::to_string(x.tid) + ": " + std::to_string(x.beg + 1) + " after " + std::to_string(pb + 1);
+            else if (code == bamidx::BAD_TID_AFTER_UNPLACED) why = "a record on reference #" + std::to_string(x.tid) + " after the unplaced records (reference -1), which must come last";
+            else if (code == bamidx::BAD_TID_BACK) why = "reference #" + std::to_string(x.tid) + " after reference #" + std::to_string(pt) + ": the records are not sorted by coordinate";
+            else why = "end " + std::to_string(x.end) + " beyond the " + std::to_string(max_end) + " positions the index geometry covers (a BAI covers 2^29: use -c for a CSI index)";
+            return fail(ctx, "record '" + ix_name(c.R, p) + "' (record " + std::to_string(r + 1) + " of the file, virtual offset " + voff_str(x.v0) + "): " + why);
+        }
+        prev_tid = rows.back().tid; prev_beg = rows.back().beg;
+        return 0;
+    };
+    if (stream_windows(ctx, "snfb_index_bam", in->path, in->first_record, n_ref, d_clen, win, tm, &n_windows, &file_bytes, on_window)) return 1;
 
     // ---- tables over all rows
     const uint64_t n_rec = rows.size();
@@ -2174,5 +2241,219 @@ extern "C" int snfb_index_bam(snfb_ctx* ctx, const snfb_index_input* in, snfb_in
     out->n_bin = nub; out->n_chunk = nm; out->n_no_coor = n_rec - n_placed; out->n_records = n_rec; out->n_windows = n_windows;
     out->device_ms = tm.ms;
     out->device_bytes = ctx->b_comp.cap + ctx->b_raw.cap + ctx->b_ing.cap + ctx->b_ix_mask.cap + ctx->b_ix_node.cap + ctx->b_ix_carry.cap + ctx->b_ix_rows.cap + ctx->b_ix_tab.cap;
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ BAM sort (bam_sort.cuh)
+extern "C" int snfb_sort_bam(snfb_ctx* ctx, const snfb_sort_input* in, snfb_sort_view* out) {
+    if (!ctx || !in || !out || !in->path || !in->out_path || !in->header || (in->n_ref && !in->contig_len)) return ctx ? fail(ctx, "snfb_sort_bam: null argument") : 1;
+    if (in->header_len < 12) return fail(ctx, "snfb_sort_bam: the output header must hold at least the magic, l_text and n_ref");
+    cudaSetDevice(ctx->device);
+    ctx->n_ev = 0;
+    *out = snfb_sort_view{};
+    const uint64_t win = std::min<uint64_t>(std::max<uint64_t>(in->window_bytes, 1), 1ull << 31);
+    const uint64_t bucket_cap = std::max<uint64_t>(in->bucket_bytes, 1);
+    const uint64_t BS = deflate::BLOCK_IN;
+    const int n_ref = (int)in->n_ref;
+    cudaStream_t st = ctx->st;
+    PhaseTimer t_keys, t_sort, t_layout, t_scatter, t_deflate;
+    long long* d_clen = nullptr;
+    if (carve(ctx->b_st_lay, [&](Carver& c) { d_clen = c.take<long long>(n_ref + 1); })) return fail(ctx, "snfb_sort_bam: out of device memory");
+    if (n_ref) CUDA_TRY(cudaMemcpyAsync(d_clen, in->contig_len, 8ull * n_ref, cudaMemcpyHostToDevice, st));
+
+    // ---- keys pass: per record its key, its length 4 + block_size and its global inflated offset; per window its geometry and the
+    // input ordinals of the records with bytes in it (those completed in it, and the one carried out of it)
+    struct SWin { uint64_t coff_beg, coff_end, G, raw_len, o0, o1; };
+    std::vector<SWin> wins;
+    std::vector<uint64_t> h_key, h_src; std::vector<uint32_t> h_len;
+    auto on_window = [&](const ChainWin& c) -> int {
+        const uint64_t row_base = h_key.size();
+        if (row_base + c.n_rows >= (1ull << 32)) return fail(ctx, "snfb_sort_bam: 2^32 records or more (record " + std::to_string(row_base + c.n_rows) + "): more than the sort's 32-bit ordinals hold");
+        wins.push_back(SWin{ c.coff_beg, c.W->coff_end, c.G, c.W->end.back() - c.G, row_base, row_base + c.n_rows + (c.open ? 1 : 0) });
+        if (!c.n_rows) return 0;
+        uint64_t* key = nullptr; uint32_t* len = nullptr; unsigned long long* src = nullptr;
+        if (carve(ctx->b_st_win, [&](Carver& cv) { key = cv.take<uint64_t>(c.n_rows); len = cv.take<uint32_t>(c.n_rows); src = cv.take<unsigned long long>(c.n_rows); }))
+            return fail(ctx, "snfb_sort_bam: out of device memory (window keys)");
+        h_key.resize(row_base + c.n_rows); h_len.resize(row_base + c.n_rows); h_src.resize(row_base + c.n_rows);
+        t_keys.begin(st);
+        mark(ctx, "sort_keys", 0);
+        launch(ctx->launches, bamsort::k_keys, grid_for(c.n, 256), 256, 0, st, (const uint8_t*)c.R, c.cand, c.is_rec, c.rec_idx, c.n, (unsigned long long)c.base, n_ref, key, len, src);
+        CUDA_TRY(cudaMemcpyAsync(h_key.data() + row_base, key, 8 * c.n_rows, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(h_len.data() + row_base, len, 4 * c.n_rows, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(h_src.data() + row_base, src, 8 * c.n_rows, cudaMemcpyDeviceToHost, st));
+        t_keys.end(st);
+        return 0;
+    };
+    uint64_t n_windows = 0, bytes_in = 0;
+    if (stream_windows(ctx, "snfb_sort_bam", in->path, in->first_record, n_ref, d_clen, win, t_keys, &n_windows, &bytes_in, on_window)) return 1;
+    const uint64_t n = h_key.size();
+    const uint32_t n_win = (uint32_t)wins.size();
+
+    // ---- sort: one stable radix sort of the keys, over only the bits they use; values = input ordinals
+    uint64_t *k0 = nullptr, *k1 = nullptr; uint32_t *v0 = nullptr, *v1 = nullptr, *len = nullptr, *hist = nullptr, *stmp = nullptr;
+    unsigned long long *src = nullptr, *dest = nullptr, *dsort = nullptr, *cnt = nullptr;
+    const size_t hist_n = prims::radix_hist_elems(n + 1);
+    if (carve(ctx->b_st_rec, [&](Carver& c) { k0 = c.take<uint64_t>(n + 1); k1 = c.take<uint64_t>(n + 1); v0 = c.take<uint32_t>(n + 1); v1 = c.take<uint32_t>(n + 1);
+                                              len = c.take<uint32_t>(n + 1); src = c.take<unsigned long long>(n + 1); dest = c.take<unsigned long long>(n + 1); dsort = c.take<unsigned long long>(n + 1);
+                                              cnt = c.take<unsigned long long>(8); hist = c.take<uint32_t>(hist_n); stmp = c.take<uint32_t>(prims::scan_tmp_elems(hist_n) + 16); }))
+        return fail(ctx, "snfb_sort_bam: out of device memory (" + std::to_string(n) + " record keys)");
+    std::vector<uint32_t> h_slen(n);
+    const uint32_t* ord = v0;
+    if (n) {
+        const unsigned long long hn = n;
+        t_sort.begin(st);
+        mark(ctx, "sort_radix", 12 * n);
+        CUDA_TRY(cudaMemcpyAsync(k0, h_key.data(), 8 * n, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(len, h_len.data(), 4 * n, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(src, h_src.data(), 8 * n, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(cnt, &hn, 8, cudaMemcpyHostToDevice, st));
+        launch(ctx->launches, bamsort::k_iota, grid_for(n, 256), 256, 0, st, v0, (unsigned long long)n);
+        bool in_first = true;
+        prims::radix_sort(ctx->launches, k0, v0, k1, v1, prims::RadixTemp{ hist, stmp }, (const unsigned long long*)cnt, n, 33 + bits_for((uint32_t)n_ref + 1), &in_first, st);
+        ord = in_first ? v0 : v1;
+        uint32_t* slen = in_first ? v1 : v0;
+        t_sort.end(st);
+        t_layout.begin(st);
+        mark(ctx, "sort_layout", 4 * n);
+        launch(ctx->launches, bamsort::k_gather_len, grid_for(n, 256), 256, 0, st, ord, (const uint32_t*)len, (unsigned long long)n, slen);
+        CUDA_TRY(cudaMemcpyAsync(h_slen.data(), slen, 4 * n, cudaMemcpyDeviceToHost, st));
+        t_layout.end(st);
+    }
+    std::vector<uint64_t>().swap(h_key); std::vector<uint32_t>().swap(h_len); std::vector<uint64_t>().swap(h_src);
+
+    // ---- layout: htslib's member cuts over the sorted lengths (sequential by definition: one host loop), each record's output offset,
+    // then buckets of whole members that start at a record start
+    const auto h0 = std::chrono::steady_clock::now();
+    const uint64_t H = in->header_len;
+    std::vector<uint64_t> mend;                    // member k = output bytes [k ? mend[k - 1] : 0, mend[k])
+    std::vector<uint32_t> unit{ 0 };               // members that start at a record start (or at the header)
+    std::vector<unsigned long long> h_dsort(n);
+    for (uint64_t o = 0; o < H;) { o = std::min(o + BS, H); mend.push_back(o); }
+    uint64_t pos = H, cur = 0;
+    for (uint64_t s = 0; s < n; ++s) {
+        uint64_t r = h_slen[s];
+        if (cur && cur + r > BS) { mend.push_back(pos); cur = 0; }
+        if (!cur) unit.push_back((uint32_t)mend.size());
+        h_dsort[s] = pos;
+        while (r) { const uint64_t take = std::min(r, BS - cur); cur += take; pos += take; r -= take; if (cur == BS) { mend.push_back(pos); cur = 0; } }
+    }
+    if (cur) mend.push_back(pos);
+    const uint32_t nm = (uint32_t)mend.size();
+    auto mbeg = [&](uint32_t m) -> uint64_t { return m ? mend[m - 1] : 0; };
+    std::vector<uint32_t> bm{ 0 };                 // bucket k = members [bm[k], bm[k + 1])
+    {
+        uint32_t last = 0;
+        for (size_t i = 1; i <= unit.size(); ++i) {
+            const uint32_t c = i < unit.size() ? unit[i] : nm;
+            if (mend[c - 1] - mbeg(bm.back()) > bucket_cap && last > bm.back()) bm.push_back(last);
+            last = c;
+        }
+        bm.push_back(nm);
+    }
+    const uint32_t n_bkt = (uint32_t)bm.size() - 1;
+    std::vector<unsigned long long> h_bkt_beg(n_bkt), h_win_beg(n_win);
+    for (uint32_t k = 0; k < n_bkt; ++k) h_bkt_beg[k] = mbeg(bm[k]);
+    for (uint32_t w = 0; w < n_win; ++w) h_win_beg[w] = wins[w].G;
+    out->ms_layout_host = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - h0).count();
+    std::vector<uint32_t> win_lo(n_win, ~0u), win_hi(n_win, 0);
+    if (n) {
+        unsigned long long *d_bkt = nullptr, *d_win = nullptr; uint32_t *d_lo = nullptr, *d_hi = nullptr;
+        if (carve(ctx->b_st_lay, [&](Carver& c) { d_bkt = c.take<unsigned long long>(n_bkt + 1); d_win = c.take<unsigned long long>(n_win + 1); d_lo = c.take<uint32_t>(n_win + 1); d_hi = c.take<uint32_t>(n_win + 1); }))
+            return fail(ctx, "snfb_sort_bam: out of device memory (bucket tables)");
+        t_layout.begin(st);
+        mark(ctx, "sort_place", 8 * n);
+        CUDA_TRY(cudaMemcpyAsync(dsort, h_dsort.data(), 8 * n, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_bkt, h_bkt_beg.data(), 8ull * n_bkt, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_win, h_win_beg.data(), 8ull * n_win, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemsetAsync(d_lo, 0xff, 4ull * n_win, st));
+        CUDA_TRY(cudaMemsetAsync(d_hi, 0, 4ull * n_win, st));
+        launch(ctx->launches, bamsort::k_place, grid_for(n, 256), 256, 0, st, ord, (const unsigned long long*)dsort, (unsigned long long)n, (const unsigned long long*)src,
+               (const uint32_t*)len, (const unsigned long long*)d_bkt, n_bkt, (const unsigned long long*)d_win, n_win, dest, d_lo, d_hi);
+        CUDA_TRY(cudaMemcpyAsync(win_lo.data(), d_lo, 4ull * n_win, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(win_hi.data(), d_hi, 4ull * n_win, cudaMemcpyDeviceToHost, st));
+        t_layout.end(st);
+    }
+    mark(ctx, nullptr);
+
+    // ---- per bucket: the windows holding its records read again, their records scattered into the bucket, its members compressed
+    FILE* fi = fopen(in->path, "rb");
+    if (!fi) return fail(ctx, std::string("cannot open ") + in->path);
+    struct Closer { FILE* f; ~Closer() { if (f) fclose(f); } } cin{ fi };
+    FILE* fo = fopen(in->out_path, "wb");
+    if (!fo) return fail(ctx, std::string("cannot create ") + in->out_path);
+    Closer cout_{ fo };
+    std::vector<uint8_t> hz, hout;
+    uint64_t reads = n_windows, bytes_out = 0;
+    for (uint32_t k = 0; k < n_bkt; ++k) {
+        const uint64_t O0 = mbeg(bm[k]), O1 = mend[bm[k + 1] - 1];
+        if (ctx->b_st_bkt.ensure(O1 - O0 + 64)) return fail(ctx, "snfb_sort_bam: out of device memory (a bucket of " + std::to_string(O1 - O0) + " bytes)");
+        uint8_t* B = ctx->b_st_bkt.as<uint8_t>();
+        if (O0 < H) CUDA_TRY(cudaMemcpyAsync(B, in->header, std::min(H, O1) - O0, cudaMemcpyHostToDevice, st));
+        for (uint32_t w = 0; w < n_win; ++w) {
+            if (win_lo[w] > k || win_hi[w] < k) continue;
+            const SWin& W = wins[w];
+            const uint64_t nz = W.coff_end - W.coff_beg;
+            hz.resize(nz);
+            if (fseeko(fi, (off_t)W.coff_beg, SEEK_SET) != 0 || fread(hz.data(), 1, nz, fi) != nz)
+                return fail(ctx, "cannot read the input again at file offset " + std::to_string(W.coff_beg) + ": the file changed while it was sorted");
+            std::vector<ingest::BgzfBlock> blocks; std::vector<uint64_t> cstart; uint64_t raw_len = 0;
+            if (walk_bgzf(ctx, hz.data(), nz, blocks, cstart, &raw_len)) return 1;
+            if (raw_len != W.raw_len) return fail(ctx, "the input changed while it was sorted (window at file offset " + std::to_string(W.coff_beg) + ")");
+            if (ctx->b_comp.ensure(nz + 64) || ctx->b_raw.ensure(raw_len + 64)) return fail(ctx, "snfb_sort_bam: out of device memory for the window");
+            ingest::IngestCounters* d_ctr = nullptr; ingest::BgzfBlock* d_blk = nullptr;
+            if (carve(ctx->b_ing, [&](Carver& c) { d_ctr = c.take<ingest::IngestCounters>(1); d_blk = c.take<ingest::BgzfBlock>(blocks.size() + 1); }))
+                return fail(ctx, "snfb_sort_bam: out of device memory (ingest tables)");
+            t_scatter.begin(st);
+            mark(ctx, "sort_scatter", raw_len);
+            CUDA_TRY(cudaMemcpyAsync(ctx->b_comp.p, hz.data(), nz, cudaMemcpyHostToDevice, st));
+            CUDA_TRY(cudaMemsetAsync(ctx->b_comp.as<uint8_t>() + nz, 0, 64, st));
+            CUDA_TRY(cudaMemsetAsync(ctx->b_raw.as<uint8_t>() + raw_len, 0, 64, st));
+            CUDA_TRY(cudaMemsetAsync(d_ctr, 0, sizeof(ingest::IngestCounters), st));
+            CUDA_TRY(cudaMemcpyAsync(d_blk, blocks.data(), sizeof(ingest::BgzfBlock) * blocks.size(), cudaMemcpyHostToDevice, st));
+            launch_inflate(ctx, d_blk, (unsigned)blocks.size(), d_ctr);
+            if (W.o1 > W.o0)
+                launch(ctx->launches, bamsort::k_scatter, grid_for((W.o1 - W.o0) * 32, 256), 256, 0, st, (const uint8_t*)ctx->b_raw.p, (unsigned long long)W.G, (unsigned long long)raw_len,
+                       (uint32_t)W.o0, (uint32_t)W.o1, (const unsigned long long*)src, (const uint32_t*)len, (const unsigned long long*)dest, (unsigned long long)O0, (unsigned long long)O1, B);
+            ingest::IngestCounters hc;
+            CUDA_TRY(cudaMemcpyAsync(&hc, d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, st));
+            t_scatter.end(st);
+            mark(ctx, nullptr);
+            if (hc.bad_blocks) {
+                const unsigned long long first = ~hc.first_bad_inv, b = first >> 8, code = first & 255u;
+                return fail(ctx, "BGZF block at file offset " + std::to_string(W.coff_beg + cstart[b]) + (code == ingest::INF_CRC_MISMATCH ? ": CRC32 mismatch" : ": failed to inflate (code " + std::to_string(code) + ")"));
+            }
+            ++reads; bytes_in += nz;
+        }
+        // the bucket's members, at most 65535 per launch
+        for (uint32_t m = bm[k]; m < bm[k + 1];) {
+            const uint32_t m2 = std::min<uint32_t>(bm[k + 1], m + 65535u);
+            std::vector<unsigned long long> moff(m2 - m + 1);
+            for (uint32_t j = m; j <= m2; ++j) moff[j - m] = mbeg(j) - mbeg(m);
+            unsigned long long n_z = 0; std::vector<uint32_t> offs;
+            t_deflate.begin(st);
+            mark(ctx, "sort_deflate", moff.back());
+            if (deflate_members(ctx, B + (mbeg(m) - O0), moff, &n_z, offs)) return 1;
+            CUDA_TRY(cudaStreamSynchronize(st));
+            hout.resize(n_z);
+            CUDA_TRY(cudaMemcpyAsync(hout.data(), ctx->b_zout.p, n_z, cudaMemcpyDeviceToHost, st));
+            t_deflate.end(st);
+            mark(ctx, nullptr);
+            if (fwrite(hout.data(), 1, n_z, fo) != n_z) return fail(ctx, std::string("cannot write ") + in->out_path);
+            bytes_out += n_z;
+            m = m2;
+        }
+    }
+    static const uint8_t eof_member[28] = { 0x1f, 0x8b, 8, 4, 0, 0, 0, 0, 0, 0xff, 6, 0, 0x42, 0x43, 2, 0, 0x1b, 0, 3, 0, 0, 0, 0, 0, 0, 0, 0, 0 };
+    if (fwrite(eof_member, 1, 28, fo) != 28 || fflush(fo) != 0) return fail(ctx, std::string("cannot write ") + in->out_path);
+    bytes_out += 28;
+    cout_.f = nullptr;
+    if (fclose(fo) != 0) return fail(ctx, std::string("cannot write ") + in->out_path);
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaGetLastError());
+    out->n_records = n; out->n_windows = n_windows; out->n_buckets = n_bkt; out->n_members = nm; out->n_input_reads = reads;
+    out->bytes_in = bytes_in; out->bytes_out = bytes_out;
+    out->device_bytes = ctx->b_comp.cap + ctx->b_raw.cap + ctx->b_ing.cap + ctx->b_ix_mask.cap + ctx->b_ix_node.cap + ctx->b_ix_carry.cap + ctx->b_st_rec.cap + ctx->b_st_win.cap
+                        + ctx->b_st_lay.cap + ctx->b_st_bkt.cap + ctx->b_zslot.cap + ctx->b_zout.cap + ctx->b_zwork.cap;
+    out->ms_keys = t_keys.ms; out->ms_sort = t_sort.ms; out->ms_layout = t_layout.ms; out->ms_scatter = t_scatter.ms; out->ms_deflate = t_deflate.ms;
     return 0;
 }

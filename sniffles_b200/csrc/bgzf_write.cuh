@@ -1,6 +1,7 @@
 // bgzf_write.cuh — BGZF compression on the device (snfb_deflate_bgzf): the encoder of deflate_core.h with a thread block per BGZF block.
 //
-//   k_deflate   one thread block (DEF_THREADS) per 0xff00-byte input block, grid-stride over the blocks with one resident block per SM
+//   k_deflate   one thread block (DEF_THREADS) per member of the table moff (member k = in[moff[k], moff[k + 1]), at most 0xff00 bytes;
+//               snfb_deflate_bgzf passes fixed 0xff00 cuts, snfb_sort_bam htslib's record-aware ones), grid-stride over the members with one resident block per SM
 //               (the block's bytes, match lengths and bit buffer take ~217 KB of shared memory).  Warp 0 finds the hash candidates
 //               while warp 1 computes the CRC-32 (crc32_group<32>); every thread computes match lengths; warp 0 parses; every thread
 //               counts symbols, thread 0 builds the codes and picks the block type; every thread writes its slice's tokens; the member
@@ -18,7 +19,7 @@ static_assert(DEF_THREADS <= deflate::MAX_THREADS, "one bit count per thread");
 constexpr size_t DEF_SMEM_BYTES = sizeof(deflate::Shared);
 static_assert(DEF_SMEM_BYTES <= 227 * 1024, "k_deflate's shared memory must fit one thread block per SM on sm_90");
 
-__global__ void __launch_bounds__(DEF_THREADS, 1) k_deflate(const uint8_t* __restrict__ in, unsigned long long n_in, unsigned nb, uint16_t* __restrict__ scratch,
+__global__ void __launch_bounds__(DEF_THREADS, 1) k_deflate(const uint8_t* __restrict__ in, const unsigned long long* __restrict__ moff, unsigned nb, uint16_t* __restrict__ scratch,
                                                              uint8_t* __restrict__ slots, uint32_t* __restrict__ sizes) {
     extern __shared__ __align__(16) uint8_t deflate_smem[];
     deflate::Shared* S = reinterpret_cast<deflate::Shared*>(deflate_smem);
@@ -27,8 +28,8 @@ __global__ void __launch_bounds__(DEF_THREADS, 1) k_deflate(const uint8_t* __res
     uint16_t* cand = scratch + 2ull * deflate::BLOCK_IN * blockIdx.x;
     uint16_t* dist = cand + deflate::BLOCK_IN;
     for (unsigned k = blockIdx.x; k < nb; k += gridDim.x) {
-        const unsigned long long off = (unsigned long long)k * deflate::BLOCK_IN;
-        const uint32_t n = (uint32_t)(n_in - off < deflate::BLOCK_IN ? n_in - off : deflate::BLOCK_IN);
+        const unsigned long long off = moff[k];
+        const uint32_t n = (uint32_t)(moff[k + 1] - off);
         __syncthreads();                                       // the previous block is written out
         deflate::stage(S, in + off, n, tid, DEF_THREADS);
         __syncthreads();

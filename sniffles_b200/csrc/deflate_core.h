@@ -119,7 +119,8 @@ SNFB_HD void put_bits(Shared* S, uint32_t off, uint64_t v, uint32_t nbits) {
 // ---------------------------------------------------------------- phase 1: stage the block, clear the per-block state
 SNFB_HD void stage(Shared* S, const uint8_t* in, uint32_t n, int tid, int nt) {
 #if defined(__CUDA_ARCH__)
-    const uint32_t n16 = n >> 4;                               // `in` is 16-byte aligned (blocks start at multiples of 0xff00)
+    // 16-byte loads when `in` is 16-byte aligned (fixed cuts start at multiples of 0xff00); byte loads for a member cut anywhere
+    const uint32_t n16 = ((uintptr_t)in & 15u) ? 0u : n >> 4;
     for (uint32_t j = tid; j < n16; j += nt) reinterpret_cast<uint4*>(S->data)[j] = reinterpret_cast<const uint4*>(in)[j];
     for (uint32_t j = 16u * n16 + tid; j < n; j += nt) S->data[j] = in[j];
 #else
