@@ -108,7 +108,7 @@ struct snfb_ctx {
     const snfb_rec* d_rec = nullptr; const uint16_t* d_cigar = nullptr; const uint8_t* d_var = nullptr; const uint8_t* d_seq = nullptr;
     DevBuf b_rec, b_cigar, b_var, b_seq, b_task, b_contig, b_tr, b_trp, b_mask, b_mask_off, b_mask_task;
     HostBuf h_c16, h_rec16;        // BAM32 host input converted to CIGAR16 before the upload
-    DevBuf b_comp, b_raw, b_ing, b_ing_work; HostBuf h_ing; uint64_t ing_sizes[8] = {0, 0, 0, 0, 0, 0, 0, 0}; bool from_bam = false;      // device BAM ingest: BGZF bytes, inflated stream, block / span tables, per-raw-record work arrays
+    DevBuf b_comp, b_raw, b_ing, b_ing_span, b_ing_work; HostBuf h_ing; uint64_t ing_sizes[8] = {0, 0, 0, 0, 0, 0, 0, 0}; bool from_bam = false;      // device BAM ingest: BGZF bytes, inflated stream, counters / block table, span tables, per-raw-record work arrays
     DevBuf b_zin, b_zslot, b_zout, b_zwork;          // BGZF compression: input bytes, 64 KiB member slots, packed members, sizes / offsets / candidate scratch
     DevBuf b_gt;                                     // force calling: candidate bin keys, sort scratch, targets and their results
     DevBuf b_rn, b_rn_text; HostBuf h_rn_meta, h_rn_text;     // read names: per-name scratch and counters, the text; counters + offsets, text on the host
@@ -511,61 +511,116 @@ int snfb_load_records(snfb_ctx* ctx, const snfb_records* R) {
 
 
 // ---- device BAM ingest (SURVEY §8 (f)3) ----
-// BGZF block headers of a buffer of whole blocks (SAM spec §4.1): payload offset / length, inflated size, start of every block
-static int walk_bgzf(snfb_ctx* ctx, const uint8_t* z, uint64_t n, std::vector<ingest::BgzfBlock>& blocks, std::vector<uint64_t>& cstart, uint64_t* raw_len) {
-    uint64_t o = 0, uo = 0;
-    while (o < n) {
-        if (o + 18 > n || z[o] != 0x1f || z[o + 1] != 0x8b || z[o + 2] != 8 || !(z[o + 3] & 4)) return fail(ctx, "not a BGZF block (gzip member with an extra field expected)");
-        const uint32_t xlen = z[o + 10] | (z[o + 11] << 8);
-        if (o + 12 + xlen > n) return fail(ctx, "truncated BGZF header");
-        uint32_t bsize = 0; uint64_t e = o + 12; const uint64_t xend = o + 12 + xlen;
-        while (e + 4 <= xend) { const uint32_t slen = z[e + 2] | (z[e + 3] << 8); if (z[e] == 66 && z[e + 1] == 67 && slen == 2 && e + 6 <= xend) bsize = (z[e + 4] | (z[e + 5] << 8)) + 1u; e += 4 + slen; }
-        if (!bsize || bsize < 12 + xlen + 8 || o + bsize > n) return fail(ctx, "BGZF block without a BC field or truncated");
-        ingest::BgzfBlock b; b.in_off = o + 12 + xlen; b.in_len = bsize - 12 - xlen - 8;
-        memcpy(&b.crc, z + o + bsize - 8, 4); memcpy(&b.isize, z + o + bsize - 4, 4); b.out_off = uo; b._pad = 0;
-        if (b.isize > 65536u) return fail(ctx, "BGZF block claims more than 64 KiB of data");
-        blocks.push_back(b); cstart.push_back(o);
-        uo += b.isize; o += bsize;
-    }
-    *raw_len = uo; return 0;
+namespace {
+// device time: events around each phase of work the host hands the stream; the host's file reading between phases is not counted
+struct PhaseTimer {
+    cudaEvent_t a = nullptr, b = nullptr; double ms = 0;
+    PhaseTimer() { cudaEventCreate(&a); cudaEventCreate(&b); }
+    ~PhaseTimer() { cudaEventDestroy(a); cudaEventDestroy(b); }
+    void begin(cudaStream_t st) { cudaEventRecord(a, st); }
+    void end(cudaStream_t st) { cudaEventRecord(b, st); cudaEventSynchronize(b); float x = 0; cudaEventElapsedTime(&x, a, b); ms += x; }
+};
+// the BGZF member at z[o, n) (SAM spec §4.1): bad = 0 and its total size, XLEN, ISIZE and CRC32, or the first rule it breaks (BGZF_*);
+// cut: the rule could not be checked because z ends inside the member
+enum { BGZF_GZIP = 1, BGZF_XLEN, BGZF_BSIZE, BGZF_ISIZE };
+struct BgzfMember { int bad = 0; bool cut = false; uint32_t size = 0, xlen = 0, isize = 0, crc = 0; };
+BgzfMember bgzf_member(const uint8_t* z, uint64_t n, uint64_t o) {
+    BgzfMember m;
+    auto broken = [&](int rule, bool cut) { m.bad = rule; m.cut = cut; return m; };
+    if (o + 18 > n) return broken(BGZF_GZIP, true);
+    if (z[o] != 0x1f || z[o + 1] != 0x8b || z[o + 2] != 8 || !(z[o + 3] & 4)) return broken(BGZF_GZIP, false);      // gzip, DEFLATE, FEXTRA
+    m.xlen = z[o + 10] | (z[o + 11] << 8);
+    const uint64_t xend = o + 12 + m.xlen;
+    if (xend > n) return broken(BGZF_XLEN, true);
+    for (uint64_t e = o + 12; e + 4 <= xend; e += 4 + (z[e + 2] | (z[e + 3] << 8)))
+        if (z[e] == 66 && z[e + 1] == 67 && (z[e + 2] | (z[e + 3] << 8)) == 2 && e + 6 <= xend) m.size = (z[e + 4] | (z[e + 5] << 8)) + 1u;
+    if (!m.size || m.size < 12 + m.xlen + 8) return broken(BGZF_BSIZE, false);
+    if (o + m.size > n) return broken(BGZF_BSIZE, true);
+    memcpy(&m.crc, z + o + m.size - 8, 4); memcpy(&m.isize, z + o + m.size - 4, 4);
+    if (m.isize > 65536u) return broken(BGZF_ISIZE, false);
+    return m;
 }
-static int inflate_to_device(snfb_ctx* ctx, const uint8_t* z, uint64_t n, std::vector<uint64_t>& cstart, std::vector<ingest::BgzfBlock>& blocks, uint64_t* raw_len, const char* h2d_mark = "h2d_bgzf") {
-    if (walk_bgzf(ctx, z, n, blocks, cstart, raw_len)) return 1;
-    if (*raw_len >= (1ull << 36)) return fail(ctx, "more than 64 GiB of inflated BAM in one ingest call: split the task list");
-    if (ctx->b_comp.ensure(n + 64) || ctx->b_raw.ensure(*raw_len + 64)) return fail(ctx, "out of device memory for the BGZF bytes / the inflated stream");
-    mark(ctx, h2d_mark, n);
-    CUDA_TRY(cudaMemcpyAsync(ctx->b_comp.p, z, n, cudaMemcpyHostToDevice, ctx->st));
-    CUDA_TRY(cudaMemsetAsync(ctx->b_comp.as<uint8_t>() + n, 0, 64, ctx->st));
-    CUDA_TRY(cudaMemsetAsync(ctx->b_raw.as<uint8_t>() + *raw_len, 0, 64, ctx->st));
+// whole BGZF members at the start of a host buffer: their k_inflate table, each one's start in the buffer, their total size and inflated
+// size; d_ctr: the counters inflate_members launched k_inflate with
+struct BgzfMembers {
+    std::vector<ingest::BgzfBlock> blk; std::vector<uint64_t> cstart; uint64_t n = 0, raw_len = 0; ingest::IngestCounters* d_ctr = nullptr;
+    void add(const BgzfMember& m) {
+        blk.push_back(ingest::BgzfBlock{ n + 12 + m.xlen, m.size - 12 - m.xlen - 8, m.isize, raw_len, m.crc, 0 });
+        cstart.push_back(n); n += m.size; raw_len += m.isize;
+    }
+};
+}  // namespace
+
+// the members of z[0, n), which must be whole BGZF members
+static int walk_bgzf(snfb_ctx* ctx, const uint8_t* z, uint64_t n, BgzfMembers& w) {
+    static const char* const why[] = { "", "not a BGZF block (gzip member with an extra field expected)", "truncated BGZF header",
+                                       "BGZF block without a BC field or truncated", "BGZF block claims more than 64 KiB of data" };
+    while (w.n < n) {
+        const BgzfMember m = bgzf_member(z, n, w.n);
+        if (m.bad) return fail(ctx, why[m.bad]);
+        w.add(m);
+    }
+    if (w.raw_len >= (1ull << 36)) return fail(ctx, "more than 64 GiB of inflated BAM in one ingest call: split the task list");
     return 0;
 }
 
-// the error of a k_inflate launch with failed blocks: their count, and the lowest failing block with its byte offset in the caller's buffer
-static int inflate_failed(snfb_ctx* ctx, const ingest::IngestCounters& hc, const std::vector<uint64_t>& cstart) {
-    const unsigned long long first = ~hc.first_bad_inv, b = first >> 8, code = first & 255u;
-    return fail(ctx, "inflate: " + std::to_string(hc.bad_blocks) + " BGZF block(s) failed to decode (first: block " + std::to_string(b) + ", code " + std::to_string(code)
-                     + (code == ingest::INF_CRC_MISMATCH ? ", CRC32 mismatch" : "") + ", at byte " + std::to_string(cstart[b]) + " of the buffer)");
+// how one inflate_members call is timed and what it reports when a buffer cannot grow.  Timing opens once the buffers have grown: tm's
+// phase and `mark` (with mark_bytes) where the uploads start, launch_mark where k_inflate starts.
+struct InflateCall {
+    PhaseTimer* tm = nullptr; const char* mark = nullptr; uint64_t mark_bytes = 0; const char* launch_mark = nullptr;
+    std::string oom = "out of device memory for the BGZF bytes / the inflated stream", oom_tables = "out of device memory (ingest tables)";
+};
+// Enqueues on ctx->st, with no host synchronisation: the members z[0, w.n) to b_comp, their table (out_off added to every block's output
+// offset) and the zeroed counters w.d_ctr to b_ing, and k_inflate of them into b_raw[out_off, out_off + w.raw_len); both buffers get 64
+// zero bytes of pad.
+static int inflate_members(snfb_ctx* ctx, const uint8_t* z, BgzfMembers& w, uint64_t out_off, const InflateCall& call) {
+    const uint64_t raw_end = out_off + w.raw_len; const size_t nb = w.blk.size();
+    if (ctx->b_comp.ensure(w.n + 64) || ctx->b_raw.ensure(raw_end + 64)) return fail(ctx, call.oom);
+    ingest::BgzfBlock* d_blk = nullptr;
+    if (carve(ctx->b_ing, [&](Carver& c) { w.d_ctr = c.take<ingest::IngestCounters>(1); d_blk = c.take<ingest::BgzfBlock>(nb + 1); })) return fail(ctx, call.oom_tables);
+    cudaStream_t st = ctx->st;
+    if (call.tm) call.tm->begin(st);
+    if (call.mark) mark(ctx, call.mark, call.mark_bytes);
+    CUDA_TRY(cudaMemcpyAsync(ctx->b_comp.p, z, w.n, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemsetAsync(ctx->b_comp.as<uint8_t>() + w.n, 0, 64, st));
+    CUDA_TRY(cudaMemsetAsync(ctx->b_raw.as<uint8_t>() + raw_end, 0, 64, st));
+    CUDA_TRY(cudaMemsetAsync(w.d_ctr, 0, sizeof(ingest::IngestCounters), st));
+    std::vector<ingest::BgzfBlock> moved;
+    if (out_off) { moved = w.blk; for (auto& b : moved) b.out_off += out_off; }
+    CUDA_TRY(cudaMemcpyAsync(d_blk, (out_off ? moved : w.blk).data(), sizeof(ingest::BgzfBlock) * nb, cudaMemcpyHostToDevice, st));
+    if (call.launch_mark) mark(ctx, call.launch_mark, w.n + w.raw_len);
+    if (nb) launch_inflate(ctx, d_blk, (unsigned)nb, w.d_ctr);
+    return 0;
+}
+
+// the lowest failing block of a k_inflate launch and its INF_* code
+struct BadBlock { uint64_t block; unsigned code; bool crc() const { return code == ingest::INF_CRC_MISMATCH; } };
+static BadBlock first_bad(const ingest::IngestCounters& hc) { const unsigned long long f = ~hc.first_bad_inv; return BadBlock{ f >> 8, (unsigned)(f & 255u) }; }
+// the error of a k_inflate launch over a caller's buffer: the count of failed blocks, the lowest one and its byte in the buffer
+static int inflate_failed(snfb_ctx* ctx, const ingest::IngestCounters& hc, const BgzfMembers& w) {
+    const BadBlock x = first_bad(hc);
+    return fail(ctx, "inflate: " + std::to_string(hc.bad_blocks) + " BGZF block(s) failed to decode (first: block " + std::to_string(x.block) + ", code " + std::to_string(x.code)
+                     + (x.crc() ? ", CRC32 mismatch" : "") + ", at byte " + std::to_string(w.cstart[x.block]) + " of the buffer)");
+}
+// the error of a k_inflate launch over members read from file offset file_off: the lowest failing block's file offset
+static int inflate_failed_in_file(snfb_ctx* ctx, const ingest::IngestCounters& hc, const BgzfMembers& w, uint64_t file_off) {
+    const BadBlock x = first_bad(hc);
+    return fail(ctx, "BGZF block at file offset " + std::to_string(file_off + w.cstart[x.block]) + (x.crc() ? ": CRC32 mismatch" : ": failed to inflate (code " + std::to_string(x.code) + ")"));
 }
 
 int snfb_inflate_bgzf(snfb_ctx* ctx, const uint8_t* bgzf, uint64_t n_bytes, uint8_t* out, uint64_t out_cap, uint64_t* out_len) {
     if (!ctx || !bgzf || !out_len) return 1;
     cudaSetDevice(ctx->device);
-    std::vector<ingest::BgzfBlock> blocks; std::vector<uint64_t> cstart; uint64_t raw_len = 0;
     ctx->n_ev = 0;
-    if (inflate_to_device(ctx, bgzf, n_bytes, cstart, blocks, &raw_len)) return 1;
+    BgzfMembers w;
+    if (walk_bgzf(ctx, bgzf, n_bytes, w) || inflate_members(ctx, bgzf, w, 0, InflateCall{ nullptr, "h2d_bgzf", n_bytes, "inflate" })) return 1;
+    const uint64_t raw_len = w.raw_len;
     *out_len = raw_len;
-    const size_t nb = blocks.size();
-    ingest::IngestCounters* d_ctr = nullptr; ingest::BgzfBlock* d_blk = nullptr;
-    if (carve(ctx->b_ing, [&](Carver& c) { d_ctr = c.take<ingest::IngestCounters>(1); d_blk = c.take<ingest::BgzfBlock>(nb + 1); })) return fail(ctx, "out of device memory (ingest tables)");
-    CUDA_TRY(cudaMemsetAsync(d_ctr, 0, sizeof(ingest::IngestCounters), ctx->st));
-    CUDA_TRY(cudaMemcpyAsync(d_blk, blocks.data(), sizeof(ingest::BgzfBlock) * nb, cudaMemcpyHostToDevice, ctx->st));
-    mark(ctx, "inflate", n_bytes + raw_len);
-    if (nb) launch_inflate(ctx, d_blk, (unsigned)nb, d_ctr);
     mark(ctx, nullptr);
     ingest::IngestCounters hc;
-    CUDA_TRY(cudaMemcpyAsync(&hc, d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, ctx->st));
+    CUDA_TRY(cudaMemcpyAsync(&hc, w.d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, ctx->st));
     CUDA_TRY(cudaStreamSynchronize(ctx->st));
-    if (hc.bad_blocks) return inflate_failed(ctx, hc, cstart);
+    if (hc.bad_blocks) return inflate_failed(ctx, hc, w);
     if (out) {
         if (out_cap < raw_len) return fail(ctx, "snfb_inflate_bgzf: output buffer too small");
         CUDA_TRY(cudaMemcpy(out, ctx->b_raw.p, raw_len, cudaMemcpyDeviceToHost));
@@ -642,9 +697,10 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
     T.n_task = in->n_task; T.n_contig = in->n_contig; T.n_tr = in->n_tr; T.n_mask = in->n_mask; T.task = in->task; T.contig = in->contig; T.tr = in->tr; T.mask = in->mask; T.mask_task_off = in->mask_task_off;
     if (check_tables(ctx, &T)) return 1;
     ctx->n_ev = 0;
-    std::vector<ingest::BgzfBlock> blocks; std::vector<uint64_t> cstart; uint64_t raw_len = 0;
-    if (inflate_to_device(ctx, in->bgzf, in->n_bytes, cstart, blocks, &raw_len)) return 1;
-    const size_t nb = blocks.size(); const uint64_t ns = in->n_span;
+    BgzfMembers w;
+    if (walk_bgzf(ctx, in->bgzf, in->n_bytes, w)) return 1;
+    const size_t nb = w.blk.size(); const uint64_t ns = in->n_span, raw_len = w.raw_len;
+    mark(ctx, "h2d_bgzf", in->n_bytes);
     // spans: virtual offsets -> offsets in the inflated stream
     std::vector<ingest::Span> spans(ns);
     for (uint64_t i = 0; i < ns; ++i) {
@@ -652,9 +708,9 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
         if (sp.task >= in->n_task) return fail(ctx, "span: task index out of range");
         auto resolve = [&](uint64_t c, uint32_t u, uint64_t* out) -> bool {
             if (c == in->n_bytes) { *out = raw_len; return u == 0; }
-            auto it = std::lower_bound(cstart.begin(), cstart.end(), c);
-            if (it == cstart.end() || *it != c) return false;
-            const ingest::BgzfBlock& b = blocks[(size_t)(it - cstart.begin())];
+            auto it = std::lower_bound(w.cstart.begin(), w.cstart.end(), c);
+            if (it == w.cstart.end() || *it != c) return false;
+            const ingest::BgzfBlock& b = w.blk[(size_t)(it - w.cstart.begin())];
             if (u > b.isize) return false;
             *out = b.out_off + u; return true;
         };
@@ -669,17 +725,14 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
         spans[i].ubeg = ub; spans[i].uend = ue; spans[i].task = sp.task; spans[i].region = rg;
     }
     if (upload_tables(ctx, &T)) return 1;
-    // counters, block and span tables
-    ingest::IngestCounters* d_ctr = nullptr; ingest::BgzfBlock* d_blk = nullptr; ingest::Span* d_span = nullptr; uint32_t* span_cnt = nullptr; uint32_t* span_base = nullptr; uint32_t* scan_tmp0 = nullptr;
-    if (carve(ctx->b_ing, [&](Carver& c) { d_ctr = c.take<ingest::IngestCounters>(1); d_blk = c.take<ingest::BgzfBlock>(nb + 1); d_span = c.take<ingest::Span>(ns + 1); span_cnt = c.take<uint32_t>(ns + 1);
-                                           span_base = c.take<uint32_t>(ns + 1); scan_tmp0 = c.take<uint32_t>(prims::scan_tmp_elems(ns + 1) + 16); }))
+    ingest::Span* d_span = nullptr; uint32_t* span_cnt = nullptr; uint32_t* span_base = nullptr; uint32_t* scan_tmp0 = nullptr;
+    if (carve(ctx->b_ing_span, [&](Carver& c) { d_span = c.take<ingest::Span>(ns + 1); span_cnt = c.take<uint32_t>(ns + 1); span_base = c.take<uint32_t>(ns + 1);
+                                                scan_tmp0 = c.take<uint32_t>(prims::scan_tmp_elems(ns + 1) + 16); }))
         return fail(ctx, "out of device memory (ingest tables)");
-    cudaStream_t st = ctx->st; const uint8_t* raw = ctx->b_raw.as<uint8_t>();
-    CUDA_TRY(cudaMemsetAsync(d_ctr, 0, sizeof(ingest::IngestCounters), st));
-    CUDA_TRY(cudaMemcpyAsync(d_blk, blocks.data(), sizeof(ingest::BgzfBlock) * nb, cudaMemcpyHostToDevice, st));
+    cudaStream_t st = ctx->st;
     if (ns) CUDA_TRY(cudaMemcpyAsync(d_span, spans.data(), sizeof(ingest::Span) * ns, cudaMemcpyHostToDevice, st));
-    mark(ctx, "inflate", in->n_bytes + raw_len);
-    if (nb) launch_inflate(ctx, d_blk, (unsigned)nb, d_ctr);
+    if (inflate_members(ctx, in->bgzf, w, 0, InflateCall{ nullptr, nullptr, 0, "inflate" })) return 1;
+    ingest::IngestCounters* d_ctr = w.d_ctr; const uint8_t* raw = ctx->b_raw.as<uint8_t>();
     mark(ctx, "walk_records", 0);
     if (ns) {
         launch(ctx->launches, ingest::k_walk, (unsigned)((ns + 127) / 128), 128, 0, st, raw, raw_len, d_span, (unsigned)ns, 0, span_cnt, nullptr, nullptr, nullptr, 0, d_ctr);
@@ -689,7 +742,7 @@ int snfb_load_bam(snfb_ctx* ctx, const snfb_bam_input* in) {
     ingest::IngestCounters* hc = ctx->h_ing.as<ingest::IngestCounters>();
     CUDA_TRY(cudaMemcpyAsync(hc, d_ctr, sizeof(*hc), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
-    if (hc->bad_blocks) return inflate_failed(ctx, *hc, cstart);
+    if (hc->bad_blocks) return inflate_failed(ctx, *hc, w);
     if (hc->bad_chain) return fail(ctx, "BAM record chain broken in " + std::to_string(hc->bad_chain) + " span(s): a span does not start or end on a record boundary, or the data is truncated");
     const uint64_t n_raw = hc->n_raw;
     if (n_raw >= (1ull << 28)) return fail(ctx, "too many records in one block (2^28)");
@@ -1751,20 +1804,15 @@ int snfb_load_reference(snfb_ctx* ctx, const snfb_ref_input* in) {
     cudaStream_t st = ctx->st;
     uint64_t raw_len = 0;
     if (in->is_bgzf) {      // the ingest's inflate, CRC-checked; the raw stream lives in b_raw until the genome is built
-        std::vector<ingest::BgzfBlock> blocks; std::vector<uint64_t> cstart;
-        if (inflate_to_device(ctx, in->bytes, in->n_bytes, cstart, blocks, &raw_len, "h2d_ref")) return 1;
-        const size_t nb = blocks.size();
-        ingest::IngestCounters* d_ctr = nullptr; ingest::BgzfBlock* d_blk = nullptr;
-        if (carve(ctx->b_ref_work, [&](Carver& c) { d_ctr = c.take<ingest::IngestCounters>(1); d_blk = c.take<ingest::BgzfBlock>(nb + 1); })) return fail(ctx, "out of device memory (reference inflate tables)");
-        CUDA_TRY(cudaMemsetAsync(d_ctr, 0, sizeof(ingest::IngestCounters), st));
-        CUDA_TRY(cudaMemcpyAsync(d_blk, blocks.data(), sizeof(ingest::BgzfBlock) * nb, cudaMemcpyHostToDevice, st));
-        mark(ctx, "inflate", in->n_bytes + raw_len);
-        if (nb) launch_inflate(ctx, d_blk, (unsigned)nb, d_ctr);
+        BgzfMembers w; InflateCall call{ nullptr, "h2d_ref", in->n_bytes, "inflate" };
+        call.oom_tables = "out of device memory (reference inflate tables)";
+        if (walk_bgzf(ctx, in->bytes, in->n_bytes, w) || inflate_members(ctx, in->bytes, w, 0, call)) return 1;
+        raw_len = w.raw_len;
         mark(ctx, nullptr);
         ingest::IngestCounters hc;
-        CUDA_TRY(cudaMemcpyAsync(&hc, d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(&hc, w.d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
-        if (hc.bad_blocks) { ctx->b_raw.reset(); ctx->b_comp.reset(); inflate_failed(ctx, hc, cstart); ctx->err = "reference " + ctx->err; return 1; }
+        if (hc.bad_blocks) { ctx->b_raw.reset(); ctx->b_comp.reset(); inflate_failed(ctx, hc, w); ctx->err = "reference " + ctx->err; return 1; }
         ctx->b_comp.reset();
     } else {
         raw_len = in->n_bytes;
@@ -1890,20 +1938,6 @@ uint64_t ix_voff(const IxWin& w, uint64_t u) {
     return (j + 1 < w.end.size() ? w.coff[j + 1] : w.coff_end) << 16;
 }
 std::string voff_str(uint64_t v) { return std::to_string(v >> 16) + ":" + std::to_string(v & 0xffff); }
-// the BGZF member at z[o..n): 0 and its total size / ISIZE; 1 when z ends inside it; 2 when it is not a BGZF member (SAM spec §4.1)
-int ix_member(const uint8_t* z, uint64_t n, uint64_t o, uint32_t* bsize, uint32_t* isize) {
-    if (o + 18 > n) return 1;
-    if (z[o] != 0x1f || z[o + 1] != 0x8b || z[o + 2] != 8 || !(z[o + 3] & 4)) return 2;
-    const uint32_t xlen = z[o + 10] | (z[o + 11] << 8);
-    if (o + 12 + xlen > n) return 1;
-    uint32_t bs = 0;
-    for (uint64_t e = o + 12; e + 4 <= o + 12 + xlen; e += 4 + (z[e + 2] | (z[e + 3] << 8)))
-        if (z[e] == 66 && z[e + 1] == 67 && (z[e + 2] | (z[e + 3] << 8)) == 2 && e + 6 <= o + 12 + xlen) bs = (z[e + 4] | (z[e + 5] << 8)) + 1u;
-    if (!bs || bs < 12 + xlen + 8) return 2;
-    if (o + bs > n) return 1;
-    memcpy(isize, z + o + bs - 4, 4); *bsize = bs;
-    return *isize > 65536u ? 2 : 0;
-}
 }  // namespace
 
 // the name of the record at R[p] of the window on the device
@@ -1915,14 +1949,6 @@ static std::string ix_name(const uint8_t* d_raw, uint64_t p) {
 }
 
 namespace {
-// device time: events around each phase of work the host hands the stream; the host's file reading between phases is not counted
-struct PhaseTimer {
-    cudaEvent_t a = nullptr, b = nullptr; double ms = 0;
-    PhaseTimer() { cudaEventCreate(&a); cudaEventCreate(&b); }
-    ~PhaseTimer() { cudaEventDestroy(a); cudaEventDestroy(b); }
-    void begin(cudaStream_t st) { cudaEventRecord(a, st); }
-    void end(cudaStream_t st) { cudaEventRecord(b, st); cudaEventSynchronize(b); float x = 0; cudaEventElapsedTime(&x, a, b); ms += x; }
-};
 // one window of the record chain, as stream_windows hands it over: the inflated bytes R[0, L) at global offset base (the carried bytes, then
 // the window's members from global offset G), the candidates cand[0, n) of which is_rec marks the n_rows complete chain records (rec_idx:
 // their index in the window, in file order); open: the chain ends in a record the window cannot finish (it is carried into the next one);
@@ -1964,25 +1990,22 @@ template <class OnWindow> static int stream_windows(snfb_ctx* ctx, const char* w
     for (;;) {
         fill(std::max<uint64_t>(win, 1 << 17) + 65536 + 64);
         if (hb.empty()) break;
-        uint64_t sel = 0, isum = 0; uint32_t nsel = 0;
-        for (;;) {
-            uint32_t bs = 0, isz = 0;
-            if (sel == hb.size()) break;
-            const int rc = ix_member(hb.data(), hb.size(), sel, &bs, &isz);
-            if (rc == 2) return fail(ctx, "not a BGZF block at file offset " + std::to_string(hb_off + sel) + ": not a BGZF-compressed BAM file");
-            if (rc == 1) {
-                if (eof) return fail(ctx, "truncated BGZF block at file offset " + std::to_string(hb_off + sel) + ": the file is truncated");
-                if (nsel) break;
+        BgzfMembers M;                                                         // the window's members: hb[0, M.n)
+        while (M.n < hb.size()) {
+            const BgzfMember m = bgzf_member(hb.data(), hb.size(), M.n);
+            if (m.bad && !m.cut) return fail(ctx, "not a BGZF block at file offset " + std::to_string(hb_off + M.n) + ": not a BGZF-compressed BAM file");
+            if (m.cut) {
+                if (eof) return fail(ctx, "truncated BGZF block at file offset " + std::to_string(hb_off + M.n) + ": the file is truncated");
+                if (M.blk.size()) break;
                 fill(hb.size() + (1 << 17));
                 continue;
             }
-            if (nsel && isum + isz > win) break;
-            sel += bs; isum += isz; ++nsel;
+            if (M.blk.size() && M.raw_len + m.isize > win) break;
+            M.add(m);
         }
-        std::vector<ingest::BgzfBlock> blocks; std::vector<uint64_t> cstart; uint64_t raw_len = 0;
-        if (walk_bgzf(ctx, hb.data(), sel, blocks, cstart, &raw_len)) return 1;
+        const uint64_t sel = M.n, raw_len = M.raw_len;
         IxWin W; W.first_beg = G; W.coff_end = hb_off + sel;
-        for (size_t k = 0; k < blocks.size(); ++k) { W.end.push_back(G + blocks[k].out_off + blocks[k].isize); W.coff.push_back(hb_off + cstart[k]); }
+        for (size_t k = 0; k < M.blk.size(); ++k) { W.end.push_back(G + M.blk[k].out_off + M.blk[k].isize); W.coff.push_back(hb_off + M.cstart[k]); }
         if (!entry_known) {                                                    // the header's end, as a global inflated offset
             const uint64_t c = first_record >> 16, u = first_record & 0xffff;
             auto it = std::find(W.coff.begin(), W.coff.end(), c);
@@ -1990,28 +2013,14 @@ template <class OnWindow> static int stream_windows(snfb_ctx* ctx, const char* w
         }
         const uint64_t base = G - carry, L = carry + raw_len, G_win = G, coff_beg = hb_off;
         // inflate and CRC-check the window behind the carried bytes
-        if (ctx->b_comp.ensure(sel + 64) || ctx->b_raw.ensure(L + 64)) return fail(ctx, oom + " for the window");
-        for (auto& b : blocks) b.out_off += carry;
+        if (inflate_members(ctx, hb.data(), M, carry, InflateCall{ &tm, nullptr, 0, nullptr, oom + " for the window", oom + " (ingest tables)" })) return 1;
         uint8_t* R = ctx->b_raw.as<uint8_t>();
-        ingest::IngestCounters* d_ctr = nullptr; ingest::BgzfBlock* d_blk = nullptr;
-        if (carve(ctx->b_ing, [&](Carver& c) { d_ctr = c.take<ingest::IngestCounters>(1); d_blk = c.take<ingest::BgzfBlock>(blocks.size() + 1); }))
-            return fail(ctx, oom + " (ingest tables)");
-        tm.begin(st);
         if (carry) CUDA_TRY(cudaMemcpyAsync(R, ctx->b_ix_carry.p, carry, cudaMemcpyDeviceToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(ctx->b_comp.p, hb.data(), sel, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemsetAsync(ctx->b_comp.as<uint8_t>() + sel, 0, 64, st));
-        CUDA_TRY(cudaMemsetAsync(R + L, 0, 64, st));
-        CUDA_TRY(cudaMemsetAsync(d_ctr, 0, sizeof(ingest::IngestCounters), st));
-        CUDA_TRY(cudaMemcpyAsync(d_blk, blocks.data(), sizeof(ingest::BgzfBlock) * blocks.size(), cudaMemcpyHostToDevice, st));
-        launch_inflate(ctx, d_blk, (unsigned)blocks.size(), d_ctr);
         ingest::IngestCounters hc;
-        CUDA_TRY(cudaMemcpyAsync(&hc, d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(&hc, M.d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, st));
         tm.end(st);
         CUDA_TRY(cudaStreamSynchronize(st));
-        if (hc.bad_blocks) {
-            const unsigned long long first = ~hc.first_bad_inv, b = first >> 8, code = first & 255u;
-            return fail(ctx, "BGZF block at file offset " + std::to_string(hb_off + cstart[b]) + (code == ingest::INF_CRC_MISMATCH ? ": CRC32 mismatch" : ": failed to inflate (code " + std::to_string(code) + ")"));
-        }
+        if (hc.bad_blocks) return inflate_failed_in_file(ctx, hc, M, hb_off);
         hb.erase(hb.begin(), hb.begin() + (ptrdiff_t)sel); hb_off += sel;
         G += raw_len; ++n_windows;
         if (!entry_known || u_entry >= base + L) continue;                   // still inside the header
@@ -2396,32 +2405,20 @@ extern "C" int snfb_sort_bam(snfb_ctx* ctx, const snfb_sort_input* in, snfb_sort
             hz.resize(nz);
             if (fseeko(fi, (off_t)W.coff_beg, SEEK_SET) != 0 || fread(hz.data(), 1, nz, fi) != nz)
                 return fail(ctx, "cannot read the input again at file offset " + std::to_string(W.coff_beg) + ": the file changed while it was sorted");
-            std::vector<ingest::BgzfBlock> blocks; std::vector<uint64_t> cstart; uint64_t raw_len = 0;
-            if (walk_bgzf(ctx, hz.data(), nz, blocks, cstart, &raw_len)) return 1;
+            BgzfMembers M;
+            if (walk_bgzf(ctx, hz.data(), nz, M)) return 1;
+            const uint64_t raw_len = M.raw_len;
             if (raw_len != W.raw_len) return fail(ctx, "the input changed while it was sorted (window at file offset " + std::to_string(W.coff_beg) + ")");
-            if (ctx->b_comp.ensure(nz + 64) || ctx->b_raw.ensure(raw_len + 64)) return fail(ctx, "snfb_sort_bam: out of device memory for the window");
-            ingest::IngestCounters* d_ctr = nullptr; ingest::BgzfBlock* d_blk = nullptr;
-            if (carve(ctx->b_ing, [&](Carver& c) { d_ctr = c.take<ingest::IngestCounters>(1); d_blk = c.take<ingest::BgzfBlock>(blocks.size() + 1); }))
-                return fail(ctx, "snfb_sort_bam: out of device memory (ingest tables)");
-            t_scatter.begin(st);
-            mark(ctx, "sort_scatter", raw_len);
-            CUDA_TRY(cudaMemcpyAsync(ctx->b_comp.p, hz.data(), nz, cudaMemcpyHostToDevice, st));
-            CUDA_TRY(cudaMemsetAsync(ctx->b_comp.as<uint8_t>() + nz, 0, 64, st));
-            CUDA_TRY(cudaMemsetAsync(ctx->b_raw.as<uint8_t>() + raw_len, 0, 64, st));
-            CUDA_TRY(cudaMemsetAsync(d_ctr, 0, sizeof(ingest::IngestCounters), st));
-            CUDA_TRY(cudaMemcpyAsync(d_blk, blocks.data(), sizeof(ingest::BgzfBlock) * blocks.size(), cudaMemcpyHostToDevice, st));
-            launch_inflate(ctx, d_blk, (unsigned)blocks.size(), d_ctr);
+            if (inflate_members(ctx, hz.data(), M, 0, InflateCall{ &t_scatter, "sort_scatter", raw_len, nullptr, "snfb_sort_bam: out of device memory for the window",
+                                                                   "snfb_sort_bam: out of device memory (ingest tables)" })) return 1;
             if (W.o1 > W.o0)
                 launch(ctx->launches, bamsort::k_scatter, grid_for((W.o1 - W.o0) * 32, 256), 256, 0, st, (const uint8_t*)ctx->b_raw.p, (unsigned long long)W.G, (unsigned long long)raw_len,
                        (uint32_t)W.o0, (uint32_t)W.o1, (const unsigned long long*)src, (const uint32_t*)len, (const unsigned long long*)dest, (unsigned long long)O0, (unsigned long long)O1, B);
             ingest::IngestCounters hc;
-            CUDA_TRY(cudaMemcpyAsync(&hc, d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(&hc, M.d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, st));
             t_scatter.end(st);
             mark(ctx, nullptr);
-            if (hc.bad_blocks) {
-                const unsigned long long first = ~hc.first_bad_inv, b = first >> 8, code = first & 255u;
-                return fail(ctx, "BGZF block at file offset " + std::to_string(W.coff_beg + cstart[b]) + (code == ingest::INF_CRC_MISMATCH ? ": CRC32 mismatch" : ": failed to inflate (code " + std::to_string(code) + ")"));
-            }
+            if (hc.bad_blocks) return inflate_failed_in_file(ctx, hc, M, W.coff_beg);
             ++reads; bytes_in += nz;
         }
         // the bucket's members, at most 65535 per launch
